@@ -1,6 +1,6 @@
-# Builds libpaimon_gpu.so (sm_100a only) in-tree, and the parity oracle.
+# Builds libpaimon_gpu.so (sm_90a only) in-tree, and the parity oracle.
 NVCC ?= /usr/local/cuda/bin/nvcc
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Iinclude -Ipaimon_b200/csrc
 SRCS := paimon_b200/csrc/merge.cu paimon_b200/csrc/emit.cu paimon_b200/csrc/api.cu \
 	paimon_b200/csrc/parquet_decode.cu paimon_b200/csrc/parquet_encode.cu paimon_b200/csrc/parquet_meta.cc \
@@ -16,7 +16,8 @@ all: $(LIB) oracle
 OBJDIR ?= build
 OBJS := $(patsubst paimon_b200/csrc/%,$(OBJDIR)/%.o,$(SRCS))
 
-$(OBJDIR)/%.o: paimon_b200/csrc/% $(HDRS)
+# the Makefile is a prerequisite too: a change of ARCH or flags rebuilds every object
+$(OBJDIR)/%.o: paimon_b200/csrc/% $(HDRS) Makefile
 	@mkdir -p $(OBJDIR)
 	$(NVCC) $(NVFLAGS) $(EXTRA_DEFS) -x cu -c -o $@ $<
 

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — merged rows/s of the LSM merge hot path on B200 (BASELINE.json metric).
+"""bench.py — merged rows/s of the LSM merge hot path on H100 (BASELINE.json metric).
 
 One "step" = one pass of the hot path over one bucket of synthetic sorted runs:
   --source parquet (default for c3):  Parquet file bytes in HBM -> column-chunk decode (one launch set for the
@@ -9,7 +9,8 @@ One "step" = one pass of the hot path over one bucket of synthetic sorted runs:
       c3 under "extra" as well).
 
 Workloads (BASELINE.json configs, SURVEY.md §8d):
-  c3 (default, the configuration the metric is quoted on): 16 runs x 6.25 M rows = 100 M rows, partial-update merge
+  c3 (default, the configuration the metric is quoted on): 16 runs x 2.5 M rows = 40 M rows (sized so that the files,
+      the decoded runs and the two merged batches of the pipelined e2e leg fit one 80 GB H100), partial-update merge
       engine, 50-column wide row (pk + 20 BIGINT + 15 DOUBLE + 14 VARCHAR(8..24)), every non-pk cell NULL with p = 0.5
   c3agg: same rows, merge-engine aggregation (sum over the numeric columns: ordered left fold, bit-exact)
   c2: 8 runs x 12.5 M rows = 100 M rows, deduplicate, BIGINT pk + 10 BIGINT columns
@@ -18,6 +19,7 @@ Workloads (BASELINE.json configs, SURVEY.md §8d):
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--workload c3|c3agg|c2|c1|c4] [--rows R] [--source ...]
     python bench.py --impl reference ...     # the reference algorithm on the host cores (CPU)
+    python bench.py --dump-outputs DIR ...   # also write a seeded sample of the last timed step's merged batch
 
 `value`     whole-job merged (= input) rows/s with the inputs (file bytes / columns) already resident in HBM.
 `e2e`       same metric through the public reader API with HOST buffers: every step copies the Parquet files
@@ -45,19 +47,19 @@ import time
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
-# decoded runs (48 GB per step on c3) are recycled through the library's buffer cache instead of the driver allocator
-os.environ.setdefault("PG_RUN_CACHE_BYTES", str(150 << 30))
+# decoded runs (19 GB per step on c3) are recycled through the library's buffer cache instead of the driver allocator
+os.environ.setdefault("PG_RUN_CACHE_BYTES", str(64 << 30))
 
 import numpy as np  # noqa: E402
 
 WORKLOADS = {
-    "c3": dict(n_runs=16, rows=100_000_000, engine="partial-update", null_prob=0.5,
-               desc="16-run partial-update, 50-col wide row (pk+20 i64+15 f64+14 varchar), 100M rows"),
+    "c3": dict(n_runs=16, rows=40_000_000, engine="partial-update", null_prob=0.5,
+               desc="16-run partial-update, 50-col wide row (pk+20 i64+15 f64+14 varchar), 40M rows"),
     # SURVEY §8d "C3-agg": same rows as C3, merge-engine aggregation: the 15 doubles and 20 bigints use `sum`
     # (ordered left fold, bit-exact), the strings last_non_null_value
-    "c3agg": dict(n_runs=16, rows=100_000_000, engine="aggregate", null_prob=0.5,
+    "c3agg": dict(n_runs=16, rows=40_000_000, engine="aggregate", null_prob=0.5,
                   desc="16-run aggregation (sum over 20 i64 + 15 f64, last_non_null_value over 14 varchar), 50-col wide "
-                       "row, 100M rows"),
+                       "row, 40M rows"),
     "c2": dict(n_runs=8, rows=100_000_000, engine="deduplicate", null_prob=0.0,
                desc="8-run deduplicate, int64 pk + 10 int64 cols, 100M rows"),
     "c1": dict(n_runs=2, rows=1_000_000, engine="deduplicate", null_prob=0.0,
@@ -497,8 +499,8 @@ def load_peak():
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    return peak, ("measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback 6.65 TB/s")
+    peak = float(peaks.get("hbm_gbs", 3350.0))
+    return peak, ("measured (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback 3.35 TB/s (H100 SXM data sheet)")
 
 
 def expected_rows(w, all_keys, all_kinds):
@@ -555,6 +557,49 @@ def parity_sample(schema, spec, rd, run_handles, all_keys, n_out, target_rows=30
                        "bit-exact against the oracle's merge of the same input rows"}
 
 
+def dump_outputs(out_dir, schema, merge_h, n_out, block_rows=256, max_blocks=64, seed=0):
+    """Write what the timed path handed its caller in the last step — the merged batch — as .npy files, so that two
+    builds can be compared output for output.  The batch is far larger than a dump should be, so a fixed, seeded set of
+    row blocks is taken (at most max_blocks * block_rows rows, ~25 MB for c3).  Per column `<name>`:
+      fixed width: <name>.npy float64 (INT64 as [high signed 32 bits, low 32 bits] pairs, exact), FLOAT float32;
+      var-len:     <name>.len.npy float64 byte lengths, <name>.bytes.npy float32 the concatenated bytes;
+      nullable:    <name>.valid.npy float32 0/1 (NULL cells dump value 0 / length 0).
+    row_index.npy holds the sampled row positions and n_rows.npy the batch's row count."""
+    from paimon_b200.columnar import unpack_validity
+    from paimon_b200.merge_tree_readers import concat_batches
+    from paimon_b200.sort_merge_reader import fetch_slice
+    from paimon_b200.types import PhysicalType, is_varlen
+    os.makedirs(out_dir, exist_ok=True)
+    n_blocks = min(max_blocks, (n_out + block_rows - 1) // block_rows)
+    starts = np.sort(np.random.default_rng(seed).choice((n_out + block_rows - 1) // block_rows, n_blocks,
+                                                        replace=False)) * block_rows
+    spans = [(int(s), int(min(s + block_rows, n_out))) for s in starts]
+    batch = concat_batches(schema, [fetch_slice(schema, merge_h, lo, hi) for lo, hi in spans])
+    n = batch.n_rows
+    out = {"n_rows": np.array([n_out], np.float64),
+           "row_index": np.concatenate([np.arange(lo, hi) for lo, hi in spans]).astype(np.float64)}
+    for f, col in zip(schema.file_fields(), batch.columns):
+        valid = unpack_validity(col.valid, n)
+        if col.valid is not None:
+            out[f"{f.name}.valid"] = valid.astype(np.float32)
+        if is_varlen(f.physical):
+            offs = np.asarray(col.offsets[:n + 1], np.int64)
+            out[f"{f.name}.len"] = np.where(valid, np.diff(offs), 0).astype(np.float64)
+            keep = np.repeat(valid, np.diff(offs))
+            out[f"{f.name}.bytes"] = np.asarray(col.data[offs[0]:offs[-1]], np.uint8)[keep].astype(np.float32)
+        elif f.physical == PhysicalType.FLOAT:
+            out[f.name] = np.where(valid, np.asarray(col.data[:n], np.float32), 0).astype(np.float32)
+        elif f.physical == PhysicalType.INT64:
+            v = np.where(valid, np.asarray(col.data[:n], np.int64), 0)
+            out[f.name] = np.stack([(v >> 32).astype(np.float64), (v & 0xFFFFFFFF).astype(np.float64)], axis=1)
+        else:
+            out[f.name] = np.where(valid, np.asarray(col.data[:n]).astype(np.float64), 0.0)
+    assert sum(a.nbytes for a in out.values()) <= 64 << 20
+    for name, arr in out.items():
+        np.save(os.path.join(out_dir, name + ".npy"), arr)
+    return {"dir": out_dir, "rows": int(n), "files": len(out)}
+
+
 # ------------------------------------------------------------------ main
 
 def main():
@@ -579,7 +624,11 @@ def main():
     ap.add_argument("--no-parity-sample", action="store_true")
     ap.add_argument("--cpu-sample-rows", type=int, default=None)
     ap.add_argument("--cpu-threads", type=int, default=None)
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write a seeded sample of the last timed step's merged batch to DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
 
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -587,7 +636,7 @@ def main():
     w = WORKLOADS[args.workload]
     rows = args.rows or w["rows"]
     source = args.source or ("parquet" if args.workload == "c3" else "columns")
-    metric = "merged rows/sec at 16 runs x 100M rows" if args.workload == "c3" else f"merged rows/sec ({args.workload})"
+    metric = "merged rows/sec at 16 runs x 40M rows" if args.workload == "c3" else f"merged rows/sec ({args.workload})"
     threads = args.cpu_threads or min(os.cpu_count() or 1, 64)
     cpu_sample = min(args.cpu_sample_rows or threads * (250_000 if args.workload in ("c3", "c3agg") else 1_000_000), rows)
     config = {"workload": f"{args.workload}: {w['desc']}", "rows_per_gpu": rows, "n_runs": w["n_runs"],
@@ -598,7 +647,7 @@ def main():
               if source == "parquet" else "columns: decoded columns resident in HBM, merge only",
               "reference_arm_sample": f"the CPU arm merges a {cpu_sample}-row sample of this shape ({threads} buckets, one "
                                       "thread each) from decoded columns, no Parquet decode",
-              "l2": "inputs (>30 GB) far exceed the 126 MB L2; no explicit flush" if rows >= 10_000_000
+              "l2": "inputs (>10 GB) far exceed the 50 MB L2; no explicit flush" if rows >= 10_000_000
                     else "small input: L2-resident (not a headline configuration)"}
 
     # ---------------- reference arm: the reference's CPU algorithm on the host cores
@@ -621,7 +670,7 @@ def main():
         print(json.dumps(line))
         return
 
-    # ---------------- B200 arm
+    # ---------------- device arm
     numa = bind_to_gpu_numa_node(local_rank)
     import torch
     import torch.distributed as dist
@@ -703,14 +752,7 @@ def main():
         dev_ms = e0.elapsed_time(e1)
         dec_ms = ms_dec / args.steps
         dec_alg = page_bytes + in_bytes
-        dec_traffic = None
-        try:
-            tjd = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-            if args.workload == "c3" and rows == w["rows"]:
-                dec_traffic = tjd["c3_decode"]["traffic"]
-        except Exception:
-            pass
-        roofline_decode = {"bound": "hbm", "stage": "parquet decode (page walk + levels + value walk + expand)", "traffic": dec_traffic,
+        roofline_decode = {"bound": "hbm", "stage": "parquet decode (page walk + levels + value walk + expand)",
                            "achieved": dec_alg / (dec_ms * 1e-3) / 1e9, "peak": peak, "unit": "GB/s",
                            "frac": dec_alg / (dec_ms * 1e-3) / 1e9 / peak, "stage_ms": dec_ms,
                            "algorithmic_bytes": int(dec_alg), "encoded_page_bytes": int(page_bytes),
@@ -748,6 +790,10 @@ def main():
         clocks = sampler.stop()
         dev_ms = e0.elapsed_time(e1)
 
+    dumped = None
+    if args.dump_outputs and rank == 0:
+        dumped = dump_outputs(args.dump_outputs, schema, rd._merge_h, n_out)
+
     t = torch.tensor([dev_ms], device=dev, dtype=torch.float64)
     if world > 1:
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
@@ -756,18 +802,9 @@ def main():
 
     alg_bytes = in_bytes + out_bytes
     emit_ms = ms_emit / args.steps
-    # DRAM traffic of the dominant kernel from the committed ncu capture of this workload at its full size
-    # (profiles/traffic.json; only meaningful for the default row count)
-    traffic = None
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-        if args.workload in tj and rows == w["rows"]:
-            traffic = tj[args.workload]["traffic"]
-    except Exception:
-        pass
     achieved = alg_bytes / (emit_ms * 1e-3) / 1e9
     roofline = {"bound": "hbm", "kernel": "k_emit", "achieved": achieved, "peak": peak, "unit": "GB/s",
-                "frac": achieved / peak, "peak_source": peak_kind, "traffic": traffic,
+                "frac": achieved / peak, "peak_source": peak_kind,
                 "algorithmic_bytes": int(alg_bytes), "kernel_ms": emit_ms,
                 "step_frac": alg_bytes / (step_ms * 1e-3) / 1e9 / peak,
                 "phase_ms": {"decode": (ms_dec / args.steps) if source == "parquet" else None,
@@ -1226,6 +1263,8 @@ def main():
             line["parity_sample_detail"] = parity
         if rewrite is not None:
             line["rewrite"] = rewrite
+        if dumped is not None:
+            line["dump_outputs"] = dumped
         if extra:
             line["extra"] = extra
         print(json.dumps(line))

@@ -1,5 +1,5 @@
 /*
- * paimon_gpu.h — C ABI of libpaimon_gpu.so, the B200 (sm_100a) implementation of Apache
+ * paimon_gpu.h — C ABI of libpaimon_gpu.so, the H100 (sm_90a) implementation of Apache
  * Paimon's merge-on-read / compaction hot path:
  *
  *     sorted-run columnar batches -> k-way merge by (key, sequence) -> per-key MergeFunction

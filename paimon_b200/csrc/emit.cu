@@ -15,11 +15,11 @@
 // Round 2 measured four restructurings of this kernel against it on the same box (profiles/experiments/README.md):
 // a size pass + copy pass per var-len column with full / empty mbarriers instead of block barriers, a ballot-based
 // bitmap select, a single-winner path for deduplicate, deeper payload gathers and an L2 prefetch of the payload.  All
-// lost (C3 50-60 ms vs 45.5 ms).  What did help: pointers to the staged data are computed from the shared-memory
-// symbol at every use (picked out of a local array they became generic loads through L1TEX: -5 %), global stores /
+// lost on C3.  What did help: pointers to the staged data are computed from the shared-memory
+// symbol at every use (picked out of a local array they became generic loads through L1TEX), global stores /
 // loads are marked global, the tile prologue loads its run bounds with one lane per run, and the pass descriptors
 // (column, ColDesc, output buffers) are staged in shared memory once per tile instead of being read from the device
-// tables at the top of every pass (two dependent global round trips in front of all 16 warps: C3 -4 %, C2 -6 %).
+// tables at the top of every pass (two dependent global round trips in front of all 16 warps).
 #include <stdio.h>
 
 #include "device_utils.cuh"

@@ -1,4 +1,4 @@
-// merge.cu — sm_100a kernels of the k-way merge + per-key-group reduce.
+// merge.cu — sm_90a kernels of the k-way merge + per-key-group reduce.
 //
 // Replaces the per-record loop of SortMergeReaderWithLoserTree.SortMergeIterator.next()
 // (reference: paimon-core/.../mergetree/compact/SortMergeReaderWithLoserTree.java:87-112,

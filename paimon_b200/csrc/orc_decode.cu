@@ -374,7 +374,7 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
     const size_t tb_s = pad(sizeof(OrcStream) * (size_t)std::max(n_streams, 1)), tb_t = pad(sizeof(orcdev::Task) * (size_t)std::max(n_tasks, 1));
     const size_t tb_r = pad(sizeof(OrcTaskRef) * (size_t)std::max(n_tasks, 1)), tb_o = pad(4 * (size_t)std::max(n_tasks, 1));
     const size_t tb_p = pad(sizeof(void *) * outs.size());
-    int sms = 148, dev = 0;
+    int sms = 132, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int inflate_ctas = !any_compressed ? std::max(1, std::min(sms, (n_streams + kOrcWarps - 1) / kOrcWarps))

@@ -830,11 +830,10 @@ k_pq_walk_dicts(const PqPage *dicts, int n_dicts, const PqChunk *chunks, int32_t
 // PLAIN BYTE_ARRAY data pages -> value start offsets in the OUTPUT payload (vstart[vs_base + j], j <= nnz).
 // The walk of one page is a dependent chain (every length word says where the next one is), so a page cannot be
 // split; a section has tens of thousands of such pages, though, so every LANE walks its own page: 32 independent
-// chains per warp instead of one lane working while 31 idle (the warp-per-page version spent ~38 issue slots per
-// value and was issue-bound: 24 ms per 700 M values).  Pages of a column chunk are neighbours in the page table, so the
+// chains per warp instead of one lane working while 31 idle (the warp-per-page version was issue-bound).  Pages of a column chunk are neighbours in the page table, so the
 // lanes of a warp walk streams of similar length.
 // Reading the length words straight from global memory makes every lane miss a 32-byte sector on nearly every value
-// (23 ms again: 32 scattered sector fetches per warp step, one round trip each), so the warp works in ROUNDS: it
+// (32 scattered sector fetches per warp step, one round trip each), so the warp works in ROUNDS: it
 // loads the next kWvWin bytes of all 32 streams into shared memory with coalesced 16-byte loads (16 lanes per stream,
 // 8 KiB in flight per warp), then every lane walks the values whose length word lies inside its window at
 // shared-memory latency.  Rows of the window buffer are XOR-swizzled per 16-byte chunk (lanes walk their rows at
@@ -1162,8 +1161,8 @@ k_pq_expand(const PqPage *pages, const PqPage *dicts, const PqChunk *chunks, con
             // kExpThreads values: the batch's stretch of the stream comes into shared memory with 16-byte async copies
             // (the NEXT batch is in flight while this one is worked on), every thread moves ONE value byte by byte
             // inside shared memory (all 32 lanes busy, no global latency), and the batch's contiguous output range
-            // leaves with 16-byte stores.  (8 lanes per value straight on global memory spent ~14 warp instructions
-            // per value and stalled on the gathers: 40 % of this kernel.)  Batches that do not fit the staging buffers
+            // leaves with 16-byte stores.  (8 lanes per value straight on global memory spent many warp
+            // instructions per value and stalled on the gathers.)  Batches that do not fit the staging buffers
             // (long values) and pages with more batches than the boundary table holds take the direct path.
             const int nnz = pg.nnz;
             const int64_t pb = pg.payload_base;
@@ -1652,7 +1651,7 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     const size_t sb_vs = pad(4 * (size_t)(pair_rows + n_pages + n_pairs + 2));
     int zs_ctas = 0;
     if (any_zstd) {
-        int dev = 0, sms = 148;
+        int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         zs_ctas = (int)std::min<int64_t>((int64_t)sms * 5, (n_pages + n_dicts + kZsWarps - 1) / kZsWarps);

@@ -2,7 +2,7 @@
 //
 // A decode + merge step has a handful of tiny read-backs (page counts, exact payload sizes, the output row count,
 // error words, Parquet footers of device-resident files).  Issued as cudaMemcpyAsync they go through the
-// device -> host copy engine, which serves its queue in order: when another thread is reading a 23 GB merged batch
+// device -> host copy engine, which serves its queue in order: when another thread is reading a multi-GB merged batch
 // back (the end-to-end pipeline of bench.py, or any reader that fetches bucket i while bucket i + 1 merges), every one
 // of them waits for hundreds of milliseconds.  Here a few threads of a kernel store the bytes into page-locked,
 // device-mapped host memory instead; the host reads them after synchronising the stream.

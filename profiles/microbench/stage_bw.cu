@@ -6,7 +6,7 @@
 //   mode 0: 1-D bulk async copies (cp.async.bulk + mbarrier), one per segment          (what k_emit does)
 //   mode 1: cp.async 16-byte copies issued by all threads (Ampere-style LDGSTS)
 //   mode 2: plain LDG.128 -> STS.128 by all threads
-// Prints achieved GB/s (bytes staged / time).  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o stage_bw stage_bw.cu
+// Prints achieved GB/s (bytes staged / time).  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o stage_bw stage_bw.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -88,7 +88,10 @@ __global__ void __launch_bounds__(512) k_stage(const uint8_t *base, size_t col_s
 int main(int argc, char **argv) {
     const int k = argc > 1 ? atoi(argv[1]) : 16, seg_bytes = argc > 2 ? atoi(argv[2]) : 2048;
     const int ncols = argc > 3 ? atoi(argv[3]) : 52, depth = argc > 4 ? atoi(argv[4]) : 2, ctas_per_sm = argc > 5 ? atoi(argv[5]) : 2;
-    const int tiles = 148 * ctas_per_sm * 24;
+    int dev = 0, sms = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int tiles = sms * ctas_per_sm * 24;
     const size_t run_stride = (size_t)tiles * seg_bytes + 4096, col_stride = run_stride * k;
     const size_t total = col_stride * ncols;
     uint8_t *d = nullptr;

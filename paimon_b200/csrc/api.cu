@@ -10,7 +10,6 @@
 #include <memory>
 #include <mutex>
 #include <queue>
-#include <unordered_map>
 
 #include "pg_internal.h"
 
@@ -40,7 +39,7 @@ struct Arena {
         return e;
     }
     void *take(size_t bytes) {
-        size_t a = (top + 255) & ~(size_t)255;
+        size_t a = align256(top);
         if (a + bytes > cap) return nullptr;
         top = a + bytes;
         return base + a;
@@ -101,46 +100,17 @@ struct Merge {
 
 // ------------------------------------------------------------------ handle tables
 
-template <typename T>
-struct Table {
-    std::mutex mu;
-    std::unordered_map<uint64_t, std::unique_ptr<T>> map;
-    uint64_t next = 1;
-    uint64_t tag;
-    explicit Table(uint64_t t) : tag(t << 56) {}
-    uint64_t put(std::unique_ptr<T> p) {
-        std::lock_guard<std::mutex> g(mu);
-        uint64_t h = tag | next++;
-        map[h] = std::move(p);
-        return h;
-    }
-    T *get(uint64_t h) {
-        std::lock_guard<std::mutex> g(mu);
-        auto it = map.find(h);
-        return it == map.end() ? nullptr : it->second.get();
-    }
-    std::unique_ptr<T> take(uint64_t h) {
-        std::lock_guard<std::mutex> g(mu);
-        auto it = map.find(h);
-        if (it == map.end()) return nullptr;
-        std::unique_ptr<T> p = std::move(it->second);
-        map.erase(it);
-        return p;
-    }
-};
-static Table<Schema> g_schemas(1);
+Table<Schema> g_schemas(1);
 static Table<Spec> g_specs(2);
-static Table<Run> g_runs(3);
+Table<Run> g_runs(3);
 static Table<Merge> g_merges(4);
 static int g_device = -1;
 
-static pg_status ensure_device() {
+pg_status ensure_device() {
     if (g_device < 0) return fail(PG_ERR_INVALID, "pg_init has not been called");
     PG_CUDA(cudaSetDevice(g_device));
     return PG_OK;
 }
-
-void buf_trim(size_t keep_bytes);
 
 // Many small copies (one per column buffer) in one driver call: cudaMemcpyBatchAsync where the driver has it,
 // else one cudaMemcpyAsync per buffer.  A wide table has hundreds of buffers per run and the per-call cost
@@ -162,8 +132,7 @@ static pg_status copy_batch(std::vector<void *> &dsts, std::vector<void *> &srcs
     for (size_t i = 0; i < dsts.size(); i++) PG_CUDA(cudaMemcpyAsync(dsts[i], srcs[i], sizes[i], kind, stream));
     return PG_OK;
 }
-// ---- device buffers of host-opened runs are recycled: a reader that streams a bucket through the device in
-// key ranges opens and frees runs at a high rate, and cudaMalloc / cudaFree would serialise the pipeline
+// ---- the recycled-buffer cache (pg_internal.h): free buffers keyed by size, up to PG_RUN_CACHE_BYTES in all
 static std::mutex g_buf_mu;
 static std::multimap<size_t, void *> g_free_bufs;
 static size_t g_free_bytes = 0;
@@ -174,7 +143,20 @@ static size_t buf_cache_limit() {
     }();
     return lim;
 }
-static void *buf_take(size_t bytes, size_t *got) {
+static void buf_trim(size_t keep_bytes) {
+    std::vector<void *> drop;
+    {
+        std::lock_guard<std::mutex> g(g_buf_mu);
+        while (g_free_bytes > keep_bytes && !g_free_bufs.empty()) {
+            auto it = std::prev(g_free_bufs.end());
+            drop.push_back(it->second);
+            g_free_bytes -= it->first;
+            g_free_bufs.erase(it);
+        }
+    }
+    for (void *p : drop) cudaFree(p);
+}
+void *buf_take(size_t bytes, size_t *got) {
     {
         std::lock_guard<std::mutex> g(g_buf_mu);
         auto it = g_free_bufs.lower_bound(bytes);
@@ -195,7 +177,7 @@ static void *buf_take(size_t bytes, size_t *got) {
     *got = bytes;
     return p;
 }
-static void buf_give(void *p, size_t bytes) {
+void buf_give(void *p, size_t bytes) {
     {
         std::lock_guard<std::mutex> g(g_buf_mu);
         if (g_free_bytes + bytes <= buf_cache_limit()) {
@@ -206,41 +188,14 @@ static void buf_give(void *p, size_t bytes) {
     }
     cudaFree(p);
 }
-void buf_trim(size_t keep_bytes) {
-    std::vector<void *> drop;
-    {
-        std::lock_guard<std::mutex> g(g_buf_mu);
-        while (g_free_bytes > keep_bytes && !g_free_bufs.empty()) {
-            auto it = std::prev(g_free_bufs.end());
-            drop.push_back(it->second);
-            g_free_bytes -= it->first;
-            g_free_bufs.erase(it);
-        }
-    }
-    for (void *p : drop) cudaFree(p);
-}
-static cudaStream_t copy_stream() {                   // one non-blocking copy stream per calling thread
+cudaStream_t copy_stream() {                          // one non-blocking copy stream per calling thread
     static thread_local cudaStream_t st = nullptr;
     if (!st) cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking);
     return st;
 }
 
-
-// hooks for the other translation units (parquet_decode.cu)
-Schema *schema_from_handle(uint64_t h) { return g_schemas.get(h); }
-Run *run_from_handle(uint64_t h) { return g_runs.get(h); }
-// recycled device buffers and the calling thread's copy stream, for the format readers
-void *device_buffer_take(size_t bytes, size_t *got) { return buf_take(bytes, got); }
-void device_buffer_give(void *p, size_t bytes) { buf_give(p, bytes); }
-cudaStream_t thread_stream() { return copy_stream(); }
-uint64_t register_run(std::unique_ptr<Run> run) { return g_runs.put(std::move(run)); }
-pg_status require_device() { return ensure_device(); }
-
-// parquet_encode.cu: the columns of a merge handle's current batch, or of a run
 pg_status batch_columns(uint64_t handle, const Schema **schema, std::vector<DevColumn> *cols, int64_t *n_rows) {
-    if ((handle >> 56) == 4) {
-        Merge *m = g_merges.get(handle);
-        if (!m) return fail(PG_ERR_INVALID, "unknown merge handle");
+    if (Merge *m = g_merges.get(handle)) {
         if (!m->has_batch) return fail(PG_ERR_INVALID, "no batch: call pg_merge_execute first");
         if (m->stream) PG_CUDA(cudaStreamSynchronize(m->stream));
         *schema = m->schema;
@@ -409,24 +364,23 @@ static pg_status build_descriptors(Merge *m) {
 
     // one device allocation for all descriptor arrays
     const int k = m->k, nk = s->n_key, nv = (int)m->varlen_cols.size();
-    auto align = [](size_t x) { return (x + 255) & ~(size_t)255; };
     size_t o_key = 0;
-    size_t o_koff = o_key + align(sizeof(void *) * k * nk);
-    size_t o_seq = o_koff + align(sizeof(void *) * k * nk);
-    size_t o_kind = o_seq + align(sizeof(void *) * k);
-    size_t o_pd = o_kind + align(sizeof(void *) * k);
-    size_t o_po = o_pd + align(sizeof(void *) * (size_t)k * nc);
-    size_t o_pv = o_po + align(sizeof(void *) * (size_t)k * nc);
-    size_t o_rows = o_pv + align(sizeof(void *) * (size_t)k * nc);
-    size_t o_cols = o_rows + align(sizeof(int64_t) * k);
-    size_t o_out = o_cols + align(sizeof(ColDesc) * nc);
-    size_t o_tot = o_out + align(sizeof(pg_out_column) * nc);
-    size_t o_err = o_tot + align(sizeof(int64_t) * (nv + 1));
+    size_t o_koff = o_key + align256(sizeof(void *) * k * nk);
+    size_t o_seq = o_koff + align256(sizeof(void *) * k * nk);
+    size_t o_kind = o_seq + align256(sizeof(void *) * k);
+    size_t o_pd = o_kind + align256(sizeof(void *) * k);
+    size_t o_po = o_pd + align256(sizeof(void *) * (size_t)k * nc);
+    size_t o_pv = o_po + align256(sizeof(void *) * (size_t)k * nc);
+    size_t o_rows = o_pv + align256(sizeof(void *) * (size_t)k * nc);
+    size_t o_cols = o_rows + align256(sizeof(int64_t) * k);
+    size_t o_out = o_cols + align256(sizeof(ColDesc) * nc);
+    size_t o_tot = o_out + align256(sizeof(pg_out_column) * nc);
+    size_t o_err = o_tot + align256(sizeof(int64_t) * (nv + 1));
     size_t o_cnt = o_err + 256;
     size_t o_ord = o_cnt + 256;
-    size_t o_vlc = o_ord + align(sizeof(int32_t) * (2 * (size_t)nc + 2));
-    size_t o_sg = o_vlc + align(sizeof(int32_t) * (size_t)(nv + 1));
-    size_t total = o_sg + align(sizeof(SeqGroups));
+    size_t o_vlc = o_ord + align256(sizeof(int32_t) * (2 * (size_t)nc + 2));
+    size_t o_sg = o_vlc + align256(sizeof(int32_t) * (size_t)(nv + 1));
+    size_t total = o_sg + align256(sizeof(SeqGroups));
     std::vector<unsigned char> host(total, 0);
     m->varlen_bound.assign(nv, 0);
     for (int r = 0; r < k; r++) {
@@ -579,7 +533,7 @@ static pg_status execute(Merge *m) {
     // one bucket layout) never goes back to the driver allocator.
     {
         size_t need = 4096;
-        auto add = [&](size_t b) { need += ((b ? b : 16) + 255) & ~(size_t)255; };
+        auto add = [&](size_t b) { need += align256(b ? b : 16); };
         for (int l = top; l >= 0; l--) {
             add(sizeof(int64_t) * (size_t)(n_tiles[l] + 1) * k);
             if (l > 0) { add(sizeof(uint64_t) * (size_t)std::max<int64_t>(level_total[l], 1)); add(sizeof(uint64_t) * (size_t)std::max<int64_t>(level_total[l], 1)); }
@@ -594,7 +548,6 @@ static pg_status execute(Merge *m) {
         *out = m->work.take(bytes ? bytes : 16);
         return *out ? cudaSuccess : cudaErrorMemoryAllocation;
     };
-    auto free_temps = [&]() {};
 
     if (!m->key.exact) {
         // window keys start behind the prefix all keys share (strings like "user_0000123", wide composites)
@@ -673,10 +626,9 @@ static pg_status execute(Merge *m) {
         pg_status rs = rb.add(m->h_totals, m->d_totals, sizeof(int64_t));
         if (!rs) rs = rb.add(m->h_err, m->d_err, sizeof(int32_t));
         if (!rs) rs = rb.finish();
-        if (rs) { free_temps(); return rs; }
+        if (rs) return rs;
     }
     if (*m->h_err != KERR_NONE) {
-        free_temps();
         return fail(*m->h_err == KERR_TILE_OVERFLOW || *m->h_err == KERR_OFFSET_OVERFLOW ? PG_ERR_INTERNAL
                                                                                         : PG_ERR_MERGE_FUNCTION,
                     kernel_error_message(*m->h_err));
@@ -691,15 +643,14 @@ static pg_status execute(Merge *m) {
         // output arena (grow-only, reused until pg_merge_release): validity bitmaps first and contiguous,
         // so that one memset clears them all
         size_t need = 4096, vbytes = 0;
-        auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
         for (int c = 0; c < nc; c++) {
             const ColDesc &cd = m->cols[c];
             if (!m->emit[c]) continue;
-            if (cd.nullable) vbytes += pad((size_t)((n_out + 31) / 32) * 4 + 64);
-            if (cd.width > 0) need += pad((size_t)n_out * cd.width + 64);
-            else need += pad((size_t)m->varlen_bound[cd.varlen_index] + 64) + pad(4 * (size_t)(n_out + 1) + 64);
+            if (cd.nullable) vbytes += align256((size_t)((n_out + 31) / 32) * 4 + 64);
+            if (cd.width > 0) need += align256((size_t)n_out * cd.width + 64);
+            else need += align256((size_t)m->varlen_bound[cd.varlen_index] + 64) + align256(4 * (size_t)(n_out + 1) + 64);
         }
-        if (nv > 0) need += pad(sizeof(uint16_t) * (size_t)nv * (size_t)(n_out + 64) + 64);   // k_emit's source scratch
+        if (nv > 0) need += align256(sizeof(uint16_t) * (size_t)nv * (size_t)(n_out + 64) + 64);   // k_emit's source scratch
         PG_CUDA(m->outbuf.reserve(need + vbytes));
         if (vbytes) {
             void *v0 = m->outbuf.take(vbytes);
@@ -707,9 +658,7 @@ static pg_status execute(Merge *m) {
             m->outbuf.top = 0;                       // validity buffers are taken again, one by one, below
         }
     }
-    bool validity_phase = true;
     auto oalloc = [&](size_t bytes, void **out) -> cudaError_t {
-        (void)validity_phase;
         *out = m->outbuf.take(bytes);
         return *out ? cudaSuccess : cudaErrorMemoryAllocation;
     };
@@ -776,7 +725,6 @@ static pg_status execute(Merge *m) {
         SmallReads rb(sm);
         pg_status rs = rb.add(m->h_err, m->d_err, sizeof(int32_t));
         if (!rs) rs = rb.add(m->h_totals, m->d_totals, sizeof(int64_t) * (nv + 1));
-        free_temps();
         if (!rs) rs = rb.finish();
         if (rs) return rs;
     }
@@ -963,15 +911,9 @@ pg_status pg_run_open(uint64_t schema, const pg_run_desc *desc, int32_t mem, uin
     if (desc->n_rows < 0 || desc->n_rows > 0x7fffffffLL) return fail(PG_ERR_INVALID, "bad row count");
     pg_status st = ensure_device();
     if (st) return st;
-    auto run = std::make_unique<Run>();
-    run->own_schema = *s;
-    run->schema = &run->own_schema;   // the run outlives the schema handle it was opened with
-    run->n_rows = desc->n_rows;
+    auto run = std::make_unique<Run>(*s, desc->n_rows);
     const int nc = s->n_cols();
     const int64_t n = desc->n_rows;
-    run->cols.resize(nc);
-    run->varlen_bytes.assign(nc, 0);
-    run->varlen_base.assign(nc, 0);
     if (mem == PG_MEM_DEVICE) {
         for (int c = 0; c < nc; c++) {
             const pg_column &pc = desc->cols[c];
@@ -987,7 +929,6 @@ pg_status pg_run_open(uint64_t schema, const pg_run_desc *desc, int32_t mem, uin
         }
     } else if (mem == PG_MEM_HOST) {
         // one device allocation per run, columns sub-allocated at 256-byte boundaries
-        auto align = [](size_t x) { return (x + 255) & ~(size_t)255; };
         std::vector<size_t> o_data(nc), o_off(nc), o_val(nc), b_data(nc), b_off(nc), b_val(nc);
         size_t total = 0;
         for (int c = 0; c < nc; c++) {
@@ -1005,17 +946,14 @@ pg_status pg_run_open(uint64_t schema, const pg_run_desc *desc, int32_t mem, uin
                 b_data[c] = (size_t)n * type_width(f.type);
             }
             b_val[c] = pc.validity ? (size_t)((n + 7) / 8) : 0;
-            o_data[c] = total; total += align(b_data[c] + 16);
-            o_off[c] = total; total += align(b_off[c]);
-            o_val[c] = total; total += align(b_val[c] + 8);
+            o_data[c] = total; total += align256(b_data[c] + 16);
+            o_off[c] = total; total += align256(b_off[c]);
+            o_val[c] = total; total += align256(b_val[c] + 8);
         }
-        size_t got = 0;
-        void *base = buf_take(total + 256, &got);
-        if (!base) return fail(PG_ERR_CUDA, "out of device memory for a run");
-        run->owned.push_back(base);
-        run->owned_bytes.push_back(got);
-        unsigned char *d = (unsigned char *)base;
         cudaStream_t cs = copy_stream();
+        Scratch scratch(cs);                          // the run's buffer until its copies are done
+        unsigned char *d = (unsigned char *)scratch.take(total + 256);
+        if (!d) return fail(PG_ERR_CUDA, "out of device memory for a run");
         std::vector<void *> cp_dst, cp_src;
         std::vector<size_t> cp_size;
         auto add_copy = [&](void *dst, const void *src, size_t bytes) {
@@ -1042,6 +980,7 @@ pg_status pg_run_open(uint64_t schema, const pg_run_desc *desc, int32_t mem, uin
         pg_status cst = copy_batch(cp_dst, cp_src, cp_size, cudaMemcpyHostToDevice, cs);
         if (cst) return cst;
         PG_CUDA(cudaStreamSynchronize(cs));
+        run->bufs.swap(scratch.bufs);
     } else {
         return fail(PG_ERR_INVALID, "bad memory kind");
     }
@@ -1050,13 +989,7 @@ pg_status pg_run_open(uint64_t schema, const pg_run_desc *desc, int32_t mem, uin
 }
 
 pg_status pg_run_free(uint64_t run) {
-    auto r = g_runs.take(run);
-    if (!r) return fail(PG_ERR_INVALID, "unknown run handle");
-    for (size_t i = 0; i < r->owned.size(); i++) {
-        if (i < r->owned_bytes.size()) buf_give(r->owned[i], r->owned_bytes[i]);
-        else cudaFree(r->owned[i]);
-    }
-    return PG_OK;
+    return g_runs.take(run) ? PG_OK : fail(PG_ERR_INVALID, "unknown run handle");
 }
 
 pg_status pg_run_layout(uint64_t run, int64_t *n_rows, int64_t *data_bytes, int32_t *has_validity, int32_t n_cols) {
@@ -1113,14 +1046,8 @@ static pg_status make_slice(uint64_t source, int64_t row_lo, int64_t row_hi, uin
     if (st) return st;
     if (row_lo < 0 || row_hi < row_lo || row_hi > n) return fail(PG_ERR_INVALID, "slice outside the source");
     const int64_t lo = row_lo & ~(int64_t)127;
-    auto run = std::make_unique<Run>();
-    run->own_schema = *s;
-    run->schema = &run->own_schema;
-    run->n_rows = row_hi - lo;
+    auto run = std::make_unique<Run>(*s, row_hi - lo);
     const int nc = s->n_cols();
-    run->cols.resize(nc);
-    run->varlen_bytes.assign(nc, 0);
-    run->varlen_base.assign(nc, 0);
     for (int c = 0; c < nc; c++) {
         const pg_field f = s->field(c);
         DevColumn dc = cols[c];

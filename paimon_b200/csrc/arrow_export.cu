@@ -17,10 +17,6 @@
 #include "pg_internal.h"
 
 namespace pg {
-
-pg_status batch_columns(uint64_t handle, const Schema **schema, std::vector<DevColumn> *cols, int64_t *n_rows);   // api.cu
-pg_status require_device();
-
 namespace {
 
 struct SchemaPriv {
@@ -216,7 +212,7 @@ using namespace pg;
 extern "C" pg_status pg_export_arrow(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
                                      struct ArrowArray *out, struct ArrowSchema *out_schema) {
     if (!out) return fail(PG_ERR_INVALID, "null argument");
-    pg_status st = require_device();
+    pg_status st = ensure_device();
     if (st) return st;
     return export_arrow(source, column_names, row0, n_rows, out, out_schema);
 }

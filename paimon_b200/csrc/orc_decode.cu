@@ -25,13 +25,6 @@
 
 namespace pg {
 
-Schema *schema_from_handle(uint64_t h);                 // api.cu
-void *device_buffer_take(size_t bytes, size_t *got);
-void device_buffer_give(void *p, size_t bytes);
-cudaStream_t thread_stream();
-uint64_t register_run(std::unique_ptr<Run> run);
-pg_status require_device();
-
 struct OrcStream {
     const uint8_t *src;        // device: the stream as stored in the file
     uint8_t *dst;              // scratch image (compressed files)
@@ -127,16 +120,6 @@ __global__ void k_orc_set_payload(orcdev::Task *tasks, int n_tasks, const int32_
     if (i < n_tasks && tasks[i].out_width == 0) tasks[i].out_payload = payload_of_out[task_out[i]];
 }
 
-static int orc_out_width(int t) {
-    switch (t) {
-        case PG_INT8: case PG_BOOL: return 1;
-        case PG_INT16: return 2;
-        case PG_INT32: case PG_FLOAT: return 4;
-        case PG_INT64: case PG_DOUBLE: return 8;
-        default: return 0;
-    }
-}
-
 // OrcTypeUtil (paimon-format/.../orc/OrcTypeUtil.java convertToOrcType): which ORC type a Paimon column has in the file;
 // the integer / float widenings schema evolution allows are accepted (orc-core's SchemaEvolution does the same)
 static bool orc_type_ok(int pg_t, const orc::Type &ty) {
@@ -156,28 +139,11 @@ static bool orc_type_ok(int pg_t, const orc::Type &ty) {
     }
 }
 
-struct OrcBufs {
-    cudaStream_t stream = nullptr;
-    std::vector<std::pair<void *, size_t>> bufs;
-    void *take(size_t bytes) {
-        size_t got = 0;
-        void *p = device_buffer_take(bytes ? bytes : 256, &got);
-        if (p) bufs.push_back({p, got});
-        return p;
-    }
-    ~OrcBufs() {
-        if (stream && !bufs.empty()) cudaStreamSynchronize(stream);
-        for (auto &b : bufs) device_buffer_give(b.first, b.second);
-    }
-};
-
 static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, int nf, int n_runs, const char *const *names,
                                     const uint8_t *read_cols, uint64_t *out_runs, pg_section_info *info) {
     const int nc = s->n_cols();
-    cudaStream_t sm = thread_stream();
-    auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    OrcBufs scratch;
-    scratch.stream = sm;
+    cudaStream_t sm = copy_stream();
+    Scratch scratch(sm);                               // file images, tables, scratch and the runs until registered
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     struct EvGuard { cudaEvent_t &a, &b; ~EvGuard() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); } } evg{e0, e1};
     PG_CUDA(cudaEventCreate(&e0));
@@ -272,48 +238,34 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
     }
 
     // ---- output columns (validity bitmaps first and contiguous: one memset)
-    std::vector<std::unique_ptr<Run>> runs(n_runs);
-    struct RunGuard {
-        std::vector<std::unique_ptr<Run>> &runs;
-        ~RunGuard() {
-            for (auto &r : runs)
-                if (r) for (size_t q = 0; q < r->owned.size(); q++) device_buffer_give(r->owned[q], r->owned_bytes[q]);
-        }
-    } run_guard{runs};
+    std::vector<std::unique_ptr<Run>> &runs = scratch.runs;
+    runs.resize(n_runs);
     struct OutCol { void *data = nullptr; int32_t *offsets = nullptr; uint32_t *validity = nullptr; };
     std::vector<OutCol> outs((size_t)n_runs * nc);
     int64_t decoded_bytes = 0;
     for (int r = 0; r < n_runs; r++) {
         const int64_t n = run_rows[r];
-        auto run = std::make_unique<Run>();
-        run->own_schema = *s;
-        run->schema = &run->own_schema;
-        run->n_rows = n;
-        run->cols.resize(nc);
-        run->varlen_bytes.assign(nc, 0);
-        run->varlen_base.assign(nc, 0);
-        const size_t vb = pad((size_t)((n + 31) / 32) * 4 + 64);
+        runs[r] = std::make_unique<Run>(*s, n);
+        const size_t vb = align256((size_t)((n + 31) / 32) * 4 + 64);
         size_t vbytes = 0, total = 0;
         // ORC columns are nullable by format: every column the read schema calls nullable gets a bitmap
         for (int c = 0; c < nc; c++) if (wanted[c] && s->field(c).nullable) vbytes += vb;
         total = vbytes;
         std::vector<size_t> o_main(nc);
         for (int c = 0; c < nc; c++) {
-            const int ow = orc_out_width(s->field(c).type);
+            const int ow = type_width(s->field(c).type);
             o_main[c] = total;
-            if (wanted[c]) total += ow ? pad((size_t)n * ow + 64) : pad(4 * (size_t)(n + 1) + 64);
+            if (wanted[c]) total += ow ? align256((size_t)n * ow + 64) : align256(4 * (size_t)(n + 1) + 64);
         }
-        size_t got = 0;
-        unsigned char *base = (unsigned char *)device_buffer_take(total + 256, &got);
+        runs[r]->bufs.emplace_back(total + 256);
+        unsigned char *base = runs[r]->bufs.back().get();
         if (!base) return fail(PG_ERR_CUDA, "orc: out of device memory");
-        run->owned.push_back(base);
-        run->owned_bytes.push_back(got);
         if (vbytes) PG_CUDA(cudaMemsetAsync(base, 0, vbytes, sm));
         size_t vt = 0;
         for (int c = 0; c < nc; c++) {
             if (!wanted[c]) continue;
             OutCol &o = outs[(size_t)r * nc + c];
-            const int ow = orc_out_width(s->field(c).type);
+            const int ow = type_width(s->field(c).type);
             if (s->field(c).nullable) { o.validity = (uint32_t *)(base + vt); vt += vb; decoded_bytes += (n + 7) / 8; }
             if (ow) { o.data = base + o_main[c]; decoded_bytes += n * ow; }
             else { o.offsets = (int32_t *)(base + o_main[c]); decoded_bytes += 4 * (n + 1); }
@@ -321,7 +273,6 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
             if (!ow || col_missing[(size_t)r * nc + c])
                 PG_CUDA(cudaMemsetAsync(base + o_main[c], 0, ow ? (size_t)n * ow : 4 * (size_t)(n + 1), sm));
         }
-        runs[r] = std::move(run);
     }
 
     // ---- stream and task tables
@@ -358,7 +309,7 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
             k.row0 = file_row0[f] + p.row0;
             k.rows = p.rows;
             k.kind = p.kind; k.enc = p.enc; k.dict_size = (int32_t)p.dict_size; k.scale = p.scale;
-            k.out_width = orc_out_width(s->field(p.col).type);
+            k.out_width = type_width(s->field(p.col).type);
             k.out_data = o.data;
             k.out_offsets = o.offsets;
             k.out_validity = o.validity;
@@ -371,15 +322,15 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
         dict_base += plans[f].dict_entries;
     }
     const int n_streams = (int)h_streams.size(), n_tasks = (int)h_tasks.size();
-    const size_t tb_s = pad(sizeof(OrcStream) * (size_t)std::max(n_streams, 1)), tb_t = pad(sizeof(orcdev::Task) * (size_t)std::max(n_tasks, 1));
-    const size_t tb_r = pad(sizeof(OrcTaskRef) * (size_t)std::max(n_tasks, 1)), tb_o = pad(4 * (size_t)std::max(n_tasks, 1));
-    const size_t tb_p = pad(sizeof(void *) * outs.size());
+    const size_t tb_s = align256(sizeof(OrcStream) * (size_t)std::max(n_streams, 1)), tb_t = align256(sizeof(orcdev::Task) * (size_t)std::max(n_tasks, 1));
+    const size_t tb_r = align256(sizeof(OrcTaskRef) * (size_t)std::max(n_tasks, 1)), tb_o = align256(4 * (size_t)std::max(n_tasks, 1));
+    const size_t tb_p = align256(sizeof(void *) * outs.size());
     int sms = 132, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int inflate_ctas = !any_compressed ? std::max(1, std::min(sms, (n_streams + kOrcWarps - 1) / kOrcWarps))
                                                   : std::max(1, std::min(sms * 4, (n_streams + kOrcWarps - 1) / kOrcWarps));
-    const size_t tb_lit = any_zstd ? pad((size_t)inflate_ctas * kOrcWarps * (size_t)(zs::kMaxBlock + 64)) : 256;
+    const size_t tb_lit = any_zstd ? align256((size_t)inflate_ctas * kOrcWarps * (size_t)(zs::kMaxBlock + 64)) : 256;
     unsigned char *tb = (unsigned char *)scratch.take(tb_s + tb_t + tb_r + tb_o + tb_p + tb_lit + 1024);
     if (!tb) return fail(PG_ERR_CUDA, "orc: out of device memory");
     OrcStream *d_streams = (OrcStream *)tb;
@@ -434,12 +385,10 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
         std::vector<uint8_t *> h_payload(outs.size(), nullptr);
         for (int r = 0; r < n_runs; r++) {
             size_t sum = 256;
-            for (size_t i = 0; i < vl.size(); i++) if (vl[i].first == r) sum += pad((size_t)totals[i] + 64);
-            size_t got = 0;
-            unsigned char *pl = (unsigned char *)device_buffer_take(sum, &got);
+            for (size_t i = 0; i < vl.size(); i++) if (vl[i].first == r) sum += align256((size_t)totals[i] + 64);
+            runs[r]->bufs.emplace_back(sum);
+            unsigned char *pl = runs[r]->bufs.back().get();
             if (!pl) return fail(PG_ERR_CUDA, "orc: out of device memory");
-            runs[r]->owned.push_back(pl);
-            runs[r]->owned_bytes.push_back(got);
             size_t pt = 0;
             for (size_t i = 0; i < vl.size(); i++) {
                 if (vl[i].first != r) continue;
@@ -447,7 +396,7 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
                 h_payload[(size_t)r * nc + vl[i].second] = pl + pt;
                 runs[r]->varlen_bytes[vl[i].second] = totals[i];
                 decoded_bytes += totals[i];
-                pt += pad((size_t)totals[i] + 64);
+                pt += align256((size_t)totals[i] + 64);
             }
         }
         PG_CUDA(cudaMemcpyAsync(d_payload, h_payload.data(), sizeof(void *) * outs.size(), cudaMemcpyHostToDevice, sm));
@@ -471,7 +420,7 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
             const OutCol &o = outs[(size_t)r * nc + c];
             DevColumn dc;
             if (wanted[c]) {
-                dc.data = o.data ? o.data : (const void *)runs[r]->owned[0];
+                dc.data = o.data ? o.data : (const void *)runs[r]->bufs[0].get();
                 dc.offsets = o.offsets;
                 dc.validity = (const uint8_t *)o.validity;
             }
@@ -479,7 +428,7 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
         }
         runs[r]->bytes_h2d = r == 0 ? file_bytes : 0;
         n_rows += run_rows[r];
-        out_runs[r] = register_run(std::move(runs[r]));
+        out_runs[r] = g_runs.put(std::move(runs[r]));
     }
     if (info) {
         memset(info, 0, sizeof(*info));
@@ -504,11 +453,11 @@ using namespace pg;
 extern "C" pg_status pg_orc_read_section(uint64_t schema, const pg_file_desc *files, int32_t n_files, int32_t n_runs,
                                          const char *const *column_names, const uint8_t *read_columns, uint64_t *out_runs,
                                          pg_section_info *info) {
-    Schema *s = schema_from_handle(schema);
+    Schema *s = g_schemas.get(schema);
     if (!s || !out_runs || n_files < 0 || n_runs < 0 || (n_files > 0 && !files))
         return fail(PG_ERR_INVALID, "bad schema handle or null argument");
     if (n_runs == 0) return n_files == 0 ? PG_OK : fail(PG_ERR_INVALID, "files without runs");
-    pg_status st = require_device();
+    pg_status st = ensure_device();
     if (st) return st;
     const Schema own = *s;
     return orc_decode_section(&own, files, n_files, n_runs, column_names, read_columns, out_runs, info);

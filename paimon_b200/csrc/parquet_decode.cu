@@ -29,7 +29,6 @@
 #include <algorithm>
 #include <cstring>
 #include <memory>
-#include <mutex>
 #include <stdexcept>
 #include <unordered_map>
 
@@ -1247,23 +1246,6 @@ __global__ void k_pq_zero_first_offset(const PqOut *outs, int n) {
 
 // ------------------------------------------------------------------ host side
 
-Schema *schema_from_handle(uint64_t h);                 // api.cu
-void *device_buffer_take(size_t bytes, size_t *got);    // api.cu: recycled device buffers
-void device_buffer_give(void *p, size_t bytes);
-cudaStream_t thread_stream();                           // api.cu: the calling thread's non-blocking stream
-uint64_t register_run(std::unique_ptr<Run> run);        // api.cu
-pg_status require_device();                             // api.cu
-
-static int out_width_of(int t) {
-    switch (t) {
-        case PG_INT8: case PG_BOOL: return 1;
-        case PG_INT16: return 2;
-        case PG_INT32: case PG_FLOAT: return 4;
-        case PG_INT64: case PG_DOUBLE: return 8;
-        default: return 0;
-    }
-}
-
 // ParquetSchemaConverter.java:76-160 — which physical type a Paimon column has in the file.  Returns the cast the
 // decoder applies (0 = none), or -1 when the file type does not map to the read type.  Besides the exact mapping, the
 // widenings Paimon's schema evolution allows without rewriting files are accepted: INT-family -> BIGINT, FLOAT -> DOUBLE.
@@ -1373,31 +1355,13 @@ struct SectionFile {
     const pq::FileMetaData *meta; // already parsed (single-file reader), or NULL
 };
 
-// recycled device buffers taken during one decode; everything not moved into a Run goes back on scope exit
-struct BufList {
-    cudaStream_t stream = nullptr;                    // kernels still using the buffers run on this stream
-    std::vector<std::pair<void *, size_t>> bufs;
-    void *take(size_t bytes) {
-        size_t got = 0;
-        void *p = device_buffer_take(bytes ? bytes : 256, &got);
-        if (p) bufs.push_back({p, got});
-        return p;
-    }
-    ~BufList() {
-        if (stream && !bufs.empty()) cudaStreamSynchronize(stream);
-        for (auto &b : bufs) device_buffer_give(b.first, b.second);
-    }
-};
-
 static pg_status decode_section(const Schema *s, const std::vector<SectionFile> &files, int n_runs,
                                 const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
                                 pg_section_info *info) {
     const int nc = s->n_cols();
     const int nf = (int)files.size();
-    cudaStream_t sm = thread_stream();
-    auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    BufList scratch;                                   // file images, tables, scratch: released on return
-    scratch.stream = sm;
+    cudaStream_t sm = copy_stream();
+    Scratch scratch(sm);                               // file images, tables, scratch and the runs until registered
     int launches = 0;
     cudaEvent_t e0 = nullptr, e1 = nullptr;
     struct EvGuard { cudaEvent_t &a, &b; ~EvGuard() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); } } evg{e0, e1};
@@ -1550,49 +1514,34 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     const int n_chunks = (int)chunks.size(), n_pairs = (int)pairs.size();
 
     // ---- output columns: one recycled buffer per run (validity bitmaps first and contiguous: one memset)
-    std::vector<std::unique_ptr<Run>> runs(n_runs);
+    std::vector<std::unique_ptr<Run>> &runs = scratch.runs;
+    runs.resize(n_runs);
     std::vector<PqOut> outs((size_t)n_runs * nc);
     int64_t decoded_bytes = 0;
     bool any_empty = false;
-    struct RunGuard {                                   // buffers of runs that were not registered go back
-        std::vector<std::unique_ptr<Run>> &runs;
-        ~RunGuard() {
-            for (auto &r : runs)
-                if (r) for (size_t q = 0; q < r->owned.size(); q++) device_buffer_give(r->owned[q], r->owned_bytes[q]);
-        }
-    } run_guard{runs};
     for (int r = 0; r < n_runs; r++) {
         const int64_t n = run_rows[r];
         if (n == 0) any_empty = true;
-        auto run = std::make_unique<Run>();
-        run->own_schema = *s;
-        run->schema = &run->own_schema;
-        run->n_rows = n;
-        run->cols.resize(nc);
-        run->varlen_bytes.assign(nc, 0);
-        run->varlen_base.assign(nc, 0);
-        run->bytes_h2d = 0;
+        runs[r] = std::make_unique<Run>(*s, n);
         size_t vbytes = 0, total = 0;
-        const size_t vb = pad((size_t)((n + 31) / 32) * 4 + 64);
+        const size_t vb = align256((size_t)((n + 31) / 32) * 4 + 64);
         for (int c = 0; c < nc; c++) if (wanted[c] && any_optional[c]) vbytes += vb;
         total = vbytes;
         std::vector<size_t> o_main(nc);
         for (int c = 0; c < nc; c++) {
-            const int ow = out_width_of(s->field(c).type);
+            const int ow = type_width(s->field(c).type);
             o_main[c] = total;
-            if (wanted[c]) total += ow ? pad((size_t)n * ow + 64) : pad(4 * (size_t)(n + 1) + 64);
+            if (wanted[c]) total += ow ? align256((size_t)n * ow + 64) : align256(4 * (size_t)(n + 1) + 64);
         }
-        size_t got = 0;
-        unsigned char *base = (unsigned char *)device_buffer_take(total + 256, &got);
+        runs[r]->bufs.emplace_back(total + 256);
+        unsigned char *base = runs[r]->bufs.back().get();
         if (!base) return oom("the columns of a run", total);
-        run->owned.push_back(base);
-        run->owned_bytes.push_back(got);
         if (vbytes) PG_CUDA(cudaMemsetAsync(base, 0, vbytes, sm));
         size_t vt = 0;
         for (int c = 0; c < nc; c++) {
             PqOut &o = outs[(size_t)r * nc + c];
             memset(&o, 0, sizeof(o));
-            const int ow = out_width_of(s->field(c).type);
+            const int ow = type_width(s->field(c).type);
             o.out_width = ow;
             o.is_bool = s->field(c).type == PG_BOOL;
             if (!wanted[c]) continue;                    // not part of the read type: the run has no such column
@@ -1603,14 +1552,13 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
             if (col_missing[(size_t)r * nc + c])
                 PG_CUDA(cudaMemsetAsync(base + o_main[c], 0, ow ? (size_t)n * ow : 4 * (size_t)(n + 1), sm));
         }
-        runs[r] = std::move(run);
     }
 
     // ---- tables to the device, page count pass
-    const size_t tb_chunks = pad(sizeof(PqChunk) * (size_t)std::max(n_chunks, 1));
-    const size_t tb_outs = pad(sizeof(PqOut) * outs.size());
-    const size_t tb_pairs = pad(sizeof(PqPair) * (size_t)std::max(n_pairs, 1));
-    const size_t tb_tot = pad(sizeof(int64_t) * (size_t)(8 + n_pairs));
+    const size_t tb_chunks = align256(sizeof(PqChunk) * (size_t)std::max(n_chunks, 1));
+    const size_t tb_outs = align256(sizeof(PqOut) * outs.size());
+    const size_t tb_pairs = align256(sizeof(PqPair) * (size_t)std::max(n_pairs, 1));
+    const size_t tb_tot = align256(sizeof(int64_t) * (size_t)(8 + n_pairs));
     unsigned char *tb = (unsigned char *)scratch.take(tb_chunks + tb_outs + tb_pairs + tb_tot + 256);
     if (!tb) return oom("the chunk tables", tb_chunks + tb_outs + tb_pairs + tb_tot);
     PqChunk *d_chunks = (PqChunk *)tb;
@@ -1643,12 +1591,12 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     if (n_pages > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet: too many pages in one section");
 
     // ---- page table + scratch, fill pass, inflate
-    const size_t sb_pages = pad(sizeof(PqPage) * (size_t)std::max<int64_t>(n_pages, 1));
-    const size_t sb_dicts = pad(sizeof(PqPage) * (size_t)std::max<int64_t>(n_dicts, 1));
-    const size_t sb_sc = pad((size_t)sc_bytes + 64);
-    const size_t sb_de = pad(4 * (size_t)(dict_entries + 1));
-    const size_t sb_ids = pad(4 * (size_t)(ids_entries + 1));
-    const size_t sb_vs = pad(4 * (size_t)(pair_rows + n_pages + n_pairs + 2));
+    const size_t sb_pages = align256(sizeof(PqPage) * (size_t)std::max<int64_t>(n_pages, 1));
+    const size_t sb_dicts = align256(sizeof(PqPage) * (size_t)std::max<int64_t>(n_dicts, 1));
+    const size_t sb_sc = align256((size_t)sc_bytes + 64);
+    const size_t sb_de = align256(4 * (size_t)(dict_entries + 1));
+    const size_t sb_ids = align256(4 * (size_t)(ids_entries + 1));
+    const size_t sb_vs = align256(4 * (size_t)(pair_rows + n_pages + n_pairs + 2));
     int zs_ctas = 0;
     if (any_zstd) {
         int dev = 0, sms = 132;
@@ -1656,7 +1604,7 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         zs_ctas = (int)std::min<int64_t>((int64_t)sms * 5, (n_pages + n_dicts + kZsWarps - 1) / kZsWarps);
     }
-    const size_t sb_zs = pad((size_t)zs_ctas * kZsWarps * (size_t)(zs::kMaxBlock + 64));
+    const size_t sb_zs = align256((size_t)zs_ctas * kZsWarps * (size_t)(zs::kMaxBlock + 64));
     unsigned char *sbuf = (unsigned char *)scratch.take(sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs + 256);
     if (!sbuf) return oom("the page table and scratch", sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs);
     PqPage *d_pages = (PqPage *)sbuf;
@@ -1712,19 +1660,17 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     if (n_pairs) {
         for (int r = 0; r < n_runs; r++) {
             size_t sum = 256;
-            for (const PqPair &pr : pairs) if (pr.run == r) sum += pad((size_t)pair_tot[pr.idx] + 64);
-            size_t got = 0;
-            unsigned char *pl = (unsigned char *)device_buffer_take(sum, &got);
+            for (const PqPair &pr : pairs) if (pr.run == r) sum += align256((size_t)pair_tot[pr.idx] + 64);
+            runs[r]->bufs.emplace_back(sum);
+            unsigned char *pl = runs[r]->bufs.back().get();
             if (!pl) return oom("the var-len payload of a run", sum);
-            runs[r]->owned.push_back(pl);
-            runs[r]->owned_bytes.push_back(got);
             size_t pt = 0;
             for (const PqPair &pr : pairs) {
                 if (pr.run != r) continue;
                 outs[(size_t)r * nc + pr.col].data = pl + pt;
                 runs[r]->varlen_bytes[pr.col] = pair_tot[pr.idx];
                 decoded_bytes += pair_tot[pr.idx];
-                pt += pad((size_t)pair_tot[pr.idx] + 64);
+                pt += align256((size_t)pair_tot[pr.idx] + 64);
             }
         }
         { pg_status ts = small_h2d(d_outs, outs.data(), sizeof(PqOut) * outs.size(), sm); if (ts) return ts; }
@@ -1805,14 +1751,14 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
             const PqOut &o = outs[(size_t)r * nc + c];
             DevColumn dc;
             if (wanted[c]) {
-                dc.data = o.data ? o.data : (const void *)runs[r]->owned[0];
+                dc.data = o.data ? o.data : (const void *)runs[r]->bufs[0].get();
                 dc.offsets = o.offsets;
                 dc.validity = (const uint8_t *)o.validity;
             }
             runs[r]->cols[c] = dc;
         }
         runs[r]->bytes_h2d = r == 0 ? h2d : 0;
-        out_runs[r] = register_run(std::move(runs[r]));
+        out_runs[r] = g_runs.put(std::move(runs[r]));
     }
     if (info) {
         memset(info, 0, sizeof(*info));
@@ -1844,14 +1790,12 @@ struct PqReader {
     int launches = 0;
 };
 
-static std::mutex g_pq_mu;
-static std::unordered_map<uint64_t, std::unique_ptr<PqReader>> g_pq;
-static uint64_t g_pq_next = 1;
+static Table<PqReader> g_pq(5);
 
 // open = footer + schema check + a host walk of the page headers, so that files the device would refuse are refused
 // here, before any device work (and on a box without a GPU)
 static pg_status pq_open(uint64_t schema_h, const uint8_t *bytes, int64_t size, uint64_t *out) {
-    Schema *s = schema_from_handle(schema_h);
+    Schema *s = g_schemas.get(schema_h);
     if (!s || !bytes || !out) return fail(PG_ERR_INVALID, "bad schema handle or null argument");
     auto rd = std::make_unique<PqReader>();
     rd->own_schema = *s;
@@ -1908,10 +1852,7 @@ static pg_status pq_open(uint64_t schema_h, const uint8_t *bytes, int64_t size, 
     }
     if (row0 != m.num_rows) return fail(PG_ERR_FORMAT, "parquet: row group row counts do not add up");
     rd->file.assign(bytes, bytes + size);
-    std::lock_guard<std::mutex> lk(g_pq_mu);
-    uint64_t h = (5ull << 56) | g_pq_next++;
-    g_pq[h] = std::move(rd);
-    *out = h;
+    *out = g_pq.put(std::move(rd));
     return PG_OK;
 }
 
@@ -1970,45 +1911,27 @@ __global__ void k_dv_copy_bytes(const uint8_t *data, const int32_t *offs, const 
     for (int b = o0 + (threadIdx.x & 7); b < o1; b += 8) out[b] = s[b - o0];
 }
 
-Run *run_from_handle(uint64_t h);                          // api.cu
-
 static pg_status apply_deletion_vector(uint64_t run_h, const uint8_t *deleted, int64_t n_bits, uint64_t *out_run) {
-    Run *in = run_from_handle(run_h);
+    Run *in = g_runs.get(run_h);
     if (!in || !out_run || (n_bits > 0 && !deleted)) return fail(PG_ERR_INVALID, "unknown run handle or null argument");
-    pg_status st = require_device();
+    pg_status st = ensure_device();
     if (st) return st;
     const Schema *s = in->schema;
     const int nc = s->n_cols();
     const int64_t n = in->n_rows;
     if (n_bits < 0) return fail(PG_ERR_INVALID, "negative deletion vector size");
-    auto run = std::make_unique<Run>();
-    run->own_schema = *s;
-    run->schema = &run->own_schema;
-    run->cols.resize(nc);
-    run->varlen_bytes.assign(nc, 0);
-    run->varlen_base.assign(nc, 0);
-    auto pad = [](size_t b) { return (b + 255) & ~(size_t)255; };
     cudaStream_t sm = 0;
+    Scratch scratch(sm);                               // temporaries, and the new run until it is registered
+    auto dv_oom = [] { return fail(PG_ERR_CUDA, "deletion vector: out of device memory"); };
     // ---- kept rows
-    uint8_t *d_del = nullptr;
-    int32_t *d_incl = nullptr, *d_src = nullptr, *d_err = nullptr;
-    int64_t *d_sums = nullptr;
     const int64_t nb = std::max<int64_t>((n + 4095) / 4096, 1);
-    std::vector<void *> temps;
-    auto tmp = [&](size_t bytes, void **p) -> cudaError_t {
-        cudaError_t e = cudaMalloc(p, bytes ? bytes : 16);
-        if (e == cudaSuccess) temps.push_back(*p);
-        return e;
-    };
-    auto free_temps = [&]() { for (void *p : temps) cudaFree(p); };
-#define DV_CUDA(x) do { cudaError_t _e = (x); if (_e != cudaSuccess) { free_temps(); for (void *q : run->owned) cudaFree(q); \
-        return fail(PG_ERR_CUDA, std::string(#x) + ": " + cudaGetErrorString(_e)); } } while (0)
-    DV_CUDA(tmp((size_t)(n_bits + 7) / 8 + 16, (void **)&d_del));
-    DV_CUDA(tmp(sizeof(int32_t) * (size_t)(n + 1), (void **)&d_incl));
-    DV_CUDA(tmp(sizeof(int64_t) * (size_t)nb, (void **)&d_sums));
-    DV_CUDA(tmp(16, (void **)&d_err));
-    DV_CUDA(cudaMemsetAsync(d_err, 0, 4, sm));
-    if (n_bits > 0) DV_CUDA(cudaMemcpyAsync(d_del, deleted, (size_t)(n_bits + 7) / 8, cudaMemcpyHostToDevice, sm));
+    uint8_t *d_del = (uint8_t *)scratch.take((size_t)(n_bits + 7) / 8 + 16);
+    int32_t *d_incl = (int32_t *)scratch.take(sizeof(int32_t) * (size_t)(n + 1));
+    int64_t *d_sums = (int64_t *)scratch.take(sizeof(int64_t) * (size_t)nb);
+    int32_t *d_err = (int32_t *)scratch.take(16);
+    if (!d_del || !d_incl || !d_sums || !d_err) return dv_oom();
+    PG_CUDA(cudaMemsetAsync(d_err, 0, 4, sm));
+    if (n_bits > 0) PG_CUDA(cudaMemcpyAsync(d_del, deleted, (size_t)(n_bits + 7) / 8, cudaMemcpyHostToDevice, sm));
     int64_t m = 0;
     if (n > 0) {
         k_dv_keep<<<(int)((n + 255) / 256), 256, 0, sm>>>(d_del, n_bits, n, d_incl);
@@ -2016,25 +1939,27 @@ static pg_status apply_deletion_vector(uint64_t run_h, const uint8_t *deleted, i
         k_scan_block_prefix<<<1, 32, 0, sm>>>(d_sums, nb, d_err);
         k_scan_apply<<<(int)nb, 256, 0, sm>>>(d_incl, n, d_sums);
         int32_t last = 0;
-        DV_CUDA(cudaMemcpyAsync(&last, d_incl + n - 1, 4, cudaMemcpyDeviceToHost, sm));
-        DV_CUDA(cudaStreamSynchronize(sm));
+        PG_CUDA(cudaMemcpyAsync(&last, d_incl + n - 1, 4, cudaMemcpyDeviceToHost, sm));
+        PG_CUDA(cudaStreamSynchronize(sm));
         m = last;
     }
-    run->n_rows = m;
-    DV_CUDA(tmp(sizeof(int32_t) * (size_t)std::max<int64_t>(m, 1), (void **)&d_src));
+    scratch.runs.push_back(std::make_unique<Run>(*s, m));
+    Run *run = scratch.runs.back().get();
+    int32_t *d_src = (int32_t *)scratch.take(sizeof(int32_t) * (size_t)std::max<int64_t>(m, 1));
+    if (!d_src) return dv_oom();
     if (n > 0) k_dv_sources<<<(int)((n + 255) / 256), 256, 0, sm>>>(d_incl, n, d_src);
     // ---- one allocation for fixed-width data, offsets and validity; payloads follow once their sizes are known
     std::vector<size_t> o_data(nc), o_off(nc), o_val(nc);
     size_t total = 0;
     for (int c = 0; c < nc; c++) {
         pg_field f = s->field(c);
-        o_data[c] = total; total += is_varlen(f.type) ? 0 : pad((size_t)m * type_width(f.type) + 16);
-        o_off[c] = total; total += is_varlen(f.type) ? pad(sizeof(int32_t) * (size_t)(m + 1) + 16) : 0;
-        o_val[c] = total; total += in->cols[c].validity ? pad((size_t)((m + 31) / 32) * 4 + 16) : 0;
+        o_data[c] = total; total += is_varlen(f.type) ? 0 : align256((size_t)m * type_width(f.type) + 16);
+        o_off[c] = total; total += is_varlen(f.type) ? align256(sizeof(int32_t) * (size_t)(m + 1) + 16) : 0;
+        o_val[c] = total; total += in->cols[c].validity ? align256((size_t)((m + 31) / 32) * 4 + 16) : 0;
     }
-    unsigned char *base = nullptr;
-    DV_CUDA(cudaMalloc(&base, total + 256));
-    run->owned.push_back(base);
+    run->bufs.emplace_back(total + 256);
+    unsigned char *base = run->bufs.back().get();
+    if (!base) return dv_oom();
     const int gm = (int)((std::max<int64_t>(m, 1) + 255) / 256);
     std::vector<int64_t *> sums(nc, nullptr);
     for (int c = 0; c < nc; c++) {
@@ -2054,7 +1979,8 @@ static pg_status apply_deletion_vector(uint64_t run_h, const uint8_t *deleted, i
             k_dv_lengths<<<gm, 256, 0, sm>>>(ic.offsets, d_src, m, oo);
             if (m > 0) {
                 const int64_t mb = (m + 4095) / 4096;
-                DV_CUDA(tmp(sizeof(int64_t) * (size_t)mb, (void **)&sums[c]));
+                sums[c] = (int64_t *)scratch.take(sizeof(int64_t) * (size_t)mb);
+                if (!sums[c]) return dv_oom();
                 k_scan_block_sums<<<(int)mb, 256, 0, sm>>>(oo + 1, m, sums[c]);
                 k_scan_block_prefix<<<1, 32, 0, sm>>>(sums[c], mb, d_err);
                 k_scan_apply<<<(int)mb, 256, 0, sm>>>(oo + 1, m, sums[c]);
@@ -2066,14 +1992,18 @@ static pg_status apply_deletion_vector(uint64_t run_h, const uint8_t *deleted, i
     std::vector<int32_t> totals(nc, 0);
     for (int c = 0; c < nc; c++)
         if (is_varlen(s->field(c).type) && m > 0)
-            DV_CUDA(cudaMemcpyAsync(&totals[c], run->cols[c].offsets + m, 4, cudaMemcpyDeviceToHost, sm));
+            PG_CUDA(cudaMemcpyAsync(&totals[c], run->cols[c].offsets + m, 4, cudaMemcpyDeviceToHost, sm));
     int32_t herr = 0;
-    DV_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, sm));
-    DV_CUDA(cudaStreamSynchronize(sm));
+    PG_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, sm));
+    PG_CUDA(cudaStreamSynchronize(sm));
     size_t ptotal = 0;
-    for (int c = 0; c < nc; c++) if (is_varlen(s->field(c).type)) ptotal += pad((size_t)totals[c] + 64);
+    for (int c = 0; c < nc; c++) if (is_varlen(s->field(c).type)) ptotal += align256((size_t)totals[c] + 64);
     unsigned char *pl = nullptr;
-    if (ptotal) { DV_CUDA(cudaMalloc(&pl, ptotal)); run->owned.push_back(pl); }
+    if (ptotal) {
+        run->bufs.emplace_back(ptotal);
+        pl = run->bufs.back().get();
+        if (!pl) return dv_oom();
+    }
     size_t pt = 0;
     for (int c = 0; c < nc; c++) {
         if (!is_varlen(s->field(c).type)) continue;
@@ -2082,17 +2012,12 @@ static pg_status apply_deletion_vector(uint64_t run_h, const uint8_t *deleted, i
         if (m > 0)
             k_dv_copy_bytes<<<(int)((m * 8 + 255) / 256), 256, 0, sm>>>((const uint8_t *)in->cols[c].data, in->cols[c].offsets,
                                                                         d_src, run->cols[c].offsets, pl + pt, m);
-        pt += pad((size_t)totals[c] + 64);
+        pt += align256((size_t)totals[c] + 64);
     }
-    DV_CUDA(cudaStreamSynchronize(sm));
-    DV_CUDA(cudaGetLastError());
-    free_temps();
-#undef DV_CUDA
-    if (herr != KERR_NONE) {
-        for (void *q : run->owned) cudaFree(q);
-        return fail(PG_ERR_INTERNAL, "deletion vector: a var-len column exceeds 2 GiB of payload");
-    }
-    *out_run = register_run(std::move(run));
+    PG_CUDA(cudaStreamSynchronize(sm));
+    PG_CUDA(cudaGetLastError());
+    if (herr != KERR_NONE) return fail(PG_ERR_INTERNAL, "deletion vector: a var-len column exceeds 2 GiB of payload");
+    *out_run = g_runs.put(std::move(scratch.runs.back()));
     return PG_OK;
 }
 
@@ -2108,29 +2033,22 @@ pg_status pg_parquet_open(uint64_t schema, const uint8_t *file_bytes, int64_t si
 }
 
 pg_status pg_parquet_describe(uint64_t reader, pg_parquet_info *out) {
-    std::lock_guard<std::mutex> lk(g_pq_mu);
-    auto it = g_pq.find(reader);
-    if (it == g_pq.end() || !out) return fail(PG_ERR_INVALID, "unknown parquet reader handle");
-    PqReader *rd = it->second.get();
-    out->n_rows = rd->n_rows;
-    out->n_row_groups = (int32_t)rd->meta.row_groups.size();
-    out->n_columns = rd->schema->n_cols();
-    out->n_data_pages = rd->n_data_pages;
-    out->n_dictionary_pages = rd->n_dict_pages;
-    out->ms_decode = rd->ms_decode;
-    out->launches = rd->launches;
-    return PG_OK;
+    const bool known = out && g_pq.with(reader, [&](PqReader &rd) {
+        out->n_rows = rd.n_rows;
+        out->n_row_groups = (int32_t)rd.meta.row_groups.size();
+        out->n_columns = rd.schema->n_cols();
+        out->n_data_pages = rd.n_data_pages;
+        out->n_dictionary_pages = rd.n_dict_pages;
+        out->ms_decode = rd.ms_decode;
+        out->launches = rd.launches;
+    });
+    return known ? PG_OK : fail(PG_ERR_INVALID, "unknown parquet reader handle");
 }
 
 pg_status pg_parquet_read_run(uint64_t reader, uint64_t *out_run) {
-    PqReader *rd;
-    {
-        std::lock_guard<std::mutex> lk(g_pq_mu);
-        auto it = g_pq.find(reader);
-        if (it == g_pq.end() || !out_run) return fail(PG_ERR_INVALID, "unknown parquet reader handle");
-        rd = it->second.get();
-    }
-    pg_status st = require_device();          // fails loudly without pg_init / a CUDA device: no CPU fallback
+    PqReader *rd = g_pq.get(reader);
+    if (!rd || !out_run) return fail(PG_ERR_INVALID, "unknown parquet reader handle");
+    pg_status st = ensure_device();           // fails loudly without pg_init / a CUDA device: no CPU fallback
     if (st) return st;
     return pq_read_run(rd, out_run);
 }
@@ -2138,11 +2056,11 @@ pg_status pg_parquet_read_run(uint64_t reader, uint64_t *out_run) {
 pg_status pg_parquet_read_section(uint64_t schema, const pg_file_desc *files, int32_t n_files, int32_t n_runs,
                                   const char *const *column_names, const uint8_t *read_columns, uint64_t *out_runs,
                                   pg_section_info *info) {
-    Schema *s = schema_from_handle(schema);
+    Schema *s = g_schemas.get(schema);
     if (!s || !out_runs || n_files < 0 || n_runs < 0 || (n_files > 0 && !files))
         return fail(PG_ERR_INVALID, "bad schema handle or null argument");
     if (n_runs == 0) return n_files == 0 ? PG_OK : fail(PG_ERR_INVALID, "files without runs");
-    pg_status st = require_device();
+    pg_status st = ensure_device();
     if (st) return st;
     std::vector<SectionFile> fs(n_files);
     for (int i = 0; i < n_files; i++) {
@@ -2158,8 +2076,7 @@ pg_status pg_run_apply_deletion_vector(uint64_t run, const uint8_t *deleted_bitm
 }
 
 pg_status pg_parquet_free(uint64_t reader) {
-    std::lock_guard<std::mutex> lk(g_pq_mu);
-    return g_pq.erase(reader) ? PG_OK : fail(PG_ERR_INVALID, "unknown parquet reader handle");
+    return g_pq.take(reader) ? PG_OK : fail(PG_ERR_INVALID, "unknown parquet reader handle");
 }
 
 }  // extern "C"

@@ -16,9 +16,7 @@
 // Pages start at multiples of 8 rows, so a nullable column's definition levels (bit width 1, bit-packed LSB first)
 // ARE the bytes of the Arrow validity bitmap: they are copied, not re-encoded.  Values of non-null rows are
 // compacted by a block-wide scan; BYTE_ARRAY values are written as [len:int32][bytes].
-#include <map>
 #include <memory>
-#include <mutex>
 #include <string>
 
 #include "device_utils.cuh"
@@ -271,13 +269,7 @@ struct EncodedFile {
     bool image_complete = false;             // host_parts have been patched into d_file
     ~EncodedFile() { if (d_file) cudaFree(d_file); }
 };
-static std::mutex g_enc_mu;
-static std::map<uint64_t, std::unique_ptr<EncodedFile>> g_enc;
-static uint64_t g_enc_next = 1;
-
-// api.cu: the columns of a merge handle's current batch or of a run handle
-pg_status batch_columns(uint64_t handle, const Schema **schema, std::vector<DevColumn> *cols, int64_t *n_rows);
-pg_status require_device();
+static Table<EncodedFile> g_enc(6);
 
 static int parquet_type_of(int t) {
     switch (t) {
@@ -289,19 +281,10 @@ static int parquet_type_of(int t) {
         default: return pq::T_BYTE_ARRAY;
     }
 }
-static int type_width_enc(int t) {
-    switch (t) {
-        case PG_BOOL: case PG_INT8: return 1;
-        case PG_INT16: return 2;
-        case PG_INT32: case PG_FLOAT: return 4;
-        case PG_INT64: case PG_DOUBLE: return 8;
-        default: return 0;
-    }
-}
 
 static pg_status encode(uint64_t source, const char *const *names, int64_t row0, int64_t n_rows,
                         const pg_parquet_write_options *opt, uint64_t *out_file) {
-    pg_status st = require_device();
+    pg_status st = ensure_device();
     if (st) return st;
     const Schema *s = nullptr;
     std::vector<DevColumn> dcols;
@@ -322,7 +305,8 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     group_rows = ((group_rows + page_rows - 1) / page_rows) * page_rows;
     const int64_t n_groups = n_rows == 0 ? 0 : (n_rows + group_rows - 1) / group_rows;
 
-    cudaEvent_t e0, e1;
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    struct EvGuard { cudaEvent_t &a, &b; ~EvGuard() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); } } evg{e0, e1};
     PG_CUDA(cudaEventCreate(&e0));
     PG_CUDA(cudaEventCreate(&e1));
     PG_CUDA(cudaEventRecord(e0, 0));
@@ -330,7 +314,7 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     std::vector<EncColumn> cols(nc);
     for (int c = 0; c < nc; c++) {
         pg_field f = s->field(c);
-        cols[c] = EncColumn{dcols[c].data, dcols[c].offsets, dcols[c].validity, f.type, type_width_enc(f.type),
+        cols[c] = EncColumn{dcols[c].data, dcols[c].offsets, dcols[c].validity, f.type, type_width(f.type),
                             (f.nullable || dcols[c].validity) ? 1 : 0, 0};
     }
     // jobs: row group major, column, page
@@ -345,22 +329,15 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         }
     }
     const size_t nj = jobs.size(), nsj = sjobs.size();
-    EncColumn *d_cols = nullptr;
-    EncJob *d_jobs = nullptr;
-    StatJob *d_sjobs = nullptr;
-    int64_t *d_counts = nullptr, *d_stats = nullptr;
     std::vector<int64_t> counts(2 * nj + 2), stats(4 * nsj + 4);
-    // temporaries are released on every path out of this function (PG_CUDA returns early)
-    struct Guard {
-        EncColumn *&a; EncJob *&b; StatJob *&c; int64_t *&d; int64_t *&e; cudaEvent_t &e0; cudaEvent_t &e1;
-        ~Guard() { cudaFree(a); cudaFree(b); cudaFree(c); cudaFree(d); cudaFree(e); cudaEventDestroy(e0); cudaEventDestroy(e1); }
-    } guard{d_cols, d_jobs, d_sjobs, d_counts, d_stats, e0, e1};
-    auto cleanup = []() {};
-    PG_CUDA(cudaMalloc(&d_cols, sizeof(EncColumn) * nc));
-    PG_CUDA(cudaMalloc(&d_jobs, sizeof(EncJob) * std::max<size_t>(nj, 1)));
-    PG_CUDA(cudaMalloc(&d_sjobs, sizeof(StatJob) * std::max<size_t>(nsj, 1)));
-    PG_CUDA(cudaMalloc(&d_counts, sizeof(int64_t) * (2 * nj + 2)));
-    PG_CUDA(cudaMalloc(&d_stats, sizeof(int64_t) * (4 * nsj + 4)));
+    Scratch scratch(0);                                      // temporaries, released on every path out of this function
+    EncColumn *d_cols = (EncColumn *)scratch.take(sizeof(EncColumn) * nc);
+    EncJob *d_jobs = (EncJob *)scratch.take(sizeof(EncJob) * std::max<size_t>(nj, 1));
+    StatJob *d_sjobs = (StatJob *)scratch.take(sizeof(StatJob) * std::max<size_t>(nsj, 1));
+    int64_t *d_counts = (int64_t *)scratch.take(sizeof(int64_t) * (2 * nj + 2));
+    int64_t *d_stats = (int64_t *)scratch.take(sizeof(int64_t) * (4 * nsj + 4));
+    if (!d_cols || !d_jobs || !d_sjobs || !d_counts || !d_stats)
+        return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the page tables");
     PG_CUDA(cudaMemcpy(d_cols, cols.data(), sizeof(EncColumn) * nc, cudaMemcpyHostToDevice));
     int launches = 0;
     if (nj) {
@@ -427,7 +404,7 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
             else if (ec.type == PG_BOOL) val_bytes = (nn + 7) / 8;
             else val_bytes = nn * (ec.width == 8 ? 8 : 4);
             const int64_t body = def_bytes + val_bytes;
-            if (body > 0x7fffffffLL) { cleanup(); return fail(PG_ERR_UNSUPPORTED, "parquet encode: page larger than 2 GiB"); }
+            if (body > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet encode: page larger than 2 GiB");
             ThriftWriter ph;                                   // PageHeader
             ph.i32(1, pq::P_DATA);
             ph.i32(2, (int32_t)body);
@@ -539,7 +516,7 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     float ms = 0;
     cudaEventElapsedTime(&ms, e0, e1);
     cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) { cleanup(); return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(le)); }
+    if (le != cudaSuccess) return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(le));
 
     ef->meta.n_rows = n_rows;
     ef->meta.file_bytes = ef->file_bytes;
@@ -550,11 +527,7 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     const ColStats &sq = ef->stats[s->n_key];
     ef->meta.min_sequence_number = sq.has_minmax ? sq.min : 0;
     ef->meta.max_sequence_number = sq.has_minmax ? sq.max : 0;
-    cleanup();
-    std::lock_guard<std::mutex> lk(g_enc_mu);
-    uint64_t h = (6ull << 56) | g_enc_next++;
-    g_enc[h] = std::move(ef);
-    *out_file = h;
+    *out_file = g_enc.put(std::move(ef));
     return PG_OK;
 }
 
@@ -571,37 +544,32 @@ pg_status pg_parquet_encode(uint64_t source, const char *const *column_names, in
 }
 
 pg_status pg_parquet_file_meta(uint64_t file, pg_file_meta *out) {
-    std::lock_guard<std::mutex> lk(g_enc_mu);
-    auto it = g_enc.find(file);
-    if (it == g_enc.end() || !out) return fail(PG_ERR_INVALID, "unknown encoded file handle");
-    *out = it->second->meta;
-    return PG_OK;
+    const bool known = out && g_enc.with(file, [&](EncodedFile &ef) { *out = ef.meta; });
+    return known ? PG_OK : fail(PG_ERR_INVALID, "unknown encoded file handle");
 }
 
 pg_status pg_parquet_file_column_stats(uint64_t file, int32_t column, int64_t *null_count, int32_t *has_min_max,
                                        void *min8, void *max8) {
-    std::lock_guard<std::mutex> lk(g_enc_mu);
-    auto it = g_enc.find(file);
-    if (it == g_enc.end()) return fail(PG_ERR_INVALID, "unknown encoded file handle");
-    if (column < 0 || column >= (int32_t)it->second->stats.size()) return fail(PG_ERR_INVALID, "column out of range");
-    const ColStats &st = it->second->stats[column];
-    if (null_count) *null_count = st.null_count;
-    if (has_min_max) *has_min_max = st.has_minmax;
-    if (min8) memcpy(min8, &st.min, 8);
-    if (max8) memcpy(max8, &st.max, 8);
-    return PG_OK;
+    pg_status st = PG_OK;
+    const bool known = g_enc.with(file, [&](EncodedFile &ef) {
+        if (column < 0 || column >= (int32_t)ef.stats.size()) {
+            st = fail(PG_ERR_INVALID, "column out of range");
+            return;
+        }
+        const ColStats &cs = ef.stats[column];
+        if (null_count) *null_count = cs.null_count;
+        if (has_min_max) *has_min_max = cs.has_minmax;
+        if (min8) memcpy(min8, &cs.min, 8);
+        if (max8) memcpy(max8, &cs.max, 8);
+    });
+    return known ? st : fail(PG_ERR_INVALID, "unknown encoded file handle");
 }
 
 pg_status pg_parquet_file_fetch(uint64_t file, void *host_buffer, int64_t capacity) {
-    EncodedFile *ef;
-    {
-        std::lock_guard<std::mutex> lk(g_enc_mu);
-        auto it = g_enc.find(file);
-        if (it == g_enc.end() || !host_buffer) return fail(PG_ERR_INVALID, "unknown encoded file handle");
-        ef = it->second.get();
-    }
+    EncodedFile *ef = g_enc.get(file);
+    if (!ef || !host_buffer) return fail(PG_ERR_INVALID, "unknown encoded file handle");
     if (capacity < ef->file_bytes) return fail(PG_ERR_INVALID, "buffer smaller than the file");
-    pg_status st = require_device();
+    pg_status st = ensure_device();
     if (st) return st;
     const auto &tail = ef->host_parts.back();
     PG_CUDA(cudaMemcpy(host_buffer, ef->d_file, (size_t)tail.first, cudaMemcpyDeviceToHost));
@@ -610,14 +578,9 @@ pg_status pg_parquet_file_fetch(uint64_t file, void *host_buffer, int64_t capaci
 }
 
 pg_status pg_parquet_file_device_image(uint64_t file, const uint8_t **device_bytes, int64_t *size) {
-    EncodedFile *ef;
-    {
-        std::lock_guard<std::mutex> lk(g_enc_mu);
-        auto it = g_enc.find(file);
-        if (it == g_enc.end() || !device_bytes || !size) return fail(PG_ERR_INVALID, "unknown encoded file handle");
-        ef = it->second.get();
-    }
-    pg_status st = require_device();
+    EncodedFile *ef = g_enc.get(file);
+    if (!ef || !device_bytes || !size) return fail(PG_ERR_INVALID, "unknown encoded file handle");
+    pg_status st = ensure_device();
     if (st) return st;
     if (!ef->image_complete) {
         std::vector<PatchJob> jobs;
@@ -627,17 +590,14 @@ pg_status pg_parquet_file_device_image(uint64_t file, const uint8_t **device_byt
             jobs.push_back(PatchJob{p.first, (int32_t)bytes.size(), (int32_t)p.second.size()});
             bytes.insert(bytes.end(), p.second.begin(), p.second.end());
         }
-        PatchJob *d_jobs = nullptr;
-        uint8_t *d_bytes = nullptr;
-        PG_CUDA(cudaMalloc(&d_jobs, sizeof(PatchJob) * jobs.size() + 16));
-        cudaError_t e = cudaMalloc(&d_bytes, bytes.size() + 16);
-        if (e != cudaSuccess) { cudaFree(d_jobs); return fail(PG_ERR_CUDA, cudaGetErrorString(e)); }
-        cudaMemcpy(d_jobs, jobs.data(), sizeof(PatchJob) * jobs.size(), cudaMemcpyHostToDevice);
-        cudaMemcpy(d_bytes, bytes.data(), bytes.size(), cudaMemcpyHostToDevice);
+        Scratch scratch(0);
+        PatchJob *d_jobs = (PatchJob *)scratch.take(sizeof(PatchJob) * jobs.size() + 16);
+        uint8_t *d_bytes = (uint8_t *)scratch.take(bytes.size() + 16);
+        if (!d_jobs || !d_bytes) return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the header patch");
+        PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(PatchJob) * jobs.size(), cudaMemcpyHostToDevice));
+        PG_CUDA(cudaMemcpy(d_bytes, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
         k_pw_patch<<<(unsigned)((jobs.size() * 32 + 127) / 128), 128>>>(d_jobs, (int)jobs.size(), d_bytes, ef->d_file);
-        e = cudaDeviceSynchronize();
-        cudaFree(d_jobs);
-        cudaFree(d_bytes);
+        cudaError_t e = cudaDeviceSynchronize();
         if (e != cudaSuccess) return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(e));
         ef->image_complete = true;
     }
@@ -647,8 +607,7 @@ pg_status pg_parquet_file_device_image(uint64_t file, const uint8_t **device_byt
 }
 
 pg_status pg_parquet_file_free(uint64_t file) {
-    std::lock_guard<std::mutex> lk(g_enc_mu);
-    return g_enc.erase(file) ? PG_OK : fail(PG_ERR_INVALID, "unknown encoded file handle");
+    return g_enc.take(file) ? PG_OK : fail(PG_ERR_INVALID, "unknown encoded file handle");
 }
 
 }  // extern "C"

@@ -4,7 +4,11 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <memory>
+#include <mutex>
 #include <string>
+#include <unordered_map>
+#include <utility>
 #include <vector>
 
 #include "paimon_gpu.h"
@@ -78,17 +82,124 @@ struct DevColumn {
     const uint8_t *validity = nullptr;
 };
 
+// ---- recycled device buffers (api.cu): a reader that streams a bucket through the device opens and frees runs at a
+// high rate, and cudaMalloc / cudaFree would serialise the pipeline.  Runs, uploads and the temporaries of a decode, a
+// deletion vector or an encode come from this cache; only the merge handles' arenas and descriptors and an encoded
+// file's image are allocated directly.
+void *buf_take(size_t bytes, size_t *got);     // NULL when the device is out of memory (after trimming the cache)
+void buf_give(void *p, size_t bytes);
+
+// One buffer from the cache (pointer and granted size), given back when destroyed.  The owner guarantees that no
+// queued work still touches it by then (see Scratch).
+class DeviceBuffer {
+ public:
+    DeviceBuffer() = default;
+    explicit DeviceBuffer(size_t bytes) { p_ = buf_take(bytes, &n_); }
+    DeviceBuffer(DeviceBuffer &&o) noexcept : p_(o.p_), n_(o.n_) { o.p_ = nullptr; o.n_ = 0; }
+    DeviceBuffer &operator=(DeviceBuffer &&o) noexcept {
+        std::swap(p_, o.p_);
+        std::swap(n_, o.n_);
+        return *this;
+    }
+    DeviceBuffer(const DeviceBuffer &) = delete;
+    DeviceBuffer &operator=(const DeviceBuffer &) = delete;
+    ~DeviceBuffer() { if (p_) buf_give(p_, n_); }
+    unsigned char *get() const { return (unsigned char *)p_; }
+    explicit operator bool() const { return p_ != nullptr; }
+
+ private:
+    void *p_ = nullptr;
+    size_t n_ = 0;
+};
+
+inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
+
 struct Run {
-    const Schema *schema = nullptr;
+    Run(const Schema &s, int64_t rows)
+        : schema(&own_schema), own_schema(s), n_rows(rows), cols(s.n_cols()), varlen_bytes(s.n_cols(), 0),
+          varlen_base(s.n_cols(), 0) {}
+    Run(const Run &) = delete;
+    Run &operator=(const Run &) = delete;
+    const Schema *schema;
     Schema own_schema;                   // copy: a run may outlive the schema handle it was opened with
-    int64_t n_rows = 0;
+    int64_t n_rows;
     std::vector<DevColumn> cols;
     std::vector<int64_t> varlen_bytes;   // per column: payload bytes of a var-len column (offsets[n_rows] - offsets[0])
     std::vector<int64_t> varlen_base;    // per column: offsets[0] (data points at byte 0 of the offsets' space)
-    std::vector<size_t> owned_bytes;     // sizes of `owned`
-    std::vector<void *> owned;           // device allocations made by pg_run_open(PG_MEM_HOST)
+    std::vector<DeviceBuffer> bufs;      // device memory the run owns (none for device-memory runs and slices)
     int64_t bytes_h2d = 0;
 };
+
+// The device buffers of one call: its temporaries, and what it builds (runs, uploads) until that is registered under a
+// handle.
+// Ordering invariant: no buffer goes back to the cache while work queued on `stream` may still touch it.  The destructor
+// synchronises the stream before the members release anything, so every early return is safe whatever was queued.  A
+// call that builds runs keeps them in `runs` until it registers them, so the run buffers a failed call drops are
+// covered by the same synchronisation.
+struct Scratch {
+    explicit Scratch(cudaStream_t s) : stream(s) {}
+    ~Scratch() { if (!bufs.empty() || !runs.empty()) cudaStreamSynchronize(stream); }
+    void *take(size_t bytes) {                     // NULL when the device is out of memory
+        DeviceBuffer b(bytes ? bytes : 256);
+        if (!b) return nullptr;
+        bufs.push_back(std::move(b));
+        return bufs.back().get();
+    }
+    cudaStream_t stream;
+    std::vector<DeviceBuffer> bufs;
+    std::vector<std::unique_ptr<Run>> runs;
+};
+
+// ---- handle tables: one per handle kind.  A handle carries its kind's tag in the top byte (1 schema, 2 merge spec,
+// 3 run, 4 merge; 5 Parquet reader, 6 encoded Parquet file, 7 upload), so a handle of one kind is never found by
+// another kind's entry points.
+template <typename T>
+class Table {
+ public:
+    explicit Table(uint64_t tag) : tag_(tag << 56) {}
+    uint64_t put(std::unique_ptr<T> p) {
+        std::lock_guard<std::mutex> g(mu_);
+        const uint64_t h = tag_ | next_++;
+        map_[h] = std::move(p);
+        return h;
+    }
+    T *get(uint64_t h) {
+        std::lock_guard<std::mutex> g(mu_);
+        auto it = map_.find(h);
+        return it == map_.end() ? nullptr : it->second.get();
+    }
+    // fn(T &) with the table locked, so that a concurrent take() cannot free the object meanwhile; false = unknown
+    template <typename F>
+    bool with(uint64_t h, F &&fn) {
+        std::lock_guard<std::mutex> g(mu_);
+        auto it = map_.find(h);
+        if (it == map_.end()) return false;
+        fn(*it->second);
+        return true;
+    }
+    std::unique_ptr<T> take(uint64_t h) {
+        std::lock_guard<std::mutex> g(mu_);
+        auto it = map_.find(h);
+        if (it == map_.end()) return nullptr;
+        std::unique_ptr<T> p = std::move(it->second);
+        map_.erase(it);
+        return p;
+    }
+
+ private:
+    std::mutex mu_;
+    std::unordered_map<uint64_t, std::unique_ptr<T>> map_;
+    uint64_t next_ = 1;
+    const uint64_t tag_;
+};
+extern Table<Schema> g_schemas;      // api.cu
+extern Table<Run> g_runs;
+
+// ---- the rest of api.cu that the format readers and writers use
+pg_status ensure_device();           // pg_init has been called; binds the calling thread to the device
+cudaStream_t copy_stream();          // the calling thread's non-blocking stream
+// the columns of a merge handle's current batch, or of a run
+pg_status batch_columns(uint64_t handle, const Schema **schema, std::vector<DevColumn> *cols, int64_t *n_rows);
 
 // ---- device-side descriptors (copied to device memory once per merge handle) ----
 

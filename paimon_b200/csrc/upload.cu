@@ -9,34 +9,22 @@
 // the copy synchronous and staged by the driver).
 #include <memory>
 #include <mutex>
-#include <unordered_map>
 #include <vector>
 
 #include "pg_internal.h"
 
 namespace pg {
-
-void *device_buffer_take(size_t bytes, size_t *got);    // api.cu: recycled device buffers
-void device_buffer_give(void *p, size_t bytes);
-cudaStream_t thread_stream();
-pg_status require_device();
-
 namespace {
 
 struct Upload {
-    std::vector<void *> bufs;
-    std::vector<size_t> got;
+    std::vector<DeviceBuffer> bufs;
     std::vector<pg_file_desc> files;
     cudaEvent_t done = nullptr;
-    ~Upload() {
-        if (done) cudaEventDestroy(done);
-        for (size_t i = 0; i < bufs.size(); i++) if (bufs[i]) device_buffer_give(bufs[i], got[i]);
-    }
+    ~Upload() { if (done) cudaEventDestroy(done); }
 };
 
-std::mutex g_up_mu;
-std::unordered_map<uint64_t, std::unique_ptr<Upload>> g_up;
-uint64_t g_up_next = 1;
+Table<Upload> g_up(7);
+std::mutex g_up_mu;                                    // creation of the upload stream
 cudaStream_t g_up_stream = nullptr;
 
 }  // namespace
@@ -46,7 +34,7 @@ using namespace pg;
 
 extern "C" pg_status pg_files_upload_begin(const pg_file_desc *files, int32_t n_files, uint64_t *out_upload) {
     if (!out_upload || n_files < 0 || (n_files > 0 && !files)) return fail(PG_ERR_INVALID, "null argument");
-    pg_status st = require_device();
+    pg_status st = ensure_device();
     if (st) return st;
     auto up = std::make_unique<Upload>();
     {
@@ -54,15 +42,13 @@ extern "C" pg_status pg_files_upload_begin(const pg_file_desc *files, int32_t n_
         if (!g_up_stream) PG_CUDA(cudaStreamCreateWithFlags(&g_up_stream, cudaStreamNonBlocking));
     }
     PG_CUDA(cudaEventCreateWithFlags(&up->done, cudaEventDisableTiming));
+    Scratch scratch(g_up_stream);                      // the buffers until the upload is registered
     for (int i = 0; i < n_files; i++) {
         if (files[i].size < 0 || (files[i].size > 0 && !files[i].bytes)) return fail(PG_ERR_INVALID, "upload: bad file descriptor");
         pg_file_desc d = files[i];
         if (files[i].mem == PG_MEM_HOST) {
-            size_t got = 0;
-            void *b = device_buffer_take((size_t)files[i].size + 64, &got);       // (readers may look 8 bytes past a page)
+            void *b = scratch.take((size_t)files[i].size + 64);                    // (readers may look 8 bytes past a page)
             if (!b) return fail(PG_ERR_CUDA, "upload: out of device memory (" + std::to_string(files[i].size) + " bytes)");
-            up->bufs.push_back(b);
-            up->got.push_back(got);
             PG_CUDA(cudaMemcpyAsync(b, files[i].bytes, (size_t)files[i].size, cudaMemcpyHostToDevice, g_up_stream));
             d.bytes = (const uint8_t *)b;
             d.mem = PG_MEM_DEVICE;
@@ -70,21 +56,14 @@ extern "C" pg_status pg_files_upload_begin(const pg_file_desc *files, int32_t n_
         up->files.push_back(d);
     }
     PG_CUDA(cudaEventRecord(up->done, g_up_stream));
-    std::lock_guard<std::mutex> lk(g_up_mu);
-    const uint64_t h = ((uint64_t)7 << 56) | g_up_next++;
-    g_up.emplace(h, std::move(up));
-    *out_upload = h;
+    up->bufs.swap(scratch.bufs);
+    *out_upload = g_up.put(std::move(up));
     return PG_OK;
 }
 
 extern "C" pg_status pg_files_upload_wait(uint64_t upload, pg_file_desc *out_files, int32_t n_files) {
-    Upload *up;
-    {
-        std::lock_guard<std::mutex> lk(g_up_mu);
-        auto it = g_up.find(upload);
-        if (it == g_up.end()) return fail(PG_ERR_INVALID, "unknown upload handle");
-        up = it->second.get();
-    }
+    Upload *up = g_up.get(upload);
+    if (!up) return fail(PG_ERR_INVALID, "unknown upload handle");
     if (n_files != (int32_t)up->files.size() || (n_files > 0 && !out_files)) return fail(PG_ERR_INVALID, "upload: one descriptor per file");
     PG_CUDA(cudaEventSynchronize(up->done));
     for (int i = 0; i < n_files; i++) out_files[i] = up->files[i];
@@ -92,17 +71,11 @@ extern "C" pg_status pg_files_upload_wait(uint64_t upload, pg_file_desc *out_fil
 }
 
 extern "C" pg_status pg_files_upload_free(uint64_t upload) {
-    std::unique_ptr<Upload> up;
-    {
-        std::lock_guard<std::mutex> lk(g_up_mu);
-        auto it = g_up.find(upload);
-        if (it == g_up.end()) return fail(PG_ERR_INVALID, "unknown upload handle");
-        up = std::move(it->second);
-        g_up.erase(it);
-    }
+    std::unique_ptr<Upload> up = g_up.take(upload);
+    if (!up) return fail(PG_ERR_INVALID, "unknown upload handle");
     // the copy itself, and the decode launches of the calling thread that read the bytes, must be done before the
     // buffers go back to the cache
     cudaEventSynchronize(up->done);
-    cudaStreamSynchronize(thread_stream());
+    cudaStreamSynchronize(copy_stream());
     return PG_OK;
 }

@@ -48,6 +48,61 @@ def test_handle_validation_without_device():
     assert lib.pg_merge_execute(999) == 1
     assert b"unknown" in lib.pg_last_error()
 
+    # every handle kind (tag in the top byte: 1 schema ... 7 upload) refuses a handle it never issued
+    n_rows = C.c_int64(0)
+    entry_points = {
+        1: [lambda h: lib.pg_schema_free(h), lambda h: lib.pg_schema_info(h, None, None)],
+        2: [lambda h: lib.pg_merge_spec_free(h)],
+        3: [lambda h: lib.pg_run_free(h), lambda h: lib.pg_run_layout(h, C.byref(n_rows), None, None, 0)],
+        4: [lambda h: lib.pg_merge_free(h), lambda h: lib.pg_merge_stats(h, C.byref(N.PgStats()))],
+        5: [lambda h: lib.pg_parquet_free(h), lambda h: lib.pg_parquet_describe(h, C.byref(N.PgParquetInfo()))],
+        6: [lambda h: lib.pg_parquet_file_free(h), lambda h: lib.pg_parquet_file_meta(h, C.byref(N.PgFileMeta()))],
+        7: [lambda h: lib.pg_files_upload_free(h), lambda h: lib.pg_files_upload_wait(h, None, 0)],
+    }
+    for tag, calls in entry_points.items():
+        for call in calls:
+            for h in (12345, (tag << 56) | 12345):
+                assert call(h) == 1, (tag, h)
+                assert b"unknown" in lib.pg_last_error(), (tag, h)
+
+    # the kinds a host can create without a device carry their own tag, are refused by every other kind's free
+    # function, and survive it
+    import numpy as np
+    import pyarrow as pa
+    import pyarrow.parquet as pq
+    field = N.PgField(4, 0)                                # PG_INT64
+    desc = N.PgSchemaDesc(1, 0, C.pointer(field), None)
+    schema, spec, reader = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+    assert lib.pg_schema_create(C.byref(desc), C.byref(schema)) == 0
+    assert lib.pg_merge_spec_create(schema.value, C.byref(N.PgMergeSpec()), C.byref(spec)) == 0
+    sink = pa.BufferOutputStream()                         # [_KEY_k, _SEQUENCE_NUMBER, _VALUE_KIND], 3 rows
+    pq.write_table(pa.table({"_KEY_k": pa.array([1, 2, 3], pa.int64()), "_SEQUENCE_NUMBER": pa.array([1, 2, 3], pa.int64()),
+                             "_VALUE_KIND": pa.array([0, 0, 0], pa.int8())}),
+                   sink, compression="none", use_dictionary=False, data_page_version="1.0")
+    file_bytes = np.frombuffer(sink.getvalue().to_pybytes(), np.uint8)
+    assert lib.pg_parquet_open(schema.value, file_bytes.ctypes.data, len(file_bytes), C.byref(reader)) == 0, \
+        lib.pg_last_error()
+
+    n_key, n_val = C.c_int32(-1), C.c_int32(-1)
+    info = N.PgParquetInfo()
+    frees = {1: lib.pg_schema_free, 2: lib.pg_merge_spec_free, 3: lib.pg_run_free, 4: lib.pg_merge_free,
+             5: lib.pg_parquet_free, 6: lib.pg_parquet_file_free, 7: lib.pg_files_upload_free}
+    live = [(1, schema.value, lambda: lib.pg_schema_info(schema.value, C.byref(n_key), C.byref(n_val)) == 0),
+            (2, spec.value, None),
+            (5, reader.value, lambda: lib.pg_parquet_describe(reader.value, C.byref(info)) == 0 and info.n_rows == 3)]
+    for tag, h, alive in live:
+        assert h >> 56 == tag
+        for other, free in frees.items():
+            if other == tag:
+                continue
+            assert free(h) == 1, (tag, other)
+            assert b"unknown" in lib.pg_last_error()
+            assert alive is None or alive(), (tag, other)
+    assert (n_key.value, n_val.value) == (1, 0)
+    for tag, h, _ in reversed(live):
+        assert frees[tag](h) == 0, tag
+        assert frees[tag](h) == 1, tag                     # freed once
+
 
 def test_interval_partition_host_logic_matches_oracle():
     import random

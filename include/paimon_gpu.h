@@ -120,6 +120,10 @@ typedef struct {
      * buffers for them (pg_parquet_read_section's read_columns), except for fields the merge itself compares
      * ('sequence.field', sequence-group fields: PartialUpdateMergeFunction.adjustReadType :576-606 keeps those) */
     const uint8_t *read_fields;         /* [n_val]; NULL = every field */
+    /* DECIMAL value fields (unscaled INT64 columns): sum / product follow the reference's DECIMAL rules (FieldSumAgg /
+     * FieldProductAgg on DecimalType: NULL on int64 overflow or when a product / quotient has more than p digits,
+     * HALF_UP rescaling, exact division on retract) instead of wrapping int64 arithmetic.  precision 1..18. */
+    const int32_t *decimal;             /* [n_val] precision << 8 | scale, 0 = not DECIMAL; NULL = none */
 } pg_merge_spec;
 
 /* one column, Arrow buffer layout */

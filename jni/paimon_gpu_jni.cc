@@ -108,13 +108,14 @@ JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_mergeSpecCreate(
     JNIEnv *env, jclass, jlong schema, jint engine, jboolean ignoreDelete, jboolean removeRecordOnDelete,
     jboolean dropDelete, jintArray seqFields, jboolean seqAscending, jintArray agg, jbooleanArray ignoreRetract,
     jintArray groupSeqStart, jintArray groupSeqFields, jintArray fieldGroup, jbooleanArray groupPartialDelete,
-    jbooleanArray readFields) {
+    jbooleanArray readFields, jintArray decimal) {
     // every per-field array has one entry per VALUE field of the schema (pg_merge_spec_create reads n_val entries)
     int32_t n_key = 0, n_val = 0;
     PG_CHECK(pg_schema_info((uint64_t)schema, &n_key, &n_val));
     const jsize nv = n_val;
     auto bad_len = [&](jarray a) { return a != nullptr && env->GetArrayLength(a) != nv; };
-    if (bad_len(agg) || bad_len(ignoreRetract) || bad_len(fieldGroup) || bad_len(groupPartialDelete) || bad_len(readFields)) {
+    if (bad_len(agg) || bad_len(ignoreRetract) || bad_len(fieldGroup) || bad_len(groupPartialDelete) || bad_len(readFields) ||
+        bad_len(decimal)) {
         env->ThrowNew(env->FindClass("java/lang/IllegalArgumentException"),
                       "per-field arrays must have one entry per value field of the schema");
         return 0;
@@ -164,6 +165,13 @@ JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_mergeSpecCreate(
         if (nv) env->GetBooleanArrayRegion(readFields, 0, nv, rf.data());
         rf8.assign(rf.begin(), rf.end());
         sp.read_fields = rf8.data();
+    }
+    // DECIMAL value fields: precision << 8 | scale, 0 for other types; null = no DECIMAL field
+    std::vector<jint> dec;
+    if (decimal && nv) {
+        dec.resize(nv);
+        env->GetIntArrayRegion(decimal, 0, nv, dec.data());
+        sp.decimal = dec.data();
     }
     uint64_t h = 0;
     PG_CHECK(pg_merge_spec_create((uint64_t)schema, &sp, &h));

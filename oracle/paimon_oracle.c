@@ -471,6 +471,60 @@ static int cmp_internal_row_utils(int type, const po_val *a, const po_val *b, in
     }
 }
 
+/* ---- DECIMAL(p, s) sum / product on unscaled int64 values (p <= 18)
+ * sum / subtract: DecimalUtils.add / subtract (paimon-common/.../utils/DecimalUtils.java:52-87): exact int64; on
+ *   overflow the BigDecimal result has more than 18 digits and Decimal.fromBigDecimal returns NULL; a result over p
+ *   digits that fits int64 is kept (fromUnscaledLong does not check the precision).
+ * product: round_half_up(a * b / 10^s), NULL over p digits (FieldProductAgg.java:47-58, Decimal.java:182-193).
+ * product retract: BigDecimal.divide is exact: it throws on a zero divisor and when the quotient does not terminate;
+ *   otherwise round_half_up(a * 10^s / b), NULL over p digits (FieldProductAgg.java:95-106).
+ * sum retract into a NULL accumulator: negative() = fromBigDecimal(-a), NULL over p digits (FieldSumAgg.java:140-143).
+ * |a|, |b| <= 2^63 and 10^s <= 10^18, so a * b and a * 10^s fit __int128. */
+static int field_decimal(const mf_t *m, int f) {
+    return m->c->spec->decimal ? m->c->spec->decimal[f] : 0;
+}
+static unsigned __int128 dec_pow10(int e) {
+    unsigned __int128 r = 1;
+    while (e-- > 0) r *= 10u;
+    return r;
+}
+static unsigned __int128 dec_abs(__int128 v) { return v < 0 ? (unsigned __int128)0 - (unsigned __int128)v : (unsigned __int128)v; }
+static __int128 dec_div_half_up(__int128 n, unsigned __int128 d) {       /* d > 0; RoundingMode.HALF_UP */
+    unsigned __int128 m = dec_abs(n), q = m / d, r = m - q * d;
+    if (r >= d - r) q += 1;
+    return n < 0 ? -(__int128)q : (__int128)q;
+}
+/* out := the DECIMAL r, or NULL when it has more than p digits */
+static void dec_set(po_val *out, __int128 r, int precision) {
+    if (dec_abs(r) >= dec_pow10(precision)) { memset(out, 0, sizeof(*out)); out->is_null = 1; }
+    else { out->is_null = 0; out->v.i = (int64_t)r; }
+}
+/* fn: 0 add, 1 subtract, 2 multiply, 3 divide, 4 negate a.  Returns -1 when BigDecimal would have thrown. */
+static int dec_arith(int decimal, int fn, int64_t a, int64_t b, po_val *out) {
+    const int precision = decimal >> 8, scale = decimal & 0xff;
+    if (fn == 0 || fn == 1) {
+        int64_t r;
+        int overflow = fn == 0 ? __builtin_add_overflow(a, b, &r) : __builtin_sub_overflow(a, b, &r);
+        if (overflow) { memset(out, 0, sizeof(*out)); out->is_null = 1; }
+        else { out->is_null = 0; out->v.i = r; }
+        return 0;
+    }
+    if (fn == 4) { dec_set(out, -(__int128)a, precision); return 0; }
+    if (fn == 2) { dec_set(out, dec_div_half_up((__int128)a * b, dec_pow10(scale)), precision); return 0; }
+    if (b == 0) return fail(a == 0 ? "ArithmeticException: Division undefined" : "ArithmeticException: Division by zero");
+    /* a / b terminates iff b / gcd(a, b) has no prime factor other than 2 and 5 */
+    uint64_t x = (uint64_t)dec_abs(a), y = (uint64_t)dec_abs(b);
+    while (x != 0) { uint64_t t = y % x; y = x; x = t; }
+    uint64_t den = (uint64_t)dec_abs(b) / y;
+    while (den % 2 == 0) den /= 2;
+    while (den % 5 == 0) den /= 5;
+    if (den != 1)
+        return fail("ArithmeticException: Non-terminating decimal expansion; no exact representable decimal result.");
+    __int128 n = (__int128)a * (__int128)dec_pow10(scale);
+    dec_set(out, dec_div_half_up(b < 0 ? -n : n, dec_abs(b)), precision);
+    return 0;
+}
+
 /* FieldAggregator.agg for the fixed-width aggregators (files listed in the header) */
 static int agg_apply(mf_t *m, int f, int agg, const po_val *acc, const po_val *in, po_val *out) {
     int type = m->c->s->val_types[f];
@@ -479,6 +533,7 @@ static int agg_apply(mf_t *m, int f, int agg, const po_val *acc, const po_val *i
         case PO_AGG_SUM: case PO_AGG_PRODUCT:       /* FieldSumAgg.java:41-84, FieldProductAgg */
             if (acc->is_null || in->is_null) { *out = acc->is_null ? *in : *acc; return 0; }
             *out = *acc;
+            if (field_decimal(m, f)) return dec_arith(field_decimal(m, f), agg == PO_AGG_PRODUCT ? 2 : 0, acc->v.i, in->v.i, out);
             {
                 int mul = agg == PO_AGG_PRODUCT;
                 switch (type) {
@@ -544,6 +599,7 @@ static int agg_retract(mf_t *m, int f, int agg, const po_val *acc, const po_val 
                 if (!acc->is_null) { *out = *acc; return 0; }
                 *out = *in;                                  /* negative(inputField) */
                 if (in->is_null) return 0;
+                if (field_decimal(m, f)) return dec_arith(field_decimal(m, f), 4, in->v.i, 0, out);
                 switch (type) {
                     case PO_INT8:  out->v.i = (int8_t)(-(int8_t)in->v.i); break;
                     case PO_INT16: out->v.i = (int16_t)(-(int16_t)in->v.i); break;
@@ -556,6 +612,7 @@ static int agg_retract(mf_t *m, int f, int agg, const po_val *acc, const po_val 
                 return 0;
             }
             *out = *acc;
+            if (field_decimal(m, f)) return dec_arith(field_decimal(m, f), 1, acc->v.i, in->v.i, out);
             switch (type) {
                 case PO_INT8:  out->v.i = (int8_t)((int8_t)acc->v.i - (int8_t)in->v.i); break;
                 case PO_INT16: out->v.i = (int16_t)((int16_t)acc->v.i - (int16_t)in->v.i); break;
@@ -569,6 +626,7 @@ static int agg_retract(mf_t *m, int f, int agg, const po_val *acc, const po_val 
         case PO_AGG_PRODUCT:                               /* FieldProductAgg retract: divide */
             if (acc->is_null || in->is_null) { *out = *acc; return 0; }
             *out = *acc;
+            if (field_decimal(m, f)) return dec_arith(field_decimal(m, f), 3, acc->v.i, in->v.i, out);
             switch (type) {
                 case PO_INT8: case PO_INT16: case PO_INT32: case PO_INT64:
                     if (in->v.i == 0) return fail("ArithmeticException: / by zero");

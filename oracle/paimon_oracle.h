@@ -111,6 +111,10 @@ typedef struct {
      * single-record passthrough — this is how the reference's MergeFunction unit tests
      * (PartialUpdateMergeFunctionTest, AggregateMergeFunctionTest) drive the function */
     int32_t bypass_wrapper;
+    /* [n_val] precision << 8 | scale of a DECIMAL(p <= 18) field (unscaled INT64), 0 = not DECIMAL; NULL = none.
+     * sum / product on such a field follow FieldSumAgg / FieldProductAgg's DECIMAL branch (DecimalUtils.add /
+     * subtract, BigDecimal multiply / divide, Decimal.fromBigDecimal), not int64 arithmetic. */
+    const int32_t *decimal;
 } po_spec;
 
 typedef struct {

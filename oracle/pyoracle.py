@@ -42,7 +42,8 @@ class _Spec(C.Structure):
                 ("agg", C.c_void_p), ("ignore_retract", C.c_void_p),
                 ("n_groups", C.c_int32), ("group_seq_start", C.c_void_p),
                 ("group_seq_fields", C.c_void_p), ("field_group", C.c_void_p),
-                ("group_partial_delete", C.c_void_p), ("bypass_wrapper", C.c_int32)]
+                ("group_partial_delete", C.c_void_p), ("bypass_wrapper", C.c_int32),
+                ("decimal", C.c_void_p)]
 
 
 class _OutCol(C.Structure):
@@ -116,11 +117,12 @@ class _Marshalled:
         gfields = np.array(gf, np.int32)
         fgroup = np.array(sp.field_group, np.int32)
         gpd = np.array([1 if b else 0 for b in sp.group_partial_delete], np.uint8)
-        self.keep += [seqf, agg, ign, gstart, gfields, fgroup, gpd]
+        dec = np.array(sp.decimal, np.int32) if sp.decimal else None
+        self.keep += [seqf, agg, ign, gstart, gfields, fgroup, gpd, dec]
         self.spec = _Spec(int(sp.engine), sort_engine, int(sp.ignore_delete), int(sp.remove_record_on_delete),
                           int(sp.drop_delete), len(sp.seq_fields), _ptr(seqf), int(sp.seq_ascending),
                           _ptr(agg), _ptr(ign), len(sp.groups), _ptr(gstart), _ptr(gfields), _ptr(fgroup),
-                          _ptr(gpd), int(bypass_wrapper))
+                          _ptr(gpd), int(bypass_wrapper), _ptr(dec))
 
         self.runs = (_Run * max(1, len(runs)))()
         self.col_arrays = []

@@ -33,7 +33,7 @@ class PgMergeSpec(C.Structure):
                 ("seq_ascending", C.c_int32), ("agg", C.c_void_p), ("ignore_retract", C.c_void_p),
                 ("n_sequence_groups", C.c_int32), ("group_seq_start", C.c_void_p),
                 ("group_seq_fields", C.c_void_p), ("field_group", C.c_void_p),
-                ("group_partial_delete", C.c_void_p), ("read_fields", C.c_void_p)]
+                ("group_partial_delete", C.c_void_p), ("read_fields", C.c_void_p), ("decimal", C.c_void_p)]
 
 
 class PgColumn(C.Structure):

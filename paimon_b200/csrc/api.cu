@@ -305,6 +305,7 @@ static pg_status build_descriptors(Merge *m) {
         cd.agg = PG_AGG_NONE;
         cd.retract = RT_OK;
         cd.varlen_index = -1;
+        cd.decimal = 0;
         if (is_varlen(f.type) && m->emit[c]) {
             cd.varlen_index = (int)m->varlen_cols.size();
             m->varlen_cols.push_back(c);
@@ -316,6 +317,9 @@ static pg_status build_descriptors(Merge *m) {
             int vi = c - s->n_key - 2;
             int agg = sp->agg.empty() ? PG_AGG_NONE : sp->agg[vi];
             bool ign = !sp->ignore_retract.empty() && sp->ignore_retract[vi];
+            // DECIMAL(p, s) of the field for sum / product (the only aggregators whose result depends on it)
+            const int32_t dec = sp->decimal.empty() ? 0 : sp->decimal[vi];
+            const int32_t fold_dec = agg == PG_AGG_SUM || agg == PG_AGG_PRODUCT ? dec : 0;
             if (sp->engine == PG_ENGINE_AGGREGATE) {
                 if (agg == PG_AGG_NONE) agg = PG_AGG_LAST_NON_NULL_VALUE;   // AggregateMergeFunction.java:199-202
                 bool numeric = f.type == PG_INT8 || f.type == PG_INT16 || f.type == PG_INT32 ||
@@ -330,6 +334,7 @@ static pg_status build_descriptors(Merge *m) {
                     return fail(PG_ERR_UNSUPPORTED, "aggregate function not implemented on the device");
                 cd.mode = CM_FOLD;
                 cd.agg = agg;
+                cd.decimal = fold_dec;
                 // an aggregator can produce NULL from non-null inputs (retract of last_value, ignored
                 // retracts only, ...) and AggregateMergeFunction does not re-check NOT NULL: the output of a
                 // folded column always carries a validity bitmap
@@ -353,6 +358,7 @@ static pg_status build_descriptors(Merge *m) {
                         // a group field with an aggregate function (PartialUpdateMergeFunction.java:228-244)
                         cd.mode = CM_GAGG;
                         cd.agg = agg;
+                        cd.decimal = fold_dec;
                         cd.group = g;
                         cd.retract = ign ? RT_IGNORE : (agg_supports_retract(agg) ? RT_OK : RT_ERROR);
                         m->has_group_aggs = true;
@@ -476,6 +482,12 @@ static const char *kernel_error_message(int code) {
             return "a var-len output column exceeds 2 GiB (int32 offsets); merge fewer rows per call";
         case KERR_DIV_ZERO:
             return "ArithmeticException: / by zero";
+        case KERR_DEC_DIV_ZERO:
+            return "ArithmeticException: Division by zero";
+        case KERR_DEC_DIV_UNDEFINED:
+            return "ArithmeticException: Division undefined";
+        case KERR_DEC_NON_TERMINATING:
+            return "ArithmeticException: Non-terminating decimal expansion; no exact representable decimal result.";
         default:
             return "unknown kernel error";
     }
@@ -850,6 +862,20 @@ pg_status pg_merge_spec_create(uint64_t schema, const pg_merge_spec *spec, uint6
     if (spec->agg) sp->agg.assign(spec->agg, spec->agg + s->n_val);
     if (spec->ignore_retract) sp->ignore_retract.assign(spec->ignore_retract, spec->ignore_retract + s->n_val);
     if (spec->read_fields) sp->read_fields.assign(spec->read_fields, spec->read_fields + s->n_val);
+    if (spec->decimal) {
+        sp->decimal.assign(spec->decimal, spec->decimal + s->n_val);
+        for (int f = 0; f < s->n_val; f++) {
+            const int32_t d = sp->decimal[f];
+            if (d == 0) continue;
+            const int p = d >> 8, sc = d & 0xff;
+            if (p > 18)
+                return fail(PG_ERR_UNSUPPORTED, "DECIMAL(p > 18) is not implemented on the device (field " +
+                                                    std::to_string(f) + ")");
+            if (p < 1 || sc > p || s->val_fields[f].type != PG_INT64)
+                return fail(PG_ERR_INVALID, "bad DECIMAL description of value field " + std::to_string(f) +
+                                                " (precision 1..18, scale <= precision, an INT64 column)");
+        }
+    }
     if (spec->n_sequence_groups > 0) {
         const int ng = spec->n_sequence_groups;
         sp->group_seq_start.assign(spec->group_seq_start, spec->group_seq_start + ng + 1);

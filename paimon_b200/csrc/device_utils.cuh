@@ -120,6 +120,75 @@ __device__ __forceinline__ uint64_t arith(int type, int width, int fn, uint64_t 
     return r;        // store_fixed truncates to the column width == Java's narrowing cast
 }
 
+// ---- DECIMAL(p, s) sum / product on unscaled int64 values (FieldSumAgg / FieldProductAgg on DecimalType)
+// sum, subtract: DecimalUtils.add / subtract (DecimalUtils.java:52-87): exact int64; on overflow the BigDecimal result
+//   has more than 18 digits and Decimal.fromBigDecimal gives NULL.  A result over p digits that fits int64 is kept
+//   (fromUnscaledLong does not check the precision).
+// product: round_half_up(a * b / 10^s), NULL over p digits (FieldProductAgg.java:47-58, Decimal.java:182-193).
+// retract of a product: BigDecimal.divide is exact (throws when the quotient does not terminate, or on a zero
+//   divisor); the result is round_half_up(a * 10^s / b), NULL over p digits (FieldProductAgg.java:95-106).
+// negate (retract of a sum into a NULL accumulator): fromBigDecimal(-a), NULL over p digits (FieldSumAgg.java:140-143).
+// |a|, |b| <= 2^63 and 10^s <= 10^18, so a * b and a * 10^s fit __int128.
+__device__ __forceinline__ unsigned __int128 dec_pow10(int e) {
+    unsigned __int128 r = 1;
+    for (int i = 0; i < e; i++) r *= 10u;
+    return r;
+}
+// round_half_up(n / d) for d > 0: ties away from zero (RoundingMode.HALF_UP)
+__device__ __forceinline__ __int128 dec_div_half_up(__int128 n, unsigned __int128 d) {
+    const bool neg = n < 0;
+    const unsigned __int128 m = neg ? (unsigned __int128)0 - (unsigned __int128)n : (unsigned __int128)n;
+    unsigned __int128 q = m / d;
+    const unsigned __int128 r = m - q * d;
+    if (r >= d - r) q += 1;
+    return neg ? -(__int128)q : (__int128)q;
+}
+__device__ __forceinline__ bool dec_fits(__int128 v, int precision) {     // BigDecimal.precision() <= p
+    const unsigned __int128 m = v < 0 ? (unsigned __int128)0 - (unsigned __int128)v : (unsigned __int128)v;
+    return m < dec_pow10(precision);
+}
+// fn: 0 add, 1 sub, 2 mul, 3 div, 4 negate a
+struct DecimalResult {
+    uint64_t value;      // unscaled
+    bool valid;          // false = NULL
+};
+__device__ __forceinline__ DecimalResult decimal_arith(int decimal, int fn, uint64_t ua, uint64_t ub, int32_t *err) {
+    const int precision = decimal >> 8, scale = decimal & 0xff;
+    const int64_t a = (int64_t)ua, b = (int64_t)ub;
+    __int128 r;
+    if (fn == 0 || fn == 1) {
+        const uint64_t u = fn == 0 ? ua + ub : ua - ub;
+        const int64_t x = (int64_t)u;
+        const bool overflow = fn == 0 ? ((a ^ x) & (b ^ x)) < 0 : ((a ^ b) & (a ^ x)) < 0;
+        return DecimalResult{overflow ? 0 : u, !overflow};
+    }
+    if (fn == 4) {
+        r = -(__int128)a;
+    } else if (fn == 2) {
+        r = dec_div_half_up((__int128)a * (__int128)b, dec_pow10(scale));
+    } else {
+        if (b == 0) {
+            atomicCAS(err, KERR_NONE, a == 0 ? KERR_DEC_DIV_UNDEFINED : KERR_DEC_DIV_ZERO);
+            return DecimalResult{0, false};
+        }
+        // a / b terminates iff b / gcd(a, b) has no prime factor other than 2 and 5
+        const uint64_t mb = b < 0 ? 0ull - ub : ub;
+        uint64_t x = a < 0 ? 0ull - ua : ua, y = mb;
+        while (x != 0) { const uint64_t t = y % x; y = x; x = t; }
+        uint64_t den = mb / y;
+        while (den % 2 == 0) den /= 2;
+        while (den % 5 == 0) den /= 5;
+        if (den != 1) {
+            atomicCAS(err, KERR_NONE, KERR_DEC_NON_TERMINATING);
+            return DecimalResult{0, false};
+        }
+        const __int128 n = (__int128)a * (__int128)dec_pow10(scale);
+        r = dec_div_half_up(b < 0 ? -n : n, (unsigned __int128)mb);
+    }
+    const bool fits = dec_fits(r, precision);
+    return DecimalResult{fits ? (uint64_t)(int64_t)r : 0, fits};
+}
+
 __device__ __forceinline__ uint64_t negate_fixed(int type, int width, uint64_t a) {
     if (type == PG_DOUBLE) return a ^ 0x8000000000000000ull;
     if (type == PG_FLOAT) return (uint32_t)a ^ 0x80000000u;

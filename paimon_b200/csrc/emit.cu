@@ -164,7 +164,22 @@ __device__ int fold_member_idx(const ColDesc &cd, const uint16_t *pm, const uint
     return acc;
 }
 
+// SUM / PRODUCT step of a fixed-width fold (fn as in arith, 4 = negate a).  Integer and float results are never
+// NULL; a DECIMAL one can be (decimal_arith).  DEC = true only inside emit_decimal_column.
+template <bool DEC>
+__device__ __forceinline__ uint64_t fold_arith(const ColDesc &cd, int fn, uint64_t a, uint64_t b, bool *valid,
+                                               int32_t *err) {
+    if (DEC) {
+        const DecimalResult d = decimal_arith(cd.decimal, fn, a, b, err);
+        *valid = d.valid;
+        return d.value;
+    }
+    *valid = true;
+    return fn == 4 ? negate_fixed(cd.type, cd.width, a) : arith(cd.type, cd.width, fn, a, b, err);
+}
+
 // strict left fold of a fixed-width column in sequence order (AggregateMergeFunction.java:91-101)
+template <bool DEC>
 __device__ void fold_fixed(const ColDesc &cd, const uint16_t *pm, const uint32_t *vw, const unsigned char *vals,
                            int last, uint64_t *out_val, bool *out_valid, int32_t *err) {
     const int w = cd.width;
@@ -182,11 +197,11 @@ __device__ void fold_fixed(const ColDesc &cd, const uint16_t *pm, const uint32_t
             if (cd.retract == RT_IGNORE) continue;
             switch (cd.agg) {
                 case PG_AGG_SUM:       // FieldSumAgg.retract :87-131, negative :133-163
-                    if (!is_valid) { if (v) { val = negate_fixed(cd.type, w, in); is_valid = true; } }
-                    else if (v) val = arith(cd.type, w, 1, val, in, err);
+                    if (!is_valid) { if (v) val = fold_arith<DEC>(cd, 4, in, 0, &is_valid, err); }
+                    else if (v) val = fold_arith<DEC>(cd, 1, val, in, &is_valid, err);
                     break;
                 case PG_AGG_PRODUCT:
-                    if (is_valid && v) val = arith(cd.type, w, 3, val, in, err);
+                    if (is_valid && v) val = fold_arith<DEC>(cd, 3, val, in, &is_valid, err);
                     break;
                 case PG_AGG_LAST_VALUE: is_valid = false; val = 0; break;
                 case PG_AGG_LAST_NON_NULL_VALUE: if (v) { is_valid = false; val = 0; } break;
@@ -198,7 +213,7 @@ __device__ void fold_fixed(const ColDesc &cd, const uint16_t *pm, const uint32_t
         switch (cd.agg) {
             case PG_AGG_SUM: case PG_AGG_PRODUCT:
                 if (!is_valid || !v) { if (!is_valid) { val = in; is_valid = v; } }
-                else val = arith(cd.type, w, cd.agg == PG_AGG_SUM ? 0 : 2, val, in, err);
+                else val = fold_arith<DEC>(cd, cd.agg == PG_AGG_SUM ? 0 : 2, val, in, &is_valid, err);
                 break;
             case PG_AGG_MAX: case PG_AGG_MIN:
                 if (!is_valid || !v) { if (!is_valid) { val = in; is_valid = v; } }
@@ -229,13 +244,14 @@ __device__ void fold_fixed(const ColDesc &cd, const uint16_t *pm, const uint32_t
 
 // agg(accumulator = a, input = b) of a fixed-width aggregator as a function of both operands, so that
 // aggReversed(acc, in) = agg(in, acc) (FieldAggregator.java:40-42) can be evaluated too
+template <bool DEC>
 __device__ void agg_pair(const ColDesc &cd, uint64_t a, bool av, uint64_t b, bool bv, bool *initialized,
                          uint64_t *out, bool *out_valid, int32_t *err) {
     const int w = cd.width;
     switch (cd.agg) {
         case PG_AGG_SUM: case PG_AGG_PRODUCT:
             if (!av || !bv) { *out = av ? a : b; *out_valid = av || bv; }
-            else { *out = arith(cd.type, w, cd.agg == PG_AGG_SUM ? 0 : 2, a, b, err); *out_valid = true; }
+            else *out = fold_arith<DEC>(cd, cd.agg == PG_AGG_SUM ? 0 : 2, a, b, out_valid, err);
             return;
         case PG_AGG_MAX: case PG_AGG_MIN:
             if (!av || !bv) { *out = av ? a : b; *out_valid = av || bv; return; }
@@ -268,6 +284,7 @@ __device__ void agg_pair(const ColDesc &cd, uint64_t a, bool av, uint64_t b, boo
 // (PartialUpdateMergeFunction.updateWithSequenceGroup :228-244, retractWithSequenceGroup :323-339): every member
 // whose group is not empty takes part — in order (agg) when its group sequence is >= the accumulated one, else
 // reversed (aggReversed); retract members call retract(); the first record of a key initialises the row.
+template <bool DEC>
 __device__ void fold_group_agg(const ColDesc &cd, const uint16_t *pm, const uint32_t *gagg, const uint32_t *vw,
                                const unsigned char *vals, int last, uint64_t *out_val, bool *out_valid, int32_t *err) {
     const int w = cd.width, g = cd.group;
@@ -287,11 +304,11 @@ __device__ void fold_group_agg(const ColDesc &cd, const uint16_t *pm, const uint
             if (!((marks >> g) & 1) || cd.retract == RT_IGNORE) continue;
             switch (cd.agg) {
                 case PG_AGG_SUM:
-                    if (!is_valid) { if (v) { val = negate_fixed(cd.type, w, in); is_valid = true; } }
-                    else if (v) val = arith(cd.type, w, 1, val, in, err);
+                    if (!is_valid) { if (v) val = fold_arith<DEC>(cd, 4, in, 0, &is_valid, err); }
+                    else if (v) val = fold_arith<DEC>(cd, 1, val, in, &is_valid, err);
                     break;
                 case PG_AGG_PRODUCT:
-                    if (is_valid && v) val = arith(cd.type, w, 3, val, in, err);
+                    if (is_valid && v) val = fold_arith<DEC>(cd, 3, val, in, &is_valid, err);
                     break;
                 case PG_AGG_LAST_VALUE: is_valid = false; val = 0; break;
                 case PG_AGG_LAST_NON_NULL_VALUE: if (v) { is_valid = false; val = 0; } break;
@@ -302,8 +319,8 @@ __device__ void fold_group_agg(const ColDesc &cd, const uint16_t *pm, const uint
         }
         uint64_t r;
         bool rv;
-        if ((marks >> g) & 1) agg_pair(cd, val, is_valid, in, v, &initialized, &r, &rv, err);
-        else if ((marks >> (16 + g)) & 1) agg_pair(cd, in, v, val, is_valid, &initialized, &r, &rv, err);
+        if ((marks >> g) & 1) agg_pair<DEC>(cd, val, is_valid, in, v, &initialized, &r, &rv, err);
+        else if ((marks >> (16 + g)) & 1) agg_pair<DEC>(cd, in, v, val, is_valid, &initialized, &r, &rv, err);
         else continue;                                                       // empty group in this record
         val = rv ? r : 0;
         is_valid = rv;
@@ -362,7 +379,7 @@ __device__ __forceinline__ void emit_fixed_column(const EmitArgs &ea, const ColD
                     if (staged_valid(vw, pj)) { val = lds_fixed<W>(vals, pj); is_valid = true; }
                 }
             } else if (GAGG && cd.mode == CM_GAGG) {
-                fold_group_agg(cd, tv.pm, ea.gagg + tv.in_base, vw, vals, last, &val, &is_valid, ea.err);
+                fold_group_agg<false>(cd, tv.pm, ea.gagg + tv.in_base, vw, vals, last, &val, &is_valid, ea.err);
                 if (!is_valid) val = 0;
             } else if (cd.mode == CM_KEY) {
                 val = lds_fixed<W>(vals, tv.pm[last] & kPmPosMask); is_valid = true;
@@ -371,10 +388,33 @@ __device__ __forceinline__ void emit_fixed_column(const EmitArgs &ea, const ColD
             } else if (cd.mode == CM_KIND) {
                 val = (uint8_t)ea.tmp_kind[result_index(tv, ob)]; is_valid = true;
             } else {
-                fold_fixed(cd, tv.pm, vw, vals, last, &val, &is_valid, ea.err);
+                fold_fixed<false>(cd, tv.pm, vw, vals, last, &val, &is_valid, ea.err);
                 if (!is_valid) val = 0;
             }
             stg_fixed<W>(oc.data, tv.out_base + ob, val);
+        }
+        if (oc.validity != nullptr) put_validity_word(oc.validity, tv.out_base, wb, tv.n_out, is_valid);
+    }
+}
+
+// A DECIMAL sum / product column (CM_FOLD or CM_GAGG, cd.decimal != 0): the same folds with the DECIMAL arithmetic.
+// It is its own pass branch (chosen once per column and tile, like the width) so that the common folds carry no
+// decimal test in their loops.  Out of line, the call costs the kernel a stack frame and spills in every pass; inlined,
+// k_emit<false> keeps 64 registers and 8 bytes of stack (k_emit<true>: 16 -> 24 bytes of stack).
+template <bool GAGG>
+__device__ __forceinline__ void emit_decimal_column(const ColDesc &cd, const pg_out_column &oc, const TileView &tv,
+                                                    const unsigned char *vals, const uint32_t *vw, const uint32_t *gagg,
+                                                    int32_t *err) {
+    const int tid = threadIdx.x, lane = tid & 31;
+    for (int wb = (tid & ~31) - tv.o_shift; wb < tv.n_out; wb += kEmitThreads) {   // warp-uniform trip count
+        const int ob = wb + lane;
+        bool is_valid = false;
+        if (ob >= 0 && ob < tv.n_out) {
+            uint64_t val = 0;
+            const int last = tv.glast[ob];
+            if (GAGG && cd.mode == CM_GAGG) fold_group_agg<true>(cd, tv.pm, gagg, vw, vals, last, &val, &is_valid, err);
+            else fold_fixed<true>(cd, tv.pm, vw, vals, last, &val, &is_valid, err);
+            stg_fixed<8>(oc.data, tv.out_base + ob, is_valid ? val : 0);
         }
         if (oc.validity != nullptr) put_validity_word(oc.validity, tv.out_base, wb, tv.n_out, is_valid);
     }
@@ -595,7 +635,8 @@ k_emit(EmitArgs ea) {
         const unsigned char *vals = stage_vals(s);
         const uint32_t *vw = stage_vw(s);
 
-        if (cd.width == 8) emit_fixed_column<8, GAGG>(ea, cd, oc, tv, vals, vw);
+        if (cd.decimal) emit_decimal_column<GAGG>(cd, oc, tv, vals, vw, GAGG ? ea.gagg + tv.in_base : nullptr, ea.err);
+        else if (cd.width == 8) emit_fixed_column<8, GAGG>(ea, cd, oc, tv, vals, vw);
         else if (cd.width == 4) emit_fixed_column<4, GAGG>(ea, cd, oc, tv, vals, vw);
         else if (cd.width == 1) emit_fixed_column<1, GAGG>(ea, cd, oc, tv, vals, vw);
         else if (cd.width == 2) emit_fixed_column<2, GAGG>(ea, cd, oc, tv, vals, vw);

@@ -46,7 +46,10 @@ enum : int {
     KERR_PQ_NO_DICT = 10,            // dictionary-encoded page in a chunk without dictionary page
     KERR_PQ_ROWS = 11,               // the pages of a chunk do not add up to the chunk's value count
     KERR_PQ_DICT_ID = 12,            // dictionary id outside the dictionary
-    KERR_PQ_LEVELS = 13              // repetition levels / unsupported level encoding
+    KERR_PQ_LEVELS = 13,             // repetition levels / unsupported level encoding
+    KERR_DEC_DIV_ZERO = 14,          // FieldProductAgg retract on DECIMAL: BigDecimal.divide by zero
+    KERR_DEC_DIV_UNDEFINED = 15,     // the same with a zero dividend (0 / 0)
+    KERR_DEC_NON_TERMINATING = 16    // the same when the exact quotient has no finite decimal expansion
 };
 
 struct Schema {
@@ -73,6 +76,7 @@ struct Spec {
     std::vector<int32_t> group_seq_start, group_seq_fields, field_group;
     std::vector<uint8_t> group_partial_delete;      // per group
     std::vector<uint8_t> read_fields;               // per value field: part of the read type (empty = all)
+    std::vector<int32_t> decimal;                   // per value field: precision << 8 | scale, 0 (empty = none)
     int n_groups() const { return group_seq_start.empty() ? 0 : (int)group_seq_start.size() - 1; }
 };
 
@@ -203,17 +207,20 @@ pg_status batch_columns(uint64_t handle, const Schema **schema, std::vector<DevC
 
 // ---- device-side descriptors (copied to device memory once per merge handle) ----
 
-// column descriptor used by the emit kernel
+// column descriptor used by the emit kernel; 32 bytes (the kernel keeps 64 of them in shared memory, and a larger
+// static footprint would cost a second resident CTA per SM at some run counts)
 struct ColDesc {
     int32_t type;        // pg_type
     int32_t width;       // bytes, 0 for var-len
-    int32_t nullable;    // output carries a validity bitmap
+    int16_t nullable;    // output carries a validity bitmap
+    int16_t retract;     // RT_*
     int32_t mode;        // CM_*
     int32_t agg;         // PG_AGG_* for CM_FOLD
-    int32_t retract;     // RT_*
     int32_t varlen_index;// index among var-len columns, -1 otherwise
     int32_t group;       // CM_GAGG: the sequence group of the field
+    int32_t decimal;     // DECIMAL value field: precision << 8 | scale (sum / product use decimal_arith), else 0
 };
+static_assert(sizeof(ColDesc) == 32, "ColDesc is staged in shared memory by the emit kernel");
 // CM_GVAL / CM_GSEQ: field / sequence field of partial-update sequence group `agg`: the cell of the member the
 // plan kernel marked for the group (verbatim, NULL included), NULL when no member is marked
 // CM_GAGG: field of a sequence group with an aggregate function (`agg`): folded over the members the plan kernel

@@ -20,7 +20,7 @@ import enum
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
 
-from .types import KeyValueSchema, PhysicalType, RowType, is_varlen
+from .types import DataField, KeyValueSchema, RowType, decimal_precision_scale, type_root
 
 
 class MergeEngine(enum.IntEnum):          # CoreOptions.MergeEngine (CoreOptions.java:3910-3917)
@@ -93,6 +93,9 @@ class MergeSpec:
     # read-type projection (MergeFunctionFactory.create(readType)): per value field, part of the merged batch;
     # empty = every field.  Field indexes everywhere in the spec stay those of the table's row type.
     read_fields: List[bool] = field(default_factory=list)
+    # per value field: precision << 8 | scale of a DECIMAL field, 0 for every other type; empty = no DECIMAL field.
+    # SUM / PRODUCT on a DECIMAL field follow DecimalUtils / BigDecimal, not int64 arithmetic on the unscaled value.
+    decimal: List[int] = field(default_factory=list)
 
     def with_read_fields(self, mask: Sequence[bool]) -> "MergeSpec":
         import copy
@@ -142,23 +145,46 @@ def _sequence_fields(options: Dict[str, str], row_type: RowType):
     return [row_type.index_of(n) for n in names], names, asc
 
 
-def _resolve_agg(name: str, field_name: str, ptype: PhysicalType) -> Agg:
+# logical type roots of the NUMERIC family (DataTypeRoot.java), the only ones FieldSumAggFactory /
+# FieldProductAggFactory accept
+_NUMERIC_ROOTS = {"TINYINT", "SMALLINT", "INT", "BIGINT", "FLOAT", "DOUBLE", "DECIMAL"}
+# roots InternalRowUtils.compare orders (InternalRowUtils.java:387-432), what FieldMaxAgg / FieldMinAgg need
+_COMPARABLE_ROOTS = _NUMERIC_ROOTS | {"DATE", "TIME", "TIMESTAMP", "CHAR", "VARCHAR", "STRING", "BINARY",
+                                      "VARBINARY", "BYTES"}
+
+
+def _resolve_agg(name: str, f: DataField) -> Agg:
+    """FieldAggregatorFactory.create: the aggregator's factory checks the field's LOGICAL type root
+    (FieldSumAggFactory.java:33-39, FieldProductAggFactory.java:33-39, FieldBoolAndAggFactory.java:33-39)."""
     if name in _UNSUPPORTED_AGGS:
         raise UnsupportedMergeSpec(
-            f"aggregate function '{name}' on field '{field_name}' keeps variable-size state and is "
+            f"aggregate function '{name}' on field '{f.name}' keeps variable-size state and is "
             f"not implemented on the device merge path")
     if name not in _AGG_NAMES:
         raise ValueError(f"Use unsupported aggregation: {name} or spell aggregate function incorrectly!")
     agg = _AGG_NAMES[name]
-    numeric = ptype in (PhysicalType.INT8, PhysicalType.INT16, PhysicalType.INT32, PhysicalType.INT64,
-                        PhysicalType.FLOAT, PhysicalType.DOUBLE)
-    if agg in (Agg.SUM, Agg.PRODUCT) and not numeric:
-        raise ValueError(f"Data type for {name} column must be numeric")       # FieldSumAggFactory
-    if agg in (Agg.BOOL_AND, Agg.BOOL_OR) and ptype != PhysicalType.BOOL:
-        raise ValueError(f"Data type for {name} column must be 'BooleanType'")
-    if agg in (Agg.MAX, Agg.MIN) and ptype == PhysicalType.BOOL:
-        raise ValueError("Incomparable type: BOOLEAN")                          # InternalRowUtils.compare
+    f.physical                                                  # refuses types the device cannot store
+    root = type_root(f.type)
+    if agg in (Agg.SUM, Agg.PRODUCT) and root not in _NUMERIC_ROOTS:
+        raise ValueError(f"Data type for {name} column must be 'NumericType' but was '{f.type}'.")
+    if agg in (Agg.BOOL_AND, Agg.BOOL_OR) and root != "BOOLEAN":
+        raise ValueError(f"Data type for {name.replace('_', ' ')} column must be 'BooleanType' but was '{f.type}'.")
+    if agg in (Agg.MAX, Agg.MIN) and root not in _COMPARABLE_ROOTS:
+        raise ValueError(f"Incomparable type: {f.type}")                     # InternalRowUtils.compare
     return agg
+
+
+def decimal_descriptors(row_type: RowType) -> List[int]:
+    """MergeSpec.decimal of a row type: precision << 8 | scale per DECIMAL field, 0 elsewhere; empty when the row has
+    no DECIMAL field."""
+    out = []
+    for f in row_type.fields:
+        if type_root(f.type) == "DECIMAL":
+            p, s = decimal_precision_scale(f.type)
+            out.append(p << 8 | s)
+        else:
+            out.append(0)
+    return out if any(out) else []
 
 
 class DeduplicateMergeFunction:
@@ -203,11 +229,11 @@ class AggregateMergeFunction:
                         name = (options.get(f"{FIELDS_PREFIX}.{f.name}.{AGG_FUNCTION}")
                                 or options.get(f"{FIELDS_PREFIX}.{DEFAULT_AGG_FUNCTION}")
                                 or "last_non_null_value")
-                    aggs.append(_resolve_agg(name, f.name, f.physical))
+                    aggs.append(_resolve_agg(name, f))
                     ign.append(_bool(options.get(f"{FIELDS_PREFIX}.{f.name}.{IGNORE_RETRACT}", False)))
                 return MergeSpec(engine=MergeEngine.AGGREGATE,
                                  remove_record_on_delete=_bool(options.get("aggregation.remove-record-on-delete", False)),
-                                 agg=aggs, ignore_retract=ign)
+                                 agg=aggs, ignore_retract=ign, decimal=decimal_descriptors(target))
         return _F()
 
 
@@ -277,7 +303,7 @@ class PartialUpdateMergeFunction:
                 if name is not None and name != "last_non_null_value" and f.name not in protected:
                     raise ValueError(f"Must use sequence group for aggregation functions but not found "
                                      f"for field {f.name}.")
-            aggs.append(Agg.NONE if name is None else _resolve_agg(name, f.name, f.physical))
+            aggs.append(Agg.NONE if name is None else _resolve_agg(name, f))
             ign.append(_bool(options.get(f"{FIELDS_PREFIX}.{f.name}.{IGNORE_RETRACT}", False)))
 
         class _F(MergeFunctionFactory):
@@ -285,7 +311,8 @@ class PartialUpdateMergeFunction:
                 spec = MergeSpec(engine=MergeEngine.PARTIAL_UPDATE, ignore_delete=ignore_delete,
                                  remove_record_on_delete=remove_on_delete, agg=list(aggs),
                                  ignore_retract=list(ign), groups=[list(g) for g in groups],
-                                 field_group=list(field_group), group_partial_delete=list(partial_delete))
+                                 field_group=list(field_group), group_partial_delete=list(partial_delete),
+                                 decimal=decimal_descriptors(row_type))
                 if read_type is not None and read_type.field_names() != names:
                     # a projected read type (PartialUpdateMergeFunction.java:492-573 re-indexes the per-field
                     # configuration; here the indexes stay those of the table and the projection is a mask)

@@ -320,14 +320,15 @@ class SortMergeReader(RecordReader):
         gpd = np.array([1 if b else 0 for b in sp.group_partial_delete], np.uint8)
         rf = np.array([1 if b else 0 for b in sp.read_fields], np.uint8) if sp.read_fields else None
         self._read_fields = list(sp.read_fields) if sp.read_fields else None
-        self._keep += [gstart, gfields, fgroup, gpd, rf]
+        dec = np.array(sp.decimal, np.int32) if sp.decimal else None
+        self._keep += [gstart, gfields, fgroup, gpd, rf, dec]
         has_groups = len(sp.groups) > 0
         cs = N.PgMergeSpec(int(sp.engine), int(sp.ignore_delete), int(sp.remove_record_on_delete),
                            int(sp.drop_delete), len(seq), _np_ptr(seq_arr) if len(seq) else None,
                            int(sp.seq_ascending), _np_ptr(agg), _np_ptr(ign), len(sp.groups),
                            _np_ptr(gstart) if has_groups else None, _np_ptr(gfields) if has_groups else None,
                            _np_ptr(fgroup) if has_groups else None, _np_ptr(gpd) if has_groups else None,
-                           _np_ptr(rf))
+                           _np_ptr(rf), _np_ptr(dec))
         h = C.c_uint64(0)
         try:
             N.check(self.lib.pg_merge_spec_create(self._schema_h.handle, C.byref(cs), C.byref(h)))

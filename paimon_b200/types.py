@@ -62,10 +62,41 @@ _LOGICAL = {
 }
 
 
-def physical_type(logical: str) -> PhysicalType:
+def type_root(logical: str) -> str:
+    """The logical type root of a Paimon SQL type name: "DECIMAL(10,2)" -> "DECIMAL", "INTEGER" -> "INT"."""
     root = logical.upper().split("(")[0].strip()
+    return "INT" if root == "INTEGER" else root
+
+
+def _type_args(logical: str) -> List[int]:
+    if "(" not in logical:
+        return []
+    inner = logical[logical.index("(") + 1: logical.rindex(")")]
+    return [int(a) for a in inner.split(",")]
+
+
+def decimal_precision_scale(logical: str):
+    """(precision, scale) of a DECIMAL type; DECIMAL alone is DECIMAL(10, 0) (DecimalType.java:41-45)."""
+    args = _type_args(logical)
+    precision = args[0] if args else 10
+    scale = args[1] if len(args) > 1 else 0
+    return precision, scale
+
+
+def physical_type(logical: str) -> PhysicalType:
+    root = type_root(logical)
     if root not in _LOGICAL:
         raise ValueError(f"unsupported type on the GPU merge path: {logical}")
+    if root == "DECIMAL":
+        p, s = decimal_precision_scale(logical)
+        if not (1 <= p <= 18) or not (0 <= s <= p):
+            raise ValueError(f"unsupported type on the GPU merge path: {logical} (DECIMAL is stored as an unscaled "
+                             f"INT64: precision 1 to 18)")
+    if root == "TIMESTAMP":
+        args = _type_args(logical)
+        if args and args[0] > 6:
+            raise ValueError(f"unsupported type on the GPU merge path: {logical} (TIMESTAMP is stored as INT64 "
+                             f"micros: precision up to 6)")
     return _LOGICAL[root]
 
 

@@ -212,6 +212,110 @@ pg_status batch_columns(uint64_t handle, const Schema **schema, std::vector<DevC
     return PG_OK;
 }
 
+// ------------------------------------------------------------------ decoded runs (pg_internal.h: RunBuilder)
+
+pg_status oom(const char *who, const char *what, size_t bytes) {
+    size_t fr = 0, tot = 0;
+    cudaMemGetInfo(&fr, &tot);
+    cudaGetLastError();
+    return fail(PG_ERR_CUDA, std::string(who) + ": out of device memory for " + what + " (" + std::to_string(bytes >> 20) +
+                                 " MiB wanted, " + std::to_string(fr >> 20) + " of " + std::to_string(tot >> 20) + " MiB free)");
+}
+
+pg_status RunBuilder::read_columns(const uint8_t *read_cols) {
+    if (!read_cols) return PG_OK;
+    for (int c = 0; c < schema.n_key + 2; c++)
+        if (!read_cols[c]) return fail(PG_ERR_INVALID, std::string(who) + ": key, sequence number and kind columns are always read");
+    for (int c = 0; c < nc; c++) read[c] = read_cols[c] != 0;
+    return PG_OK;
+}
+
+pg_status RunBuilder::check_rows() const {
+    for (int64_t n : run_rows)
+        if (n > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, std::string(who) + ": more than 2^31 rows in one run");
+    return PG_OK;
+}
+
+pg_status RunBuilder::alloc(const std::vector<uint8_t> &bitmap, const std::vector<uint8_t> &zero) {
+    const int n_runs = (int)run_rows.size();
+    scratch.runs.resize(n_runs);
+    out.assign((size_t)n_runs * nc, OutColumn());
+    for (int r = 0; r < n_runs; r++) {
+        const int64_t n = run_rows[r];
+        scratch.runs[r] = std::make_unique<Run>(schema, n);
+        // values, or int32 offsets
+        auto main_bytes = [&](int c) { const int w = type_width(schema.field(c).type); return w ? (size_t)n * w : 4 * (size_t)(n + 1); };
+        const size_t vb = align256((size_t)((n + 31) / 32) * 4 + 64);
+        size_t vbytes = 0;
+        for (int c = 0; c < nc; c++) if (read[c] && bitmap[c]) vbytes += vb;
+        size_t total = vbytes;
+        std::vector<size_t> o_main(nc);
+        for (int c = 0; c < nc; c++) {
+            o_main[c] = total;
+            if (read[c]) total += align256(main_bytes(c) + 64);
+        }
+        scratch.runs[r]->bufs.emplace_back(total + 256);
+        unsigned char *base = scratch.runs[r]->bufs.back().get();
+        if (!base) return oom(who, "the columns of a run", total);
+        if (vbytes) PG_CUDA(cudaMemsetAsync(base, 0, vbytes, scratch.stream));
+        size_t vt = 0;
+        for (int c = 0; c < nc; c++) {
+            if (!read[c]) continue;
+            OutColumn &o = out[(size_t)r * nc + c];
+            if (bitmap[c]) { o.validity = (uint32_t *)(base + vt); vt += vb; decoded_bytes += (n + 7) / 8; }
+            if (type_width(schema.field(c).type)) o.data = base + o_main[c];
+            else o.offsets = (int32_t *)(base + o_main[c]);
+            decoded_bytes += (int64_t)main_bytes(c);
+            if (zero[(size_t)r * nc + c]) PG_CUDA(cudaMemsetAsync(base + o_main[c], 0, main_bytes(c), scratch.stream));
+        }
+    }
+    return PG_OK;
+}
+
+pg_status RunBuilder::alloc_payload(const std::vector<int64_t> &payload) {
+    bool any = false;
+    for (int c = 0; c < nc; c++) any |= read[c] && is_varlen(schema.field(c).type);
+    if (!any) return PG_OK;
+    for (int r = 0; r < (int)run_rows.size(); r++) {
+        size_t sum = 256;
+        for (int c = 0; c < nc; c++)
+            if (read[c] && is_varlen(schema.field(c).type)) sum += align256((size_t)payload[(size_t)r * nc + c] + 64);
+        Run &run = *scratch.runs[r];
+        run.bufs.emplace_back(sum);
+        unsigned char *pl = run.bufs.back().get();
+        if (!pl) return oom(who, "the var-len payload of a run", sum);
+        size_t pt = 0;
+        for (int c = 0; c < nc; c++) {
+            if (!read[c] || !is_varlen(schema.field(c).type)) continue;
+            const int64_t bytes = payload[(size_t)r * nc + c];
+            out[(size_t)r * nc + c].data = pl + pt;
+            run.varlen_bytes[c] = bytes;
+            decoded_bytes += bytes;
+            pt += align256((size_t)bytes + 64);
+        }
+    }
+    return PG_OK;
+}
+
+void RunBuilder::finish(uint64_t *out_runs, int64_t bytes_h2d, pg_section_info *info) {
+    const int n_runs = (int)run_rows.size();
+    for (int r = 0; r < n_runs; r++) {
+        Run &run = *scratch.runs[r];
+        for (int c = 0; c < nc; c++) {
+            const OutColumn &o = out[(size_t)r * nc + c];
+            if (read[c]) run.cols[c] = DevColumn{o.data ? o.data : run.bufs[0].get(), o.offsets, (const uint8_t *)o.validity};
+        }
+        run.bytes_h2d = r == 0 ? bytes_h2d : 0;
+        out_runs[r] = g_runs.put(std::move(scratch.runs[r]));
+    }
+    if (info) {
+        memset(info, 0, sizeof(*info));
+        for (int64_t n : run_rows) info->n_rows += n;
+        info->n_runs = n_runs;
+        info->decoded_bytes = decoded_bytes;
+    }
+}
+
 // drop the current batch; the arena itself is kept for the next execute unless `release_memory`
 static void free_outputs(Merge *m, bool release_memory = false) {
     m->out_cols.clear();

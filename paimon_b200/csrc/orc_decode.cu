@@ -144,22 +144,19 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
     const int nc = s->n_cols();
     cudaStream_t sm = copy_stream();
     Scratch scratch(sm);                               // file images, tables, scratch and the runs until registered
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    struct EvGuard { cudaEvent_t &a, &b; ~EvGuard() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); } } evg{e0, e1};
-    PG_CUDA(cudaEventCreate(&e0));
-    PG_CUDA(cudaEventCreate(&e1));
-    PG_CUDA(cudaEventRecord(e0, sm));
-    if (read_cols)
-        for (int c = 0; c < s->n_key + 2; c++)
-            if (!read_cols[c]) return fail(PG_ERR_INVALID, "orc: key, sequence number and kind columns are always read");
-    std::vector<uint8_t> wanted(nc, 1);
-    for (int c = 0; c < nc; c++) wanted[c] = !read_cols || read_cols[c];
+    RunBuilder b(*s, n_runs, scratch, "orc");
+    SectionTimer tm;
+    PG_CUDA(cudaEventCreate(&tm.e0));
+    PG_CUDA(cudaEventCreate(&tm.e1));
+    PG_CUDA(cudaEventRecord(tm.e0, sm));
+    { pg_status st = b.read_columns(read_cols); if (st) return st; }
+    const std::vector<uint8_t> &wanted = b.read;
 
     // ---- file tails, schema mapping by name, plans
     std::vector<orc::FileTail> tails(nf);
     std::vector<orc::Plan> plans(nf);
     std::vector<const uint8_t *> d_file(nf, nullptr);
-    std::vector<int64_t> run_rows(n_runs, 0), file_row0(nf, 0);
+    std::vector<int64_t> file_row0(nf, 0);
     int64_t file_bytes = 0, page_bytes = 0;
     bool any_compressed = false, any_zstd = false;
     std::vector<uint8_t> col_missing((size_t)n_runs * nc, 0);
@@ -210,17 +207,15 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
             const bool refusal = strstr(e.what(), "is not decoded") != nullptr || strstr(e.what(), "not supported") != nullptr;
             return fail(refusal ? PG_ERR_UNSUPPORTED : PG_ERR_FORMAT, e.what());
         }
-        file_row0[f] = run_rows[files[f].run];
-        run_rows[files[f].run] += (int64_t)tails[f].rows;
+        file_row0[f] = b.place_file(files[f].run, (int64_t)tails[f].rows);
         files_of_run[files[f].run]++;
         file_bytes += files[f].size;
         uint8_t *d = (uint8_t *)scratch.take((size_t)files[f].size + 64);
-        if (!d) return fail(PG_ERR_CUDA, "orc: out of device memory");
+        if (!d) return oom("orc", "a file image", (size_t)files[f].size);
         PG_CUDA(cudaMemcpyAsync(d, files[f].bytes, (size_t)files[f].size, cudaMemcpyHostToDevice, sm));
         d_file[f] = d;
     }
-    for (int r = 0; r < n_runs; r++)
-        if (run_rows[r] > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "orc: more than 2^31 rows in one run");
+    { pg_status st = b.check_rows(); if (st) return st; }
     // a var-len column that only some files of a run have would need offsets filled for the other files' rows
     {
         std::vector<int> present_files((size_t)n_runs * nc, 0);
@@ -237,42 +232,14 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
                     return fail(PG_ERR_UNSUPPORTED, "orc: a var-len column exists in some files of a sorted run only");
     }
 
-    // ---- output columns (validity bitmaps first and contiguous: one memset)
-    std::vector<std::unique_ptr<Run>> &runs = scratch.runs;
-    runs.resize(n_runs);
-    struct OutCol { void *data = nullptr; int32_t *offsets = nullptr; uint32_t *validity = nullptr; };
-    std::vector<OutCol> outs((size_t)n_runs * nc);
-    int64_t decoded_bytes = 0;
-    for (int r = 0; r < n_runs; r++) {
-        const int64_t n = run_rows[r];
-        runs[r] = std::make_unique<Run>(*s, n);
-        const size_t vb = align256((size_t)((n + 31) / 32) * 4 + 64);
-        size_t vbytes = 0, total = 0;
-        // ORC columns are nullable by format: every column the read schema calls nullable gets a bitmap
-        for (int c = 0; c < nc; c++) if (wanted[c] && s->field(c).nullable) vbytes += vb;
-        total = vbytes;
-        std::vector<size_t> o_main(nc);
-        for (int c = 0; c < nc; c++) {
-            const int ow = type_width(s->field(c).type);
-            o_main[c] = total;
-            if (wanted[c]) total += ow ? align256((size_t)n * ow + 64) : align256(4 * (size_t)(n + 1) + 64);
-        }
-        runs[r]->bufs.emplace_back(total + 256);
-        unsigned char *base = runs[r]->bufs.back().get();
-        if (!base) return fail(PG_ERR_CUDA, "orc: out of device memory");
-        if (vbytes) PG_CUDA(cudaMemsetAsync(base, 0, vbytes, sm));
-        size_t vt = 0;
-        for (int c = 0; c < nc; c++) {
-            if (!wanted[c]) continue;
-            OutCol &o = outs[(size_t)r * nc + c];
-            const int ow = type_width(s->field(c).type);
-            if (s->field(c).nullable) { o.validity = (uint32_t *)(base + vt); vt += vb; decoded_bytes += (n + 7) / 8; }
-            if (ow) { o.data = base + o_main[c]; decoded_bytes += n * ow; }
-            else { o.offsets = (int32_t *)(base + o_main[c]); decoded_bytes += 4 * (n + 1); }
-            // var-len lengths are scanned in place: rows nobody writes must read 0; missing columns are all NULL
-            if (!ow || col_missing[(size_t)r * nc + c])
-                PG_CUDA(cudaMemsetAsync(base + o_main[c], 0, ow ? (size_t)n * ow : 4 * (size_t)(n + 1), sm));
-        }
+    // ---- output columns.  ORC columns are nullable by format: every column the read schema calls nullable gets a
+    // bitmap.  Var-len lengths are scanned in place: rows nobody writes must read 0; missing columns are all NULL.
+    {
+        std::vector<uint8_t> bitmap(nc), zero((size_t)n_runs * nc);
+        for (int c = 0; c < nc; c++) bitmap[c] = s->field(c).nullable;
+        for (size_t i = 0; i < zero.size(); i++) zero[i] = is_varlen(s->field((int)(i % nc)).type) || col_missing[i];
+        pg_status st = b.alloc(bitmap, zero);
+        if (st) return st;
     }
 
     // ---- stream and task tables
@@ -283,9 +250,9 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
     uint64_t sc_bytes = 0, dict_entries = 0;
     for (int f = 0; f < nf; f++) { sc_bytes += plans[f].scratch_bytes; dict_entries += plans[f].dict_entries; }
     uint8_t *d_sc = !any_compressed ? nullptr : (uint8_t *)scratch.take((size_t)sc_bytes + 256);
-    if (any_compressed && !d_sc) return fail(PG_ERR_CUDA, "orc: out of device memory");
+    if (any_compressed && !d_sc) return oom("orc", "the stream scratch", (size_t)sc_bytes);
     int32_t *d_dict_off = (int32_t *)scratch.take(4 * (size_t)(dict_entries + 1) + 256);
-    if (!d_dict_off) return fail(PG_ERR_CUDA, "orc: out of device memory");
+    if (!d_dict_off) return oom("orc", "the dictionary offsets", 4 * (size_t)(dict_entries + 1));
     uint64_t sc_base = 0, dict_base = 0;
     for (int f = 0; f < nf; f++) {
         const int s0 = (int)h_streams.size();
@@ -303,7 +270,7 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
         auto idx = [&](int i) { return i < 0 ? -1 : s0 + i; };
         for (const orc::PlanTask &p : plans[f].tasks) {
             const int r = files[f].run;
-            const OutCol &o = outs[(size_t)r * nc + p.col];
+            const OutColumn &o = b.out[(size_t)r * nc + p.col];
             orcdev::Task k;
             memset(&k, 0, sizeof(k));
             k.row0 = file_row0[f] + p.row0;
@@ -324,7 +291,7 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
     const int n_streams = (int)h_streams.size(), n_tasks = (int)h_tasks.size();
     const size_t tb_s = align256(sizeof(OrcStream) * (size_t)std::max(n_streams, 1)), tb_t = align256(sizeof(orcdev::Task) * (size_t)std::max(n_tasks, 1));
     const size_t tb_r = align256(sizeof(OrcTaskRef) * (size_t)std::max(n_tasks, 1)), tb_o = align256(4 * (size_t)std::max(n_tasks, 1));
-    const size_t tb_p = align256(sizeof(void *) * outs.size());
+    const size_t tb_p = align256(sizeof(void *) * b.out.size());
     int sms = 132, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -332,7 +299,7 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
                                                   : std::max(1, std::min(sms * 4, (n_streams + kOrcWarps - 1) / kOrcWarps));
     const size_t tb_lit = any_zstd ? align256((size_t)inflate_ctas * kOrcWarps * (size_t)(zs::kMaxBlock + 64)) : 256;
     unsigned char *tb = (unsigned char *)scratch.take(tb_s + tb_t + tb_r + tb_o + tb_p + tb_lit + 1024);
-    if (!tb) return fail(PG_ERR_CUDA, "orc: out of device memory");
+    if (!tb) return oom("orc", "the stream and task tables", tb_s + tb_t + tb_r + tb_o + tb_p + tb_lit);
     OrcStream *d_streams = (OrcStream *)tb;
     orcdev::Task *d_tasks = (orcdev::Task *)(tb + tb_s);
     OrcTaskRef *d_refs = (OrcTaskRef *)(tb + tb_s + tb_t);
@@ -358,20 +325,16 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
         launches++;
     }
     // ---- var-len columns: lengths -> offsets, exact payload sizes (one read-back), payload
-    std::vector<std::pair<int, int>> vl;                 // (run, col)
-    for (int r = 0; r < n_runs; r++)
-        for (int c = 0; c < nc; c++)
-            if (wanted[c] && is_varlen(s->field(c).type)) vl.push_back({r, c});
-    std::vector<int32_t> totals(vl.size() + 1, 0);
+    std::vector<int32_t> totals(b.out.size(), 0);          // per (run, column)
     int32_t herr = 0;
-    if (!vl.empty()) {
-        int64_t max_n = 0;
-        for (int r = 0; r < n_runs; r++) max_n = std::max(max_n, run_rows[r]);
+    if (std::any_of(b.out.begin(), b.out.end(), [](const OutColumn &o) { return o.offsets != nullptr; })) {
+        const int64_t max_n = *std::max_element(b.run_rows.begin(), b.run_rows.end());
         int64_t *d_sums = (int64_t *)scratch.take(8 * (size_t)(max_n / 4096 + 4));
-        if (!d_sums) return fail(PG_ERR_CUDA, "orc: out of device memory");
-        for (size_t i = 0; i < vl.size(); i++) {
-            const OutCol &o = outs[(size_t)vl[i].first * nc + vl[i].second];
-            const int64_t n = run_rows[vl[i].first];
+        if (!d_sums) return oom("orc", "the offsets scan", 8 * (size_t)(max_n / 4096 + 4));
+        for (size_t i = 0; i < b.out.size(); i++) {
+            const OutColumn &o = b.out[i];
+            if (!o.offsets) continue;
+            const int64_t n = b.run_rows[i / nc];
             launch_offsets_scan(o.offsets, n, d_sums, d_err, sm);
             launches += n > 0 ? 3 : 0;
             PG_CUDA(cudaMemcpyAsync(&totals[i], o.offsets + n, 4, cudaMemcpyDeviceToHost, sm));
@@ -382,24 +345,10 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
             return fail(herr == KERR_OFFSET_OVERFLOW ? PG_ERR_INTERNAL : PG_ERR_FORMAT,
                         herr == KERR_OFFSET_OVERFLOW ? "orc: a var-len column exceeds 2 GiB of payload"
                                                      : "orc: a stream does not decode (malformed file or unsupported encoding)");
-        std::vector<uint8_t *> h_payload(outs.size(), nullptr);
-        for (int r = 0; r < n_runs; r++) {
-            size_t sum = 256;
-            for (size_t i = 0; i < vl.size(); i++) if (vl[i].first == r) sum += align256((size_t)totals[i] + 64);
-            runs[r]->bufs.emplace_back(sum);
-            unsigned char *pl = runs[r]->bufs.back().get();
-            if (!pl) return fail(PG_ERR_CUDA, "orc: out of device memory");
-            size_t pt = 0;
-            for (size_t i = 0; i < vl.size(); i++) {
-                if (vl[i].first != r) continue;
-                outs[(size_t)r * nc + vl[i].second].data = pl + pt;
-                h_payload[(size_t)r * nc + vl[i].second] = pl + pt;
-                runs[r]->varlen_bytes[vl[i].second] = totals[i];
-                decoded_bytes += totals[i];
-                pt += align256((size_t)totals[i] + 64);
-            }
-        }
-        PG_CUDA(cudaMemcpyAsync(d_payload, h_payload.data(), sizeof(void *) * outs.size(), cudaMemcpyHostToDevice, sm));
+        { pg_status st = b.alloc_payload(std::vector<int64_t>(totals.begin(), totals.end())); if (st) return st; }
+        std::vector<uint8_t *> h_payload(b.out.size());   // (k_orc_set_payload reads the var-len entries only)
+        for (size_t i = 0; i < b.out.size(); i++) h_payload[i] = (uint8_t *)b.out[i].data;
+        PG_CUDA(cudaMemcpyAsync(d_payload, h_payload.data(), sizeof(void *) * h_payload.size(), cudaMemcpyHostToDevice, sm));
         if (n_tasks) {
             k_orc_set_payload<<<(n_tasks + 127) / 128, 128, 0, sm>>>(d_tasks, n_tasks, d_task_out, d_payload);
             k_orc_task<1><<<(n_tasks + 31) / 32, 32, 0, sm>>>(d_tasks, d_refs, d_streams, n_tasks, d_err);
@@ -407,41 +356,20 @@ static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, 
         }
         PG_CUDA(cudaStreamSynchronize(sm));               // (h_payload is a local)
     }
-    PG_CUDA(cudaEventRecord(e1, sm));
+    PG_CUDA(cudaEventRecord(tm.e1, sm));
     PG_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, sm));
     PG_CUDA(cudaStreamSynchronize(sm));
     PG_CUDA(cudaGetLastError());
     if (herr != KERR_NONE) return fail(PG_ERR_FORMAT, "orc: a stream does not decode (malformed file or unsupported encoding)");
-    float ms = 0;
-    cudaEventElapsedTime(&ms, e0, e1);
-    int64_t n_rows = 0;
-    for (int r = 0; r < n_runs; r++) {
-        for (int c = 0; c < nc; c++) {
-            const OutCol &o = outs[(size_t)r * nc + c];
-            DevColumn dc;
-            if (wanted[c]) {
-                dc.data = o.data ? o.data : (const void *)runs[r]->bufs[0].get();
-                dc.offsets = o.offsets;
-                dc.validity = (const uint8_t *)o.validity;
-            }
-            runs[r]->cols[c] = dc;
-        }
-        runs[r]->bytes_h2d = r == 0 ? file_bytes : 0;
-        n_rows += run_rows[r];
-        out_runs[r] = g_runs.put(std::move(runs[r]));
-    }
+    b.finish(out_runs, file_bytes, info);
     if (info) {
-        memset(info, 0, sizeof(*info));
-        info->n_rows = n_rows;
         info->file_bytes = file_bytes;
         info->page_bytes = page_bytes;
-        info->decoded_bytes = decoded_bytes;
         info->n_files = nf;
-        info->n_runs = n_runs;
         info->n_chunks = n_tasks;
         info->n_data_pages = n_streams;
         info->launches = launches;
-        info->ms_decode = ms;
+        info->ms_decode = tm.ms();
     }
     return PG_OK;
 }

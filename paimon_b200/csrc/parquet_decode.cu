@@ -1339,14 +1339,6 @@ static pg_status kernel_error_status(int code) {
     }
 }
 
-static pg_status oom(const char *what, size_t bytes) {
-    size_t fr = 0, tot = 0;
-    cudaMemGetInfo(&fr, &tot);
-    cudaGetLastError();
-    return fail(PG_ERR_CUDA, std::string("parquet: out of device memory for ") + what + " (" + std::to_string(bytes >> 20) +
-                                 " MiB wanted, " + std::to_string(fr >> 20) + " of " + std::to_string(tot >> 20) + " MiB free)");
-}
-
 struct SectionFile {
     const uint8_t *bytes;
     int64_t size;
@@ -1355,117 +1347,76 @@ struct SectionFile {
     const pq::FileMetaData *meta; // already parsed (single-file reader), or NULL
 };
 
-static pg_status decode_section(const Schema *s, const std::vector<SectionFile> &files, int n_runs,
-                                const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
-                                pg_section_info *info) {
-    const int nc = s->n_cols();
+// the footers of the files that come without one: device-resident files bring theirs to the host (two small copies per
+// file, two syncs per section), host files are parsed in place
+static pg_status fetch_footers(const std::vector<SectionFile> &files, cudaStream_t sm, std::vector<pq::FileMetaData> &own_meta,
+                               std::vector<const pq::FileMetaData *> &meta) {
     const int nf = (int)files.size();
-    cudaStream_t sm = copy_stream();
-    Scratch scratch(sm);                               // file images, tables, scratch and the runs until registered
-    int launches = 0;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    struct EvGuard { cudaEvent_t &a, &b; ~EvGuard() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); } } evg{e0, e1};
-    PG_CUDA(cudaEventCreate(&e0));
-    PG_CUDA(cudaEventCreate(&e1));
-
-    // ---- file bytes on the device, footers on the host
-    std::vector<const uint8_t *> d_file(nf, nullptr);
-    std::vector<pq::FileMetaData> own_meta(nf);
-    std::vector<const pq::FileMetaData *> meta(nf, nullptr);
-    int64_t file_bytes = 0, h2d = 0;
-    PG_CUDA(cudaEventRecord(e0, sm));
+    std::vector<int> need;
     for (int f = 0; f < nf; f++) {
-        const SectionFile &sf = files[f];
-        if (!sf.bytes || sf.size < 12) return fail(PG_ERR_FORMAT, "parquet: missing PAR1 magic (encrypted or not a Parquet file)");
-        if (sf.run < 0 || sf.run >= n_runs) return fail(PG_ERR_INVALID, "parquet section: run index out of range");
-        file_bytes += sf.size;
-        if (sf.mem == PG_MEM_DEVICE) d_file[f] = sf.bytes;
-        else {
-            uint8_t *d = (uint8_t *)scratch.take((size_t)sf.size + 64);
-            if (!d) return oom("a file image", (size_t)sf.size);
-            PG_CUDA(cudaMemcpyAsync(d, sf.bytes, (size_t)sf.size, cudaMemcpyHostToDevice, sm));
-            d_file[f] = d;
-            h2d += sf.size;
-        }
+        if (files[f].meta) meta[f] = files[f].meta;
+        else if (files[f].mem == PG_MEM_DEVICE) need.push_back(f);
     }
-    {
-        // device-resident files: bring the footers to the host (two small copies per file, two syncs per section)
-        std::vector<int> need;
-        for (int f = 0; f < nf; f++) {
-            if (files[f].meta) meta[f] = files[f].meta;
-            else if (files[f].mem == PG_MEM_DEVICE) need.push_back(f);
-        }
-        std::vector<uint8_t> tails(8 * need.size() + 8);
-        SmallReads rb(sm);
+    std::vector<uint8_t> tails(8 * need.size() + 8);
+    SmallReads rb(sm);
+    for (size_t i = 0; i < need.size(); i++) {
+        pg_status rs = rb.add(tails.data() + 8 * i, files[need[i]].bytes + files[need[i]].size - 8, 8);
+        if (rs) return rs;
+    }
+    if (!need.empty()) { pg_status rs = rb.finish(); if (rs) return rs; }
+    std::vector<std::vector<uint8_t>> footers(need.size());
+    try {
         for (size_t i = 0; i < need.size(); i++) {
-            pg_status rs = rb.add(tails.data() + 8 * i, files[need[i]].bytes + files[need[i]].size - 8, 8);
+            const int64_t flen = pq::footer_length(tails.data() + 8 * i);
+            if (flen + 12 > files[need[i]].size) return fail(PG_ERR_FORMAT, "parquet: bad footer length");
+            footers[i].resize((size_t)flen + 8);
+            pg_status rs = rb.add(footers[i].data(), files[need[i]].bytes + files[need[i]].size - 8 - flen, (size_t)flen);
             if (rs) return rs;
         }
         if (!need.empty()) { pg_status rs = rb.finish(); if (rs) return rs; }
-        std::vector<std::vector<uint8_t>> footers(need.size());
-        try {
-            for (size_t i = 0; i < need.size(); i++) {
-                const int64_t flen = pq::footer_length(tails.data() + 8 * i);
-                if (flen + 12 > files[need[i]].size) return fail(PG_ERR_FORMAT, "parquet: bad footer length");
-                footers[i].resize((size_t)flen + 8);
-                pg_status rs = rb.add(footers[i].data(), files[need[i]].bytes + files[need[i]].size - 8 - flen, (size_t)flen);
-                if (rs) return rs;
-            }
-            if (!need.empty()) { pg_status rs = rb.finish(); if (rs) return rs; }
-            for (size_t i = 0; i < need.size(); i++) {
-                own_meta[need[i]] = pq::parse_footer_thrift(footers[i].data(), (int64_t)footers[i].size() - 8);
-                meta[need[i]] = &own_meta[need[i]];
-            }
-            for (int f = 0; f < nf; f++)
-                if (!meta[f]) {
-                    own_meta[f] = pq::parse_footer(files[f].bytes, files[f].size);
-                    meta[f] = &own_meta[f];
-                }
-        } catch (const std::exception &e) {
-            return fail(PG_ERR_FORMAT, e.what());
+        for (size_t i = 0; i < need.size(); i++) {
+            own_meta[need[i]] = pq::parse_footer_thrift(footers[i].data(), (int64_t)footers[i].size() - 8);
+            meta[need[i]] = &own_meta[need[i]];
         }
+        for (int f = 0; f < nf; f++)
+            if (!meta[f]) {
+                own_meta[f] = pq::parse_footer(files[f].bytes, files[f].size);
+                meta[f] = &own_meta[f];
+            }
+    } catch (const std::exception &e) {
+        return fail(PG_ERR_FORMAT, e.what());
     }
-    if (read_cols)
-        for (int c = 0; c < s->n_key + 2; c++)
-            if (!read_cols[c]) return fail(PG_ERR_INVALID, "parquet: key, sequence number and kind columns are always read");
-    std::vector<uint8_t> any_optional(nc, 0), wanted(nc, 1);
-    std::vector<std::vector<int>> file_col(nf);
-    for (int c = 0; c < nc; c++) wanted[c] = !read_cols || read_cols[c];
-    for (int f = 0; f < nf; f++) {
-        pg_status st = map_file_schema(s, *meta[f], names, read_cols, &file_col[f]);
-        if (st) return st;
-        for (int c = 0; c < nc; c++) {
-            const int fc = file_col[f][c];
-            if (fc == -1 || (fc >= 0 && meta[f]->schema[fc + 1].repetition == pq::R_OPTIONAL)) any_optional[c] = 1;
-        }
-    }
+    return PG_OK;
+}
 
-    // ---- rows: a file's rows land behind the rows of the files in front of it in its run
-    std::vector<int64_t> run_rows(n_runs, 0), file_row0(nf, 0);
-    std::vector<std::vector<int>> run_files(n_runs);
-    for (int f = 0; f < nf; f++) {
-        file_row0[f] = run_rows[files[f].run];
-        run_rows[files[f].run] += meta[f]->num_rows;
-        run_files[files[f].run].push_back(f);
-    }
-    for (int r = 0; r < n_runs; r++)
-        if (run_rows[r] > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet: more than 2^31 rows in one run");
-
-    // ---- chunk table, ordered (run, column, file, row group): the pages of a (run, column) end up contiguous
+// the chunk table, ordered (run, column, file, row group) so that the pages of a (run, column) end up contiguous, and
+// the (run, var-len column) pairs
+struct ChunkTables {
     std::vector<PqChunk> chunks;
     std::vector<PqPair> pairs;
+    std::vector<uint8_t> col_missing;     // per (run, column): 1 = some, 2 = every file of the run lacks the column
     bool any_snappy = false, any_delta = false, any_zstd = false;
     int64_t pair_rows = 0;
+};
+
+static pg_status build_chunk_tables(const Schema *s, const std::vector<SectionFile> &files,
+                                    const std::vector<const uint8_t *> &d_file, const std::vector<const pq::FileMetaData *> &meta,
+                                    const std::vector<std::vector<int>> &file_col, const std::vector<int64_t> &file_row0,
+                                    const RunBuilder &b, ChunkTables &t) {
+    const int nc = s->n_cols();
+    const int n_runs = (int)b.run_rows.size();
+    std::vector<std::vector<int>> run_files(n_runs);
+    for (int f = 0; f < (int)files.size(); f++) run_files[files[f].run].push_back(f);
     // (run, column) pairs some / all of whose files lack the column: the rows of those files are NULL
-    std::vector<uint8_t> col_missing((size_t)n_runs * nc, 0);          // 1 = in some files, 2 = in every file of the run
+    t.col_missing.assign((size_t)n_runs * nc, 0);
     for (int r = 0; r < n_runs; r++) {
         for (int c = 0; c < nc; c++) {
-            if (!wanted[c]) continue;
-            const int chunk0 = (int)chunks.size();
+            if (!b.read[c]) continue;
+            const int chunk0 = (int)t.chunks.size();
             int n_missing = 0;
             for (int f : run_files[r]) if (file_col[f][c] < 0) n_missing++;
             if (n_missing > 0) {
-                col_missing[(size_t)r * nc + c] = n_missing == (int)run_files[r].size() ? 2 : 1;
+                t.col_missing[(size_t)r * nc + c] = n_missing == (int)run_files[r].size() ? 2 : 1;
                 if (n_missing != (int)run_files[r].size() && is_varlen(s->field(c).type))
                     return fail(PG_ERR_UNSUPPORTED, "parquet: a var-len column exists in some files of a sorted run only "
                                                     "(mixed table schemas inside one run: not decoded on device)");
@@ -1495,64 +1446,125 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
                     ch.phys_width = phys_width_of(cc.type);
                     ch.cast = phys_cast(s->field(c).type, cc.type);
                     if (cc.type != m.schema[fc + 1].type) return fail(PG_ERR_FORMAT, "parquet: column chunk type differs from the schema");
-                    if (cc.codec == pq::C_SNAPPY) any_snappy = true;
-                    if (cc.codec == pq::C_ZSTD || cc.codec == pq::C_GZIP) any_zstd = true;
-                    for (int32_t e : cc.encodings) if (e == pq::E_DELTA_BINARY_PACKED) any_delta = true;
-                    if (cc.num_values > 0) chunks.push_back(ch);
+                    if (cc.codec == pq::C_SNAPPY) t.any_snappy = true;
+                    if (cc.codec == pq::C_ZSTD || cc.codec == pq::C_GZIP) t.any_zstd = true;
+                    for (int32_t e : cc.encodings) if (e == pq::E_DELTA_BINARY_PACKED) t.any_delta = true;
+                    if (cc.num_values > 0) t.chunks.push_back(ch);
                     rg_row0 += g.num_rows;
                     rows += g.num_rows;
                 }
                 if (rows != m.num_rows) return fail(PG_ERR_FORMAT, "parquet: row group row counts do not add up");
             }
             if (is_varlen(s->field(c).type)) {
-                PqPair pr{r, c, chunk0, (int)chunks.size(), pair_rows, (int)pairs.size(), 0};
-                pairs.push_back(pr);
-                pair_rows += run_rows[r];
+                PqPair pr{r, c, chunk0, (int)t.chunks.size(), t.pair_rows, (int)t.pairs.size(), 0};
+                t.pairs.push_back(pr);
+                t.pair_rows += b.run_rows[r];
             }
         }
     }
-    const int n_chunks = (int)chunks.size(), n_pairs = (int)pairs.size();
+    return PG_OK;
+}
 
-    // ---- output columns: one recycled buffer per run (validity bitmaps first and contiguous: one memset)
-    std::vector<std::unique_ptr<Run>> &runs = scratch.runs;
-    runs.resize(n_runs);
-    std::vector<PqOut> outs((size_t)n_runs * nc);
-    int64_t decoded_bytes = 0;
-    bool any_empty = false;
-    for (int r = 0; r < n_runs; r++) {
-        const int64_t n = run_rows[r];
-        if (n == 0) any_empty = true;
-        runs[r] = std::make_unique<Run>(*s, n);
-        size_t vbytes = 0, total = 0;
-        const size_t vb = align256((size_t)((n + 31) / 32) * 4 + 64);
-        for (int c = 0; c < nc; c++) if (wanted[c] && any_optional[c]) vbytes += vb;
-        total = vbytes;
-        std::vector<size_t> o_main(nc);
-        for (int c = 0; c < nc; c++) {
-            const int ow = type_width(s->field(c).type);
-            o_main[c] = total;
-            if (wanted[c]) total += ow ? align256((size_t)n * ow + 64) : align256(4 * (size_t)(n + 1) + 64);
-        }
-        runs[r]->bufs.emplace_back(total + 256);
-        unsigned char *base = runs[r]->bufs.back().get();
-        if (!base) return oom("the columns of a run", total);
-        if (vbytes) PG_CUDA(cudaMemsetAsync(base, 0, vbytes, sm));
-        size_t vt = 0;
-        for (int c = 0; c < nc; c++) {
-            PqOut &o = outs[(size_t)r * nc + c];
-            memset(&o, 0, sizeof(o));
-            const int ow = type_width(s->field(c).type);
-            o.out_width = ow;
-            o.is_bool = s->field(c).type == PG_BOOL;
-            if (!wanted[c]) continue;                    // not part of the read type: the run has no such column
-            if (any_optional[c]) { o.validity = (uint32_t *)(base + vt); vt += vb; decoded_bytes += (n + 7) / 8; }
-            if (ow) { o.data = base + o_main[c]; decoded_bytes += n * ow; }
-            else { o.offsets = (int32_t *)(base + o_main[c]); decoded_bytes += 4 * (n + 1); }
-            // rows of files that lack the column stay NULL (validity is zeroed); give them defined contents
-            if (col_missing[(size_t)r * nc + c])
-                PG_CUDA(cudaMemsetAsync(base + o_main[c], 0, ow ? (size_t)n * ow : 4 * (size_t)(n + 1), sm));
+// The value walk and the expansion.  With var-len columns, the value walk (one lane per page: latency-bound at low
+// occupancy) and the PLAIN BYTE_ARRAY pages that need it run on a side stream beside the expansion of all other pages.
+static pg_status expand_pages(cudaStream_t sm, bool byte_arrays, PqPage *d_pages, int np, const PqPage *d_dicts,
+                              const PqChunk *d_chunks, const PqOut *d_outs, int nc, const int32_t *d_ids, int32_t *d_vstart,
+                              const int32_t *d_dict_off, const int32_t *d_dict_len, int32_t *d_err, int *launches) {
+    if (!byte_arrays) {
+        k_pq_expand<<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
+                                                d_dict_len, d_err, 0);
+        (*launches)++;
+        return PG_OK;
+    }
+    static thread_local cudaStream_t side = nullptr;
+    static thread_local cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+    if (!side) {
+        // (highest priority: its few, long-running CTAs must get their slots before the expansion's 250 k short
+        // ones fill every SM — otherwise the walk only starts when the expansion drains)
+        int prio_lo = 0, prio_hi = 0;
+        cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
+        PG_CUDA(cudaStreamCreateWithPriority(&side, cudaStreamNonBlocking, prio_hi));
+        PG_CUDA(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
+        PG_CUDA(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
+    }
+    PG_CUDA(cudaEventRecord(ev_fork, sm));
+    PG_CUDA(cudaStreamWaitEvent(side, ev_fork, 0));
+    k_pq_walk_values<<<(np + kWvWarps * 32 - 1) / (kWvWarps * 32), kWvWarps * 32, 0, side>>>(
+        d_pages, np, d_chunks, d_vstart, d_err);
+    // the PLAIN BYTE_ARRAY pages follow their walk on the side stream; everything else expands on the main one
+    k_pq_expand<<<np, kExpThreads, 0, side>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
+                                              d_dict_len, d_err, 2);
+    PG_CUDA(cudaEventRecord(ev_join, side));
+    k_pq_expand<<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
+                                            d_dict_len, d_err, 1);
+    PG_CUDA(cudaStreamWaitEvent(sm, ev_join, 0));
+    *launches += 3;
+    return PG_OK;
+}
+
+static pg_status decode_section(const Schema *s, const std::vector<SectionFile> &files, int n_runs,
+                                const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
+                                pg_section_info *info) {
+    const int nc = s->n_cols();
+    const int nf = (int)files.size();
+    cudaStream_t sm = copy_stream();
+    Scratch scratch(sm);                               // file images, tables, scratch and the runs until registered
+    RunBuilder b(*s, n_runs, scratch, "parquet");
+    int launches = 0;
+    SectionTimer tm;
+    PG_CUDA(cudaEventCreate(&tm.e0));
+    PG_CUDA(cudaEventCreate(&tm.e1));
+
+    // ---- file bytes on the device, footers on the host
+    std::vector<const uint8_t *> d_file(nf, nullptr);
+    std::vector<pq::FileMetaData> own_meta(nf);
+    std::vector<const pq::FileMetaData *> meta(nf, nullptr);
+    int64_t file_bytes = 0, h2d = 0;
+    PG_CUDA(cudaEventRecord(tm.e0, sm));
+    for (int f = 0; f < nf; f++) {
+        const SectionFile &sf = files[f];
+        if (!sf.bytes || sf.size < 12) return fail(PG_ERR_FORMAT, "parquet: missing PAR1 magic (encrypted or not a Parquet file)");
+        if (sf.run < 0 || sf.run >= n_runs) return fail(PG_ERR_INVALID, "parquet section: run index out of range");
+        file_bytes += sf.size;
+        if (sf.mem == PG_MEM_DEVICE) d_file[f] = sf.bytes;
+        else {
+            uint8_t *d = (uint8_t *)scratch.take((size_t)sf.size + 64);
+            if (!d) return oom("parquet", "a file image", (size_t)sf.size);
+            PG_CUDA(cudaMemcpyAsync(d, sf.bytes, (size_t)sf.size, cudaMemcpyHostToDevice, sm));
+            d_file[f] = d;
+            h2d += sf.size;
         }
     }
+    { pg_status st = fetch_footers(files, sm, own_meta, meta); if (st) return st; }
+    { pg_status st = b.read_columns(read_cols); if (st) return st; }
+    std::vector<uint8_t> any_optional(nc, 0);
+    std::vector<std::vector<int>> file_col(nf);
+    for (int f = 0; f < nf; f++) {
+        pg_status st = map_file_schema(s, *meta[f], names, read_cols, &file_col[f]);
+        if (st) return st;
+        for (int c = 0; c < nc; c++) {
+            const int fc = file_col[f][c];
+            if (fc == -1 || (fc >= 0 && meta[f]->schema[fc + 1].repetition == pq::R_OPTIONAL)) any_optional[c] = 1;
+        }
+    }
+    std::vector<int64_t> file_row0(nf, 0);
+    for (int f = 0; f < nf; f++) file_row0[f] = b.place_file(files[f].run, meta[f]->num_rows);
+    { pg_status st = b.check_rows(); if (st) return st; }
+    ChunkTables ct;
+    { pg_status st = build_chunk_tables(s, files, d_file, meta, file_col, file_row0, b, ct); if (st) return st; }
+    const int n_chunks = (int)ct.chunks.size(), n_pairs = (int)ct.pairs.size();
+
+    // ---- output columns (the rows of files that lack a column stay NULL and get defined contents)
+    { pg_status st = b.alloc(any_optional, ct.col_missing); if (st) return st; }
+    std::vector<PqOut> outs((size_t)n_runs * nc);
+    auto fill_outs = [&] {
+        for (size_t i = 0; i < outs.size(); i++) {
+            const int t = s->field((int)(i % nc)).type;
+            outs[i] = PqOut{b.out[i].data, b.out[i].offsets, b.out[i].validity, type_width(t), t == PG_BOOL};
+        }
+    };
+    fill_outs();
+    const bool any_empty = std::find(b.run_rows.begin(), b.run_rows.end(), 0) != b.run_rows.end();
 
     // ---- tables to the device, page count pass
     const size_t tb_chunks = align256(sizeof(PqChunk) * (size_t)std::max(n_chunks, 1));
@@ -1560,7 +1572,7 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     const size_t tb_pairs = align256(sizeof(PqPair) * (size_t)std::max(n_pairs, 1));
     const size_t tb_tot = align256(sizeof(int64_t) * (size_t)(8 + n_pairs));
     unsigned char *tb = (unsigned char *)scratch.take(tb_chunks + tb_outs + tb_pairs + tb_tot + 256);
-    if (!tb) return oom("the chunk tables", tb_chunks + tb_outs + tb_pairs + tb_tot);
+    if (!tb) return oom("parquet", "the chunk tables", tb_chunks + tb_outs + tb_pairs + tb_tot);
     PqChunk *d_chunks = (PqChunk *)tb;
     PqOut *d_outs = (PqOut *)(tb + tb_chunks);
     PqPair *d_pairs = (PqPair *)(tb + tb_chunks + tb_outs);
@@ -1569,9 +1581,9 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     PG_CUDA(cudaMemsetAsync(d_totals, 0, tb_tot, sm));
     // (tables go through small_h2d: a kernel reads them out of mapped host memory, so they do not queue behind an
     // asynchronous upload of the next section on the copy engine)
-    if (n_chunks) { pg_status ts = small_h2d(d_chunks, chunks.data(), sizeof(PqChunk) * n_chunks, sm); if (ts) return ts; }
+    if (n_chunks) { pg_status ts = small_h2d(d_chunks, ct.chunks.data(), sizeof(PqChunk) * n_chunks, sm); if (ts) return ts; }
     { pg_status ts = small_h2d(d_outs, outs.data(), sizeof(PqOut) * outs.size(), sm); if (ts) return ts; }
-    if (n_pairs) { pg_status ts = small_h2d(d_pairs, pairs.data(), sizeof(PqPair) * n_pairs, sm); if (ts) return ts; }
+    if (n_pairs) { pg_status ts = small_h2d(d_pairs, ct.pairs.data(), sizeof(PqPair) * n_pairs, sm); if (ts) return ts; }
     int64_t h_tot[8] = {0, 0, 0, 0, 0, 0, 0, 0};
     if (n_chunks) {
         k_pq_walk<false><<<(n_chunks + 63) / 64, 64, 0, sm>>>(d_chunks, n_chunks, nullptr, nullptr, nullptr, d_err);
@@ -1596,9 +1608,9 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     const size_t sb_sc = align256((size_t)sc_bytes + 64);
     const size_t sb_de = align256(4 * (size_t)(dict_entries + 1));
     const size_t sb_ids = align256(4 * (size_t)(ids_entries + 1));
-    const size_t sb_vs = align256(4 * (size_t)(pair_rows + n_pages + n_pairs + 2));
+    const size_t sb_vs = align256(4 * (size_t)(ct.pair_rows + n_pages + n_pairs + 2));
     int zs_ctas = 0;
-    if (any_zstd) {
+    if (ct.any_zstd) {
         int dev = 0, sms = 132;
         cudaGetDevice(&dev);
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
@@ -1606,7 +1618,7 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     }
     const size_t sb_zs = align256((size_t)zs_ctas * kZsWarps * (size_t)(zs::kMaxBlock + 64));
     unsigned char *sbuf = (unsigned char *)scratch.take(sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs + 256);
-    if (!sbuf) return oom("the page table and scratch", sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs);
+    if (!sbuf) return oom("parquet", "the page table and scratch", sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs);
     PqPage *d_pages = (PqPage *)sbuf;
     PqPage *d_dicts = (PqPage *)(sbuf + sb_pages);
     uint8_t *d_sc = sbuf + sb_pages + sb_dicts;
@@ -1620,16 +1632,16 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     if (np > 0) {
         k_pq_walk<true><<<(n_chunks + 63) / 64, 64, 0, sm>>>(d_chunks, n_chunks, d_pages, d_dicts, d_sc, d_err);
         launches++;
-        if (any_snappy) {
+        if (ct.any_snappy) {
             const int64_t th = (int64_t)(np + nd) * 32;
             k_pq_snappy<<<(unsigned)((th + 127) / 128), 128, 0, sm>>>(d_pages, np, d_dicts, nd, d_chunks, d_err);
             launches++;
         }
-        if (any_zstd && zs_ctas > 0) {
+        if (ct.any_zstd && zs_ctas > 0) {
             k_pq_zstd<<<zs_ctas, kZsWarps * 32, 0, sm>>>(d_pages, np, d_dicts, nd, d_chunks, d_zs_lit, (int32_t *)(d_totals + 7), d_err);
             launches++;
         }
-        if (any_delta) {
+        if (ct.any_delta) {
             k_pq_delta<<<(unsigned)(((int64_t)np * 32 + 127) / 128), 128, 0, sm>>>(d_pages, np, d_chunks, d_err);
             launches++;
         }
@@ -1658,80 +1670,22 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
 
     // ---- var-len payload buffers (one per run), then the value walk and the expansion
     if (n_pairs) {
-        for (int r = 0; r < n_runs; r++) {
-            size_t sum = 256;
-            for (const PqPair &pr : pairs) if (pr.run == r) sum += align256((size_t)pair_tot[pr.idx] + 64);
-            runs[r]->bufs.emplace_back(sum);
-            unsigned char *pl = runs[r]->bufs.back().get();
-            if (!pl) return oom("the var-len payload of a run", sum);
-            size_t pt = 0;
-            for (const PqPair &pr : pairs) {
-                if (pr.run != r) continue;
-                outs[(size_t)r * nc + pr.col].data = pl + pt;
-                runs[r]->varlen_bytes[pr.col] = pair_tot[pr.idx];
-                decoded_bytes += pair_tot[pr.idx];
-                pt += align256((size_t)pair_tot[pr.idx] + 64);
-            }
-        }
+        std::vector<int64_t> payload((size_t)n_runs * nc, 0);
+        for (const PqPair &pr : ct.pairs) payload[(size_t)pr.run * nc + pr.col] = pair_tot[pr.idx];
+        { pg_status st = b.alloc_payload(payload); if (st) return st; }
+        fill_outs();
         { pg_status ts = small_h2d(d_outs, outs.data(), sizeof(PqOut) * outs.size(), sm); if (ts) return ts; }
     }
     if (np > 0) {
-        if (n_pairs) {
-            // the value walk (one lane per page: latency-bound at low occupancy) and the PLAIN BYTE_ARRAY pages that need it
-            // run on a side stream beside the expansion of all other pages
-            static thread_local cudaStream_t side = nullptr;
-            static thread_local cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-            if (!side) {
-                // (highest priority: its few, long-running CTAs must get their slots before the expansion's 250 k short
-                // ones fill every SM — otherwise the walk only starts when the expansion drains)
-                int prio_lo = 0, prio_hi = 0;
-                cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-                PG_CUDA(cudaStreamCreateWithPriority(&side, cudaStreamNonBlocking, prio_hi));
-                PG_CUDA(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
-                PG_CUDA(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
-            }
-            // PAIMON_GPU_TRACE=1: per-phase times of this part of the section on stderr (experiments)
-            static const bool trace = getenv("PAIMON_GPU_TRACE") != nullptr;
-            cudaEvent_t tv[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
-            if (trace) for (auto &e : tv) cudaEventCreate(&e);
-            PG_CUDA(cudaEventRecord(ev_fork, sm));
-            if (trace) cudaEventRecord(tv[0], sm);
-            PG_CUDA(cudaStreamWaitEvent(side, ev_fork, 0));
-            k_pq_walk_values<<<(np + kWvWarps * 32 - 1) / (kWvWarps * 32), kWvWarps * 32, 0, side>>>(
-                d_pages, np, d_chunks, d_vstart, d_err);
-            if (trace) cudaEventRecord(tv[1], side);
-            // the PLAIN BYTE_ARRAY pages follow their walk on the side stream; everything else expands on the main one
-            k_pq_expand<<<np, kExpThreads, 0, side>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                                      d_dict_len, d_err, 2);
-            PG_CUDA(cudaEventRecord(ev_join, side));
-            if (trace) cudaEventRecord(tv[3], side);
-            k_pq_expand<<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                                    d_dict_len, d_err, 1);
-            if (trace) cudaEventRecord(tv[2], sm);
-            PG_CUDA(cudaStreamWaitEvent(sm, ev_join, 0));
-            if (trace) {
-                cudaEventRecord(tv[4], sm);
-                cudaEventSynchronize(tv[4]);
-                float a = 0, b = 0, c = 0, d = 0;
-                cudaEventElapsedTime(&a, tv[0], tv[1]);
-                cudaEventElapsedTime(&b, tv[0], tv[2]);
-                cudaEventElapsedTime(&c, tv[0], tv[3]);
-                cudaEventElapsedTime(&d, tv[0], tv[4]);
-                fprintf(stderr, "[decode trace] since fork: value walk done %.2f ms, expand(no walk) done %.2f, expand(byte arrays) done %.2f, joined %.2f\n", a, b, c, d);
-                for (auto &e : tv) cudaEventDestroy(e);
-            }
-            launches += 3;
-        } else {
-            k_pq_expand<<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                                    d_dict_len, d_err, 0);
-            launches++;
-        }
+        pg_status st = expand_pages(sm, n_pairs > 0, d_pages, np, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
+                                    d_dict_len, d_err, &launches);
+        if (st) return st;
     }
     if (any_empty && n_pairs) {
         k_pq_zero_first_offset<<<(n_runs * nc + 127) / 128, 128, 0, sm>>>(d_outs, n_runs * nc);
         launches++;
     }
-    PG_CUDA(cudaEventRecord(e1, sm));
+    PG_CUDA(cudaEventRecord(tm.e1, sm));
     {
         SmallReads rb(sm);
         pg_status rs = rb.add(h_tot, d_totals, sizeof(int64_t) * 8);
@@ -1743,36 +1697,16 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
         const int herr = (int)(h_tot[6] & 0xffffffff);
         if (herr != KERR_NONE) return kernel_error_status(herr);
     }
-    float ms = 0;
-    cudaEventElapsedTime(&ms, e0, e1);
-
-    for (int r = 0; r < n_runs; r++) {
-        for (int c = 0; c < nc; c++) {
-            const PqOut &o = outs[(size_t)r * nc + c];
-            DevColumn dc;
-            if (wanted[c]) {
-                dc.data = o.data ? o.data : (const void *)runs[r]->bufs[0].get();
-                dc.offsets = o.offsets;
-                dc.validity = (const uint8_t *)o.validity;
-            }
-            runs[r]->cols[c] = dc;
-        }
-        runs[r]->bytes_h2d = r == 0 ? h2d : 0;
-        out_runs[r] = g_runs.put(std::move(runs[r]));
-    }
+    b.finish(out_runs, h2d, info);
     if (info) {
-        memset(info, 0, sizeof(*info));
-        for (int r = 0; r < n_runs; r++) info->n_rows += run_rows[r];
         info->file_bytes = file_bytes;
         info->page_bytes = page_bytes;
-        info->decoded_bytes = decoded_bytes;
         info->n_files = nf;
-        info->n_runs = n_runs;
         info->n_chunks = n_chunks;
         info->n_data_pages = np;
         info->n_dictionary_pages = nd;
         info->launches = launches;
-        info->ms_decode = ms;
+        info->ms_decode = tm.ms();
     }
     return PG_OK;
 }
@@ -1922,102 +1856,68 @@ static pg_status apply_deletion_vector(uint64_t run_h, const uint8_t *deleted, i
     if (n_bits < 0) return fail(PG_ERR_INVALID, "negative deletion vector size");
     cudaStream_t sm = 0;
     Scratch scratch(sm);                               // temporaries, and the new run until it is registered
-    auto dv_oom = [] { return fail(PG_ERR_CUDA, "deletion vector: out of device memory"); };
     // ---- kept rows
     const int64_t nb = std::max<int64_t>((n + 4095) / 4096, 1);
     uint8_t *d_del = (uint8_t *)scratch.take((size_t)(n_bits + 7) / 8 + 16);
     int32_t *d_incl = (int32_t *)scratch.take(sizeof(int32_t) * (size_t)(n + 1));
-    int64_t *d_sums = (int64_t *)scratch.take(sizeof(int64_t) * (size_t)nb);
+    int64_t *d_sums = (int64_t *)scratch.take(sizeof(int64_t) * (size_t)nb);     // (also the offsets scans: m <= n)
     int32_t *d_err = (int32_t *)scratch.take(16);
-    if (!d_del || !d_incl || !d_sums || !d_err) return dv_oom();
+    if (!d_del || !d_incl || !d_sums || !d_err) return oom("deletion vector", "the row scan", sizeof(int32_t) * (size_t)n);
     PG_CUDA(cudaMemsetAsync(d_err, 0, 4, sm));
     if (n_bits > 0) PG_CUDA(cudaMemcpyAsync(d_del, deleted, (size_t)(n_bits + 7) / 8, cudaMemcpyHostToDevice, sm));
     int64_t m = 0;
     if (n > 0) {
         k_dv_keep<<<(int)((n + 255) / 256), 256, 0, sm>>>(d_del, n_bits, n, d_incl);
-        k_scan_block_sums<<<(int)nb, 256, 0, sm>>>(d_incl, n, d_sums);
-        k_scan_block_prefix<<<1, 32, 0, sm>>>(d_sums, nb, d_err);
-        k_scan_apply<<<(int)nb, 256, 0, sm>>>(d_incl, n, d_sums);
+        launch_inclusive_scan(d_incl, n, d_sums, d_err, sm);
         int32_t last = 0;
         PG_CUDA(cudaMemcpyAsync(&last, d_incl + n - 1, 4, cudaMemcpyDeviceToHost, sm));
         PG_CUDA(cudaStreamSynchronize(sm));
         m = last;
     }
-    scratch.runs.push_back(std::make_unique<Run>(*s, m));
-    Run *run = scratch.runs.back().get();
     int32_t *d_src = (int32_t *)scratch.take(sizeof(int32_t) * (size_t)std::max<int64_t>(m, 1));
-    if (!d_src) return dv_oom();
+    if (!d_src) return oom("deletion vector", "the row sources", sizeof(int32_t) * (size_t)m);
     if (n > 0) k_dv_sources<<<(int)((n + 255) / 256), 256, 0, sm>>>(d_incl, n, d_src);
-    // ---- one allocation for fixed-width data, offsets and validity; payloads follow once their sizes are known
-    std::vector<size_t> o_data(nc), o_off(nc), o_val(nc);
-    size_t total = 0;
+    // ---- the kept rows of the columns the input has, with the bitmaps the input has
+    RunBuilder b(*s, 1, scratch, "deletion vector");
+    b.place_file(0, m);
+    std::vector<uint8_t> bitmap(nc), no_zero(nc, 0);
     for (int c = 0; c < nc; c++) {
-        pg_field f = s->field(c);
-        o_data[c] = total; total += is_varlen(f.type) ? 0 : align256((size_t)m * type_width(f.type) + 16);
-        o_off[c] = total; total += is_varlen(f.type) ? align256(sizeof(int32_t) * (size_t)(m + 1) + 16) : 0;
-        o_val[c] = total; total += in->cols[c].validity ? align256((size_t)((m + 31) / 32) * 4 + 16) : 0;
+        b.read[c] = in->cols[c].data || in->cols[c].offsets;
+        bitmap[c] = in->cols[c].validity != nullptr;
     }
-    run->bufs.emplace_back(total + 256);
-    unsigned char *base = run->bufs.back().get();
-    if (!base) return dv_oom();
+    st = b.alloc(bitmap, no_zero);
+    if (st) return st;
     const int gm = (int)((std::max<int64_t>(m, 1) + 255) / 256);
-    std::vector<int64_t *> sums(nc, nullptr);
     for (int c = 0; c < nc; c++) {
-        pg_field f = s->field(c);
+        if (!b.read[c]) continue;
         const DevColumn &ic = in->cols[c];
-        DevColumn oc;
-        if (ic.validity) {
-            oc.validity = base + o_val[c];
-            if (m > 0) k_dv_gather_bits<<<gm, 256, 0, sm>>>(ic.validity, d_src, m, (uint32_t *)(base + o_val[c]));
-        }
-        if (!is_varlen(f.type)) {
-            oc.data = base + o_data[c];
-            if (m > 0) k_dv_gather_fixed<<<gm, 256, 0, sm>>>(ic.data, type_width(f.type), d_src, m, base + o_data[c]);
+        const OutColumn &oc = b.out[c];
+        if (oc.validity && m > 0) k_dv_gather_bits<<<gm, 256, 0, sm>>>(ic.validity, d_src, m, oc.validity);
+        if (!is_varlen(s->field(c).type)) {
+            if (m > 0) k_dv_gather_fixed<<<gm, 256, 0, sm>>>(ic.data, type_width(s->field(c).type), d_src, m, oc.data);
         } else {
-            int32_t *oo = (int32_t *)(base + o_off[c]);
-            oc.offsets = oo;
-            k_dv_lengths<<<gm, 256, 0, sm>>>(ic.offsets, d_src, m, oo);
-            if (m > 0) {
-                const int64_t mb = (m + 4095) / 4096;
-                sums[c] = (int64_t *)scratch.take(sizeof(int64_t) * (size_t)mb);
-                if (!sums[c]) return dv_oom();
-                k_scan_block_sums<<<(int)mb, 256, 0, sm>>>(oo + 1, m, sums[c]);
-                k_scan_block_prefix<<<1, 32, 0, sm>>>(sums[c], mb, d_err);
-                k_scan_apply<<<(int)mb, 256, 0, sm>>>(oo + 1, m, sums[c]);
-            }
+            k_dv_lengths<<<gm, 256, 0, sm>>>(ic.offsets, d_src, m, oc.offsets);
+            launch_offsets_scan(oc.offsets, m, d_sums, d_err, sm);
         }
-        run->cols[c] = oc;
     }
     // payload sizes: one read-back for all var-len columns
     std::vector<int32_t> totals(nc, 0);
     for (int c = 0; c < nc; c++)
-        if (is_varlen(s->field(c).type) && m > 0)
-            PG_CUDA(cudaMemcpyAsync(&totals[c], run->cols[c].offsets + m, 4, cudaMemcpyDeviceToHost, sm));
+        if (b.out[c].offsets && m > 0)
+            PG_CUDA(cudaMemcpyAsync(&totals[c], b.out[c].offsets + m, 4, cudaMemcpyDeviceToHost, sm));
     int32_t herr = 0;
     PG_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, sm));
     PG_CUDA(cudaStreamSynchronize(sm));
-    size_t ptotal = 0;
-    for (int c = 0; c < nc; c++) if (is_varlen(s->field(c).type)) ptotal += align256((size_t)totals[c] + 64);
-    unsigned char *pl = nullptr;
-    if (ptotal) {
-        run->bufs.emplace_back(ptotal);
-        pl = run->bufs.back().get();
-        if (!pl) return dv_oom();
-    }
-    size_t pt = 0;
-    for (int c = 0; c < nc; c++) {
-        if (!is_varlen(s->field(c).type)) continue;
-        run->cols[c].data = pl ? pl + pt : base;
-        run->varlen_bytes[c] = totals[c];
-        if (m > 0)
+    st = b.alloc_payload(std::vector<int64_t>(totals.begin(), totals.end()));
+    if (st) return st;
+    for (int c = 0; c < nc; c++)
+        if (b.out[c].offsets && m > 0)
             k_dv_copy_bytes<<<(int)((m * 8 + 255) / 256), 256, 0, sm>>>((const uint8_t *)in->cols[c].data, in->cols[c].offsets,
-                                                                        d_src, run->cols[c].offsets, pl + pt, m);
-        pt += align256((size_t)totals[c] + 64);
-    }
+                                                                        d_src, b.out[c].offsets, (uint8_t *)b.out[c].data, m);
     PG_CUDA(cudaStreamSynchronize(sm));
     PG_CUDA(cudaGetLastError());
     if (herr != KERR_NONE) return fail(PG_ERR_INTERNAL, "deletion vector: a var-len column exceeds 2 GiB of payload");
-    *out_run = g_runs.put(std::move(scratch.runs.back()));
+    b.finish(out_run, 0, nullptr);
     return PG_OK;
 }
 

@@ -154,6 +154,64 @@ struct Scratch {
     std::vector<std::unique_ptr<Run>> runs;
 };
 
+// PG_ERR_CUDA "<who>: out of device memory for <what> (N MiB wanted, F of T MiB free)"
+pg_status oom(const char *who, const char *what, size_t bytes);
+
+// where a decoder writes column c of run r: RunBuilder::out[r * n_cols + c]
+struct OutColumn {
+    void *data = nullptr;            // fixed-width values, or the var-len payload (set by alloc_payload)
+    int32_t *offsets = nullptr;
+    uint32_t *validity = nullptr;
+};
+
+// The runs a section decode or a deletion vector builds (api.cu), in the layout of DESIGN.md §3: per run one buffer
+// with the validity bitmaps first and contiguous (one memset clears them), then the values or int32 offsets of each
+// read column; after the caller's read-back of the exact sizes, one payload buffer per run for its var-len columns.
+// The runs stay in scratch.runs until finish() registers them.  `who` prefixes the error messages.
+struct RunBuilder {
+    RunBuilder(const Schema &s, int n_runs, Scratch &scratch, const char *who)
+        : schema(s), nc(s.n_cols()), scratch(scratch), who(who), read(s.n_cols(), 1), run_rows(n_runs, 0) {}
+    // read[c] from a read-column mask (NULL = every column); the key, sequence number and kind columns are always read
+    pg_status read_columns(const uint8_t *read_cols);
+    // the rows of a file land behind those of the files in front of it in its run: returns its first row
+    int64_t place_file(int run, int64_t rows) {
+        const int64_t row0 = run_rows[run];
+        run_rows[run] += rows;
+        return row0;
+    }
+    pg_status check_rows() const;    // no run holds more than 2^31 rows
+    // one buffer per run (validity cleared); bitmap[c]: a read column carries validity, zero[r * nc + c]: clear the
+    // values / offsets of that column of that run as well
+    pg_status alloc(const std::vector<uint8_t> &bitmap, const std::vector<uint8_t> &zero);
+    // payload[r * nc + c]: exact payload bytes of each var-len read column
+    pg_status alloc_payload(const std::vector<int64_t> &payload);
+    // registers the runs; *info (if any) is zeroed but for n_rows, n_runs and decoded_bytes
+    void finish(uint64_t *out_runs, int64_t bytes_h2d, pg_section_info *info);
+
+    const Schema &schema;
+    const int nc;
+    Scratch &scratch;
+    const char *who;
+    std::vector<uint8_t> read;       // per column: part of the read type (a run has no buffers for the others)
+    std::vector<int64_t> run_rows;
+    std::vector<OutColumn> out;
+    int64_t decoded_bytes = 0;       // validity (n + 7) / 8, values n * width, offsets 4 (n + 1), payload bytes
+};
+
+// the two events ms_decode is measured between
+struct SectionTimer {
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    ~SectionTimer() {
+        if (e0) cudaEventDestroy(e0);
+        if (e1) cudaEventDestroy(e1);
+    }
+    float ms() const {
+        float ms = 0;
+        cudaEventElapsedTime(&ms, e0, e1);
+        return ms;
+    }
+};
+
 // ---- handle tables: one per handle kind.  A handle carries its kind's tag in the top byte (1 schema, 2 merge spec,
 // 3 run, 4 merge; 5 Parquet reader, 6 encoded Parquet file, 7 upload), so a handle of one kind is never found by
 // another kind's entry points.

@@ -50,13 +50,18 @@ static __global__ void __launch_bounds__(256) k_scan_apply(int32_t *data, int64_
 }
 
 
-// offsets[1..n] hold lengths, offsets[0] = 0: turn them into Arrow offsets.  `sums` = scratch of n / 4096 + 2 int64.
-static inline void launch_offsets_scan(int32_t *offsets, int64_t n, int64_t *sums, int32_t *err, cudaStream_t st) {
+// data[0..n) -> its inclusive scan, in place.  `sums` = scratch of n / 4096 + 2 int64.
+static inline void launch_inclusive_scan(int32_t *data, int64_t n, int64_t *sums, int32_t *err, cudaStream_t st) {
     if (n <= 0) return;
     const int64_t nb = (n + 4095) / 4096;
-    k_scan_block_sums<<<(unsigned)nb, 256, 0, st>>>(offsets + 1, n, sums);
+    k_scan_block_sums<<<(unsigned)nb, 256, 0, st>>>(data, n, sums);
     k_scan_block_prefix<<<1, 1024, 0, st>>>(sums, nb, err);
-    k_scan_apply<<<(unsigned)nb, 256, 0, st>>>(offsets + 1, n, sums);
+    k_scan_apply<<<(unsigned)nb, 256, 0, st>>>(data, n, sums);
+}
+
+// offsets[1..n] hold lengths, offsets[0] = 0: turn them into Arrow offsets
+static inline void launch_offsets_scan(int32_t *offsets, int64_t n, int64_t *sums, int32_t *err, cudaStream_t st) {
+    launch_inclusive_scan(offsets + 1, n, sums, err, st);
 }
 
 }  // namespace pg

@@ -31,7 +31,14 @@
  *                            paimon-format/.../parquet/ParquetReaderFactory.java:113-148
  *
  * Threading: the library is re-entrant across handles; one merge handle (one CUDA stream) per
- * Java reader thread, like the reference's thread-confined readers.
+ * Java reader thread, like the reference's thread-confined readers.  A handle may be freed while another thread is
+ * inside a call on it (the call finishes on the object it found); one merge handle still belongs to one thread at a
+ * time.
+ *
+ * Ownership: pg_*_free drops the handle.  Objects that use it (a spec's schema, a merge's spec and runs, a run's view,
+ * a Parquet reader's schema) keep it alive until they are freed themselves.  A merge keeps its runs until an execute
+ * has merged them, so that a caller may free the runs of one section before it decodes the next; a later execute
+ * without a rebind fails if one of them has been freed by then.
  */
 #ifndef PAIMON_GPU_H
 #define PAIMON_GPU_H
@@ -187,9 +194,9 @@ pg_status pg_merge_spec_free(uint64_t spec);
 
 /* Register one sorted run.  PG_MEM_HOST: the buffers are copied to the device now (they may be
  * freed after the call).  PG_MEM_DEVICE: the pointers are device pointers that the caller keeps
- * alive until pg_run_free; every buffer must be 16-byte aligned and readable up to the next multiple
- * of 16 bytes (true for any cudaMalloc'ed / framework-allocated buffer): the kernels stage column
- * segments with 16-byte bulk async copies. */
+ * alive until pg_run_free and until no merge or view uses the run any more; every buffer must be 16-byte aligned and
+ * readable up to the next multiple of 16 bytes (true for any cudaMalloc'ed / framework-allocated buffer): the kernels
+ * stage column segments with 16-byte bulk async copies. */
 pg_status pg_run_open(uint64_t schema, const pg_run_desc *run, int32_t mem, uint64_t *out_run);
 pg_status pg_run_free(uint64_t run);
 
@@ -257,8 +264,10 @@ pg_status pg_export_arrow(uint64_t source, const char *const *column_names, int6
                           struct ArrowArray *out, struct ArrowSchema *out_schema);
 
 /* A VIEW (no copy) of rows [row_lo, row_hi) of a run handle, or of the current batch of a merge handle: a new run
- * handle whose columns point into the source's device buffers (the source must outlive it; pg_run_free drops the
- * view only).  The view starts at the 128-row boundary at or below row_lo (every buffer stays 16-byte aligned);
+ * handle whose columns point into the source's device buffers (pg_run_free drops the view only).  A view of a run
+ * keeps the run alive, so it stays valid after pg_run_free(source).  A view of a merge batch does not keep the merge:
+ * it is valid until that merge's next execute, rebind, release or free, which overwrite or free the batch.  The view
+ * starts at the 128-row boundary at or below row_lo (every buffer stays 16-byte aligned);
  * *start_row receives row_lo's position inside the view — pass it as start_rows[i] to pg_merge_rebind, or skip that
  * many rows after pg_run_fetch.  Used to re-merge / read back a key range of a bucket (parity samples at full size,
  * readers that hand out a large batch piece by piece). */

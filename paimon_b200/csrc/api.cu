@@ -22,7 +22,7 @@ pg_status fail(pg_status code, const std::string &msg) {
     return code;
 }
 
-
+static int g_device = -1;
 
 // grow-only device arena with a bump pointer
 struct Arena {
@@ -49,12 +49,13 @@ struct Arena {
         base = nullptr;
         cap = top = 0;
     }
+    ~Arena() { release(); }
 };
 
 struct Merge {
-    const Spec *spec = nullptr;
-    const Schema *schema = nullptr;
-    std::vector<const Run *> runs;
+    std::shared_ptr<const Spec> spec;
+    std::vector<std::shared_ptr<const Run>> runs;  // from the bind until an execute has merged them (see execute)
+    std::vector<std::weak_ptr<const Run>> bound;   // the same runs, for a re-execute
     std::vector<int64_t> row0;          // per run: first row that takes part (pg_merge_rebind), else 0
     int k = 0;
     int64_t n_in = 0;
@@ -96,6 +97,15 @@ struct Merge {
     int64_t n_out = 0;
     bool has_batch = false;
     pg_stats stats{};
+    // may run on a thread that never bound the device; the arenas, runs and spec are released after this body
+    ~Merge() {
+        if (g_device >= 0) cudaSetDevice(g_device);
+        if (stream) cudaStreamSynchronize(stream);
+        if (d_desc) cudaFree(d_desc);
+        if (h_totals) cudaFreeHost(h_totals);
+        for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+        if (stream) cudaStreamDestroy(stream);
+    }
 };
 
 // ------------------------------------------------------------------ handle tables
@@ -104,7 +114,6 @@ Table<Schema> g_schemas(1);
 static Table<Spec> g_specs(2);
 Table<Run> g_runs(3);
 static Table<Merge> g_merges(4);
-static int g_device = -1;
 
 pg_status ensure_device() {
     if (g_device < 0) return fail(PG_ERR_INVALID, "pg_init has not been called");
@@ -194,21 +203,22 @@ cudaStream_t copy_stream() {                          // one non-blocking copy s
     return st;
 }
 
-pg_status batch_columns(uint64_t handle, const Schema **schema, std::vector<DevColumn> *cols, int64_t *n_rows) {
-    if (Merge *m = g_merges.get(handle)) {
+pg_status batch_columns(uint64_t handle, BatchColumns *out) {
+    if (std::shared_ptr<Merge> m = g_merges.get(handle)) {
         if (!m->has_batch) return fail(PG_ERR_INVALID, "no batch: call pg_merge_execute first");
         if (m->stream) PG_CUDA(cudaStreamSynchronize(m->stream));
-        *schema = m->schema;
-        *n_rows = m->n_out;
-        cols->clear();
-        for (const pg_out_column &oc : m->out_cols) cols->push_back(DevColumn{oc.data, oc.offsets, oc.validity});
+        out->schema = m->spec->schema;
+        out->n_rows = m->n_out;
+        for (const pg_out_column &oc : m->out_cols) out->cols.push_back(DevColumn{oc.data, oc.offsets, oc.validity});
+        out->merge = std::move(m);
         return PG_OK;
     }
-    Run *r = g_runs.get(handle);
+    std::shared_ptr<Run> r = g_runs.get(handle);
     if (!r) return fail(PG_ERR_INVALID, "unknown run / merge handle");
-    *schema = r->schema;
-    *n_rows = r->n_rows;
-    *cols = r->cols;
+    out->schema = r->schema;
+    out->n_rows = r->n_rows;
+    out->cols = r->cols;
+    out->run = std::move(r);
     return PG_OK;
 }
 
@@ -224,7 +234,7 @@ pg_status oom(const char *who, const char *what, size_t bytes) {
 
 pg_status RunBuilder::read_columns(const uint8_t *read_cols) {
     if (!read_cols) return PG_OK;
-    for (int c = 0; c < schema.n_key + 2; c++)
+    for (int c = 0; c < schema->n_key + 2; c++)
         if (!read_cols[c]) return fail(PG_ERR_INVALID, std::string(who) + ": key, sequence number and kind columns are always read");
     for (int c = 0; c < nc; c++) read[c] = read_cols[c] != 0;
     return PG_OK;
@@ -244,7 +254,7 @@ pg_status RunBuilder::alloc(const std::vector<uint8_t> &bitmap, const std::vecto
         const int64_t n = run_rows[r];
         scratch.runs[r] = std::make_unique<Run>(schema, n);
         // values, or int32 offsets
-        auto main_bytes = [&](int c) { const int w = type_width(schema.field(c).type); return w ? (size_t)n * w : 4 * (size_t)(n + 1); };
+        auto main_bytes = [&](int c) { const int w = type_width(schema->field(c).type); return w ? (size_t)n * w : 4 * (size_t)(n + 1); };
         const size_t vb = align256((size_t)((n + 31) / 32) * 4 + 64);
         size_t vbytes = 0;
         for (int c = 0; c < nc; c++) if (read[c] && bitmap[c]) vbytes += vb;
@@ -263,7 +273,7 @@ pg_status RunBuilder::alloc(const std::vector<uint8_t> &bitmap, const std::vecto
             if (!read[c]) continue;
             OutColumn &o = out[(size_t)r * nc + c];
             if (bitmap[c]) { o.validity = (uint32_t *)(base + vt); vt += vb; decoded_bytes += (n + 7) / 8; }
-            if (type_width(schema.field(c).type)) o.data = base + o_main[c];
+            if (type_width(schema->field(c).type)) o.data = base + o_main[c];
             else o.offsets = (int32_t *)(base + o_main[c]);
             decoded_bytes += (int64_t)main_bytes(c);
             if (zero[(size_t)r * nc + c]) PG_CUDA(cudaMemsetAsync(base + o_main[c], 0, main_bytes(c), scratch.stream));
@@ -274,19 +284,19 @@ pg_status RunBuilder::alloc(const std::vector<uint8_t> &bitmap, const std::vecto
 
 pg_status RunBuilder::alloc_payload(const std::vector<int64_t> &payload) {
     bool any = false;
-    for (int c = 0; c < nc; c++) any |= read[c] && is_varlen(schema.field(c).type);
+    for (int c = 0; c < nc; c++) any |= read[c] && is_varlen(schema->field(c).type);
     if (!any) return PG_OK;
     for (int r = 0; r < (int)run_rows.size(); r++) {
         size_t sum = 256;
         for (int c = 0; c < nc; c++)
-            if (read[c] && is_varlen(schema.field(c).type)) sum += align256((size_t)payload[(size_t)r * nc + c] + 64);
+            if (read[c] && is_varlen(schema->field(c).type)) sum += align256((size_t)payload[(size_t)r * nc + c] + 64);
         Run &run = *scratch.runs[r];
         run.bufs.emplace_back(sum);
         unsigned char *pl = run.bufs.back().get();
         if (!pl) return oom(who, "the var-len payload of a run", sum);
         size_t pt = 0;
         for (int c = 0; c < nc; c++) {
-            if (!read[c] || !is_varlen(schema.field(c).type)) continue;
+            if (!read[c] || !is_varlen(schema->field(c).type)) continue;
             const int64_t bytes = payload[(size_t)r * nc + c];
             out[(size_t)r * nc + c].data = pl + pt;
             run.varlen_bytes[c] = bytes;
@@ -326,17 +336,6 @@ static void free_outputs(Merge *m, bool release_memory = false) {
     }
 }
 
-static void destroy_merge(Merge *m) {
-    if (!m) return;
-    if (m->stream) cudaStreamSynchronize(m->stream);
-    free_outputs(m, true);
-    m->work.release();
-    if (m->d_desc) cudaFree(m->d_desc);
-    if (m->h_totals) cudaFreeHost(m->h_totals);
-    for (auto &e : m->ev) if (e) cudaEventDestroy(e);
-    if (m->stream) { cudaStreamSynchronize(m->stream); cudaStreamDestroy(m->stream); }
-}
-
 // ------------------------------------------------------------------ plan-time validation
 
 static bool agg_supports_retract(int agg) {
@@ -345,8 +344,8 @@ static bool agg_supports_retract(int agg) {
 }
 
 static pg_status build_descriptors(Merge *m) {
-    const Schema *s = m->schema;
-    const Spec *sp = m->spec;
+    const Schema *s = m->spec->schema.get();
+    const Spec *sp = m->spec.get();
     // primary key: a 64-bit order-preserving prefix lives in shared memory; keys that do not fit it exactly
     // (strings, binaries, composites wider than 8 bytes) fall back to a full comparison on prefix ties
     if (s->n_key < 1 || s->n_key > PG_MAX_KEY_FIELDS)
@@ -494,7 +493,7 @@ static pg_status build_descriptors(Merge *m) {
     std::vector<unsigned char> host(total, 0);
     m->varlen_bound.assign(nv, 0);
     for (int r = 0; r < k; r++) {
-        const Run *run = m->runs[r];
+        const Run *run = m->runs[r].get();
         for (int f = 0; f < nk; f++) {
             ((const void **)(host.data() + o_key))[r * nk + f] = run->cols[f].data;
             ((const void **)(host.data() + o_koff))[r * nk + f] = run->cols[f].offsets;
@@ -604,7 +603,12 @@ static pg_status execute(Merge *m) {
     if (st) return st;
     cudaStream_t sm = m->stream;
     free_outputs(m);
-    const Schema *s = m->schema;
+    for (size_t r = m->runs.size(); r < m->bound.size(); r++)     // a re-execute takes the merged runs back
+        if (!m->runs.emplace_back(m->bound[r].lock())) {
+            m->runs.clear();
+            return fail(PG_ERR_INVALID, "a run of this merge has been freed since it was merged: rebind first");
+        }
+    const Schema *s = m->spec->schema.get();
     const int k = m->k, nc = s->n_cols(), nv = (int)m->varlen_cols.size();
     m->stats = pg_stats{};
     m->stats.rows_in = m->n_in;
@@ -862,6 +866,9 @@ static pg_status execute(Merge *m) {
     cudaEventElapsedTime(&m->stats.ms_alloc, m->ev[2], m->ev[4]);
     cudaEventElapsedTime(&m->stats.ms_emit, m->ev[4], m->ev[3]);
     cudaEventElapsedTime(&m->stats.ms_total, m->ev[0], m->ev[3]);
+    // The read-back above waited for the kernels, so the runs may go: a reader that frees them before it decodes the
+    // next section gets their buffers back at once, instead of holding two sections' runs per merge handle.
+    m->runs.clear();
     return PG_OK;
 }
 
@@ -926,7 +933,7 @@ pg_status pg_schema_create(const pg_schema_desc *desc, uint64_t *out_schema) {
 }
 
 pg_status pg_schema_info(uint64_t schema, int32_t *n_key, int32_t *n_val) {
-    Schema *s = g_schemas.get(schema);
+    std::shared_ptr<Schema> s = g_schemas.get(schema);
     if (!s) return fail(PG_ERR_INVALID, "unknown schema handle");
     if (n_key) *n_key = s->n_key;
     if (n_val) *n_val = s->n_val;
@@ -938,7 +945,7 @@ pg_status pg_schema_free(uint64_t schema) {
 }
 
 pg_status pg_merge_spec_create(uint64_t schema, const pg_merge_spec *spec, uint64_t *out_spec) {
-    Schema *s = g_schemas.get(schema);
+    std::shared_ptr<Schema> s = g_schemas.get(schema);
     if (!s || !spec || !out_spec) return fail(PG_ERR_INVALID, "bad schema handle or null argument");
     if (spec->engine < PG_ENGINE_DEDUPLICATE || spec->engine > PG_ENGINE_FIRST_ROW)
         return fail(PG_ERR_INVALID, "Unsupported merge engine");
@@ -950,7 +957,6 @@ pg_status pg_merge_spec_create(uint64_t schema, const pg_merge_spec *spec, uint6
     if (spec->n_sequence_groups > PG_MAX_SEQ_GROUPS)
         return fail(PG_ERR_UNSUPPORTED, "more than 16 sequence groups are not implemented on the device");
     auto sp = std::make_unique<Spec>();
-    sp->schema_h = schema;
     sp->schema = s;
     sp->engine = spec->engine;
     sp->ignore_delete = spec->ignore_delete != 0;
@@ -1036,12 +1042,12 @@ pg_status pg_trim(void) {
 }
 
 pg_status pg_run_open(uint64_t schema, const pg_run_desc *desc, int32_t mem, uint64_t *out_run) {
-    Schema *s = g_schemas.get(schema);
+    std::shared_ptr<Schema> s = g_schemas.get(schema);
     if (!s || !desc || !out_run) return fail(PG_ERR_INVALID, "bad schema handle or null argument");
     if (desc->n_rows < 0 || desc->n_rows > 0x7fffffffLL) return fail(PG_ERR_INVALID, "bad row count");
     pg_status st = ensure_device();
     if (st) return st;
-    auto run = std::make_unique<Run>(*s, desc->n_rows);
+    auto run = std::make_unique<Run>(s, desc->n_rows);
     const int nc = s->n_cols();
     const int64_t n = desc->n_rows;
     if (mem == PG_MEM_DEVICE) {
@@ -1123,7 +1129,7 @@ pg_status pg_run_free(uint64_t run) {
 }
 
 pg_status pg_run_layout(uint64_t run, int64_t *n_rows, int64_t *data_bytes, int32_t *has_validity, int32_t n_cols) {
-    Run *r = g_runs.get(run);
+    std::shared_ptr<Run> r = g_runs.get(run);
     if (!r || !n_rows) return fail(PG_ERR_INVALID, "unknown run handle");
     const int nc = r->schema->n_cols();
     if (n_cols != nc) return fail(PG_ERR_INVALID, "column count mismatch");
@@ -1138,7 +1144,7 @@ pg_status pg_run_layout(uint64_t run, int64_t *n_rows, int64_t *data_bytes, int3
 }
 
 pg_status pg_run_fetch(uint64_t run, const pg_out_column *host_cols, int32_t n_cols) {
-    Run *r = g_runs.get(run);
+    std::shared_ptr<Run> r = g_runs.get(run);
     if (!r || !host_cols) return fail(PG_ERR_INVALID, "unknown run handle");
     const int nc = r->schema->n_cols();
     if (n_cols != nc) return fail(PG_ERR_INVALID, "column count mismatch");
@@ -1169,18 +1175,17 @@ pg_status pg_run_fetch(uint64_t run, const pg_out_column *host_cols, int32_t n_c
 // a view of rows [row_lo & ~127, row_hi) of a run or of a merge handle's batch: no copy, the columns point into the
 // source's buffers (128 rows keep every buffer 16-byte aligned: 1-byte values, 4-byte offsets, 1-bit validity)
 static pg_status make_slice(uint64_t source, int64_t row_lo, int64_t row_hi, uint64_t *out_run, int64_t *start_row) {
-    const Schema *s = nullptr;
-    std::vector<DevColumn> cols;
-    int64_t n = 0;
-    pg_status st = batch_columns(source, &s, &cols, &n);
+    BatchColumns batch;
+    pg_status st = batch_columns(source, &batch);
     if (st) return st;
-    if (row_lo < 0 || row_hi < row_lo || row_hi > n) return fail(PG_ERR_INVALID, "slice outside the source");
+    if (row_lo < 0 || row_hi < row_lo || row_hi > batch.n_rows) return fail(PG_ERR_INVALID, "slice outside the source");
     const int64_t lo = row_lo & ~(int64_t)127;
-    auto run = std::make_unique<Run>(*s, row_hi - lo);
-    const int nc = s->n_cols();
+    auto run = std::make_unique<Run>(batch.schema, row_hi - lo);
+    run->source = batch.run;
+    const int nc = batch.schema->n_cols();
     for (int c = 0; c < nc; c++) {
-        const pg_field f = s->field(c);
-        DevColumn dc = cols[c];
+        const pg_field f = batch.schema->field(c);
+        DevColumn dc = batch.cols[c];
         if (is_varlen(f.type)) {
             if (dc.offsets && run->n_rows > 0) {
                 int32_t b[2] = {0, 0};
@@ -1221,16 +1226,18 @@ pg_status pg_thread_stream(void **out_cuda_stream) {
 // (re)binds a merge handle to k runs; runs without rows to merge are dropped (exhausted readers are legal,
 // SortMergeReaderTestBase.java:53-56)
 static pg_status bind_runs(Merge *m, const uint64_t *runs, int32_t k, const int64_t *row0) {
-    const Spec *sp = m->spec;
+    const Spec *sp = m->spec.get();
     m->runs.clear();
+    m->bound.clear();
     m->row0.clear();
+    m->k = 0;                                    // a failed bind merges nothing: the descriptors may be stale
     m->n_in = 0;
     m->stats = pg_stats{};
     for (int i = 0; i < k; i++) {
-        Run *r = g_runs.get(runs[i]);
+        std::shared_ptr<Run> r = g_runs.get(runs[i]);
         if (!r) return fail(PG_ERR_INVALID, "unknown run handle");
         if (r->schema != sp->schema) {           // different handles are fine as long as the schemas are equal
-            const Schema *a = r->schema, *b = sp->schema;
+            const Schema *a = r->schema.get(), *b = sp->schema.get();
             bool same = a->n_key == b->n_key && a->n_val == b->n_val;
             for (int c = 0; same && c < a->n_cols(); c++)
                 same = a->field(c).type == b->field(c).type && a->field(c).nullable == b->field(c).nullable;
@@ -1241,16 +1248,18 @@ static pg_status bind_runs(Merge *m, const uint64_t *runs, int32_t k, const int6
         m->stats.bytes_h2d += r->bytes_h2d;
         if (r->n_rows - skip == 0) continue;
         m->runs.push_back(r);
+        m->bound.push_back(r);
         m->row0.push_back(skip);
         m->n_in += r->n_rows - skip;
     }
     m->k = (int)m->runs.size();
-    if (m->k > 0) return build_descriptors(m);
-    return PG_OK;
+    pg_status st = m->k > 0 ? build_descriptors(m) : PG_OK;
+    if (st) m->k = 0;
+    return st;
 }
 
 pg_status pg_merge_open(uint64_t spec, const uint64_t *runs, int32_t k, uint64_t *out_merge) {
-    Spec *sp = g_specs.get(spec);
+    std::shared_ptr<Spec> sp = g_specs.get(spec);
     if (!sp || !out_merge || (k > 0 && !runs)) return fail(PG_ERR_INVALID, "bad spec handle or null argument");
     if (k < 0) return fail(PG_ERR_INVALID, "negative run count");
     if (k > PG_MAX_RUNS)
@@ -1258,47 +1267,46 @@ pg_status pg_merge_open(uint64_t spec, const uint64_t *runs, int32_t k, uint64_t
     pg_status st = ensure_device();
     if (st) return st;
     std::unique_ptr<Merge> m(new Merge());
-    m->spec = sp;
-    m->schema = sp->schema;
+    m->spec = std::move(sp);
     PG_CUDA(cudaStreamCreateWithFlags(&m->stream, cudaStreamNonBlocking));
     for (auto &e : m->ev) PG_CUDA(cudaEventCreate(&e));
     st = bind_runs(m.get(), runs, k, nullptr);
-    if (st) { destroy_merge(m.get()); return st; }
+    if (st) return st;
     *out_merge = g_merges.put(std::move(m));
     return PG_OK;
 }
 
 pg_status pg_merge_rebind(uint64_t merge, const uint64_t *runs, int32_t k, const int64_t *start_rows) {
-    Merge *m = g_merges.get(merge);
+    std::shared_ptr<Merge> m = g_merges.get(merge);
     if (!m || (k > 0 && !runs)) return fail(PG_ERR_INVALID, "unknown merge handle or null argument");
     if (k < 0 || k > PG_MAX_RUNS) return fail(PG_ERR_INVALID, "bad run count");
     pg_status st = ensure_device();
     if (st) return st;
     PG_CUDA(cudaStreamSynchronize(m->stream));
-    free_outputs(m);
-    return bind_runs(m, runs, k, start_rows);
+    free_outputs(m.get());
+    return bind_runs(m.get(), runs, k, start_rows);
 }
 
 pg_status pg_merge_execute(uint64_t merge) {
-    Merge *m = g_merges.get(merge);
+    std::shared_ptr<Merge> m = g_merges.get(merge);
     if (!m) return fail(PG_ERR_INVALID, "unknown merge handle");
     if (m->k == 0 || m->n_in == 0) {
         // no input rows: one empty batch
-        free_outputs(m);
+        free_outputs(m.get());
         m->n_out = 0;
-        m->out_cols.assign(m->schema->n_cols(), pg_out_column{});
+        m->out_cols.assign(m->spec->schema->n_cols(), pg_out_column{});
         m->has_batch = true;
         m->stats = pg_stats{};
         return PG_OK;
     }
     int64_t h2d = m->stats.bytes_h2d;
-    pg_status st = execute(m);
+    pg_status st = execute(m.get());
     m->stats.bytes_h2d = h2d;
     return st;
 }
 
 pg_status pg_merge_device_batch(uint64_t merge, pg_batch *out) {
-    Merge *m = g_merges.get(merge);
+    std::shared_ptr<Merge> m = g_merges.get(merge);
     if (!m || !out) return fail(PG_ERR_INVALID, "unknown merge handle");
     if (!m->has_batch) return fail(PG_ERR_INVALID, "no batch: call pg_merge_execute first");
     out->n_rows = m->n_out;
@@ -1308,7 +1316,7 @@ pg_status pg_merge_device_batch(uint64_t merge, pg_batch *out) {
 }
 
 pg_status pg_merge_fetch(uint64_t merge, const pg_out_column *host_cols, int32_t n_cols) {
-    Merge *m = g_merges.get(merge);
+    std::shared_ptr<Merge> m = g_merges.get(merge);
     if (!m || !host_cols) return fail(PG_ERR_INVALID, "unknown merge handle");
     if (!m->has_batch) return fail(PG_ERR_INVALID, "no batch: call pg_merge_execute first");
     if (n_cols != (int32_t)m->out_cols.size()) return fail(PG_ERR_INVALID, "column count mismatch");
@@ -1345,32 +1353,28 @@ pg_status pg_merge_fetch(uint64_t merge, const pg_out_column *host_cols, int32_t
 }
 
 pg_status pg_merge_release(uint64_t merge) {
-    Merge *m = g_merges.get(merge);
+    std::shared_ptr<Merge> m = g_merges.get(merge);
     if (!m) return fail(PG_ERR_INVALID, "unknown merge handle");
-    if (ensure_device() == PG_OK) free_outputs(m, true);
+    if (ensure_device() == PG_OK) free_outputs(m.get(), true);
     return PG_OK;
 }
 
 pg_status pg_merge_stats(uint64_t merge, pg_stats *out) {
-    Merge *m = g_merges.get(merge);
+    std::shared_ptr<Merge> m = g_merges.get(merge);
     if (!m || !out) return fail(PG_ERR_INVALID, "unknown merge handle");
     *out = m->stats;
     return PG_OK;
 }
 
 pg_status pg_merge_stream(uint64_t merge, void **out_cuda_stream) {
-    Merge *m = g_merges.get(merge);
+    std::shared_ptr<Merge> m = g_merges.get(merge);
     if (!m || !out_cuda_stream) return fail(PG_ERR_INVALID, "unknown merge handle");
     *out_cuda_stream = (void *)m->stream;
     return PG_OK;
 }
 
 pg_status pg_merge_free(uint64_t merge) {
-    auto m = g_merges.take(merge);
-    if (!m) return fail(PG_ERR_INVALID, "unknown merge handle");
-    if (g_device >= 0) cudaSetDevice(g_device);
-    destroy_merge(m.get());
-    return PG_OK;
+    return g_merges.take(merge) ? PG_OK : fail(PG_ERR_INVALID, "unknown merge handle");
 }
 
 // IntervalPartition.partition(), paimon-core/.../mergetree/compact/IntervalPartition.java:67-125.

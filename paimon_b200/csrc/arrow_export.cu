@@ -68,17 +68,17 @@ const char *arrow_format(int t) {
 
 static pg_status export_arrow(uint64_t source, const char *const *names, int64_t row0, int64_t n_rows,
                               ArrowArray *out, ArrowSchema *out_schema) {
-    const Schema *s = nullptr;
-    std::vector<DevColumn> cols;
-    int64_t total = 0;
-    pg_status st = batch_columns(source, &s, &cols, &total);
+    BatchColumns batch;                                 // held until the copies below are done
+    pg_status st = batch_columns(source, &batch);
     if (st) return st;
-    if (n_rows < 0) n_rows = total - row0;
-    if (row0 < 0 || n_rows < 0 || row0 + n_rows > total) return fail(PG_ERR_INVALID, "arrow export: row range outside the batch");
+    const Schema *s = batch.schema.get();
+    std::vector<DevColumn> &cols = batch.cols;
+    if (n_rows < 0) n_rows = batch.n_rows - row0;
+    if (row0 < 0 || n_rows < 0 || row0 + n_rows > batch.n_rows) return fail(PG_ERR_INVALID, "arrow export: row range outside the batch");
     // columns a read-type projection left out of the batch are not exported
     std::vector<int> present;
     for (int c = 0; c < s->n_cols(); c++)
-        if (cols[c].data || cols[c].offsets || total == 0) present.push_back(c);
+        if (cols[c].data || cols[c].offsets || batch.n_rows == 0) present.push_back(c);
     {
         std::vector<DevColumn> pc;
         for (int c : present) pc.push_back(cols[c]);

@@ -139,12 +139,13 @@ static bool orc_type_ok(int pg_t, const orc::Type &ty) {
     }
 }
 
-static pg_status orc_decode_section(const Schema *s, const pg_file_desc *files, int nf, int n_runs, const char *const *names,
-                                    const uint8_t *read_cols, uint64_t *out_runs, pg_section_info *info) {
+static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, const pg_file_desc *files, int nf, int n_runs,
+                                    const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
+                                    pg_section_info *info) {
     const int nc = s->n_cols();
     cudaStream_t sm = copy_stream();
     Scratch scratch(sm);                               // file images, tables, scratch and the runs until registered
-    RunBuilder b(*s, n_runs, scratch, "orc");
+    RunBuilder b(s, n_runs, scratch, "orc");
     SectionTimer tm;
     PG_CUDA(cudaEventCreate(&tm.e0));
     PG_CUDA(cudaEventCreate(&tm.e1));
@@ -381,12 +382,11 @@ using namespace pg;
 extern "C" pg_status pg_orc_read_section(uint64_t schema, const pg_file_desc *files, int32_t n_files, int32_t n_runs,
                                          const char *const *column_names, const uint8_t *read_columns, uint64_t *out_runs,
                                          pg_section_info *info) {
-    Schema *s = g_schemas.get(schema);
+    std::shared_ptr<Schema> s = g_schemas.get(schema);
     if (!s || !out_runs || n_files < 0 || n_runs < 0 || (n_files > 0 && !files))
         return fail(PG_ERR_INVALID, "bad schema handle or null argument");
     if (n_runs == 0) return n_files == 0 ? PG_OK : fail(PG_ERR_INVALID, "files without runs");
     pg_status st = ensure_device();
     if (st) return st;
-    const Schema own = *s;
-    return orc_decode_section(&own, files, n_files, n_runs, column_names, read_columns, out_runs, info);
+    return orc_decode_section(s, files, n_files, n_runs, column_names, read_columns, out_runs, info);
 }

@@ -1502,14 +1502,14 @@ static pg_status expand_pages(cudaStream_t sm, bool byte_arrays, PqPage *d_pages
     return PG_OK;
 }
 
-static pg_status decode_section(const Schema *s, const std::vector<SectionFile> &files, int n_runs,
-                                const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
+static pg_status decode_section(const std::shared_ptr<const Schema> &s, const std::vector<SectionFile> &files,
+                                int n_runs, const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
                                 pg_section_info *info) {
     const int nc = s->n_cols();
     const int nf = (int)files.size();
     cudaStream_t sm = copy_stream();
     Scratch scratch(sm);                               // file images, tables, scratch and the runs until registered
-    RunBuilder b(*s, n_runs, scratch, "parquet");
+    RunBuilder b(s, n_runs, scratch, "parquet");
     int launches = 0;
     SectionTimer tm;
     PG_CUDA(cudaEventCreate(&tm.e0));
@@ -1540,7 +1540,7 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     std::vector<uint8_t> any_optional(nc, 0);
     std::vector<std::vector<int>> file_col(nf);
     for (int f = 0; f < nf; f++) {
-        pg_status st = map_file_schema(s, *meta[f], names, read_cols, &file_col[f]);
+        pg_status st = map_file_schema(s.get(), *meta[f], names, read_cols, &file_col[f]);
         if (st) return st;
         for (int c = 0; c < nc; c++) {
             const int fc = file_col[f][c];
@@ -1551,7 +1551,7 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
     for (int f = 0; f < nf; f++) file_row0[f] = b.place_file(files[f].run, meta[f]->num_rows);
     { pg_status st = b.check_rows(); if (st) return st; }
     ChunkTables ct;
-    { pg_status st = build_chunk_tables(s, files, d_file, meta, file_col, file_row0, b, ct); if (st) return st; }
+    { pg_status st = build_chunk_tables(s.get(), files, d_file, meta, file_col, file_row0, b, ct); if (st) return st; }
     const int n_chunks = (int)ct.chunks.size(), n_pairs = (int)ct.pairs.size();
 
     // ---- output columns (the rows of files that lack a column stay NULL and get defined contents)
@@ -1714,8 +1714,7 @@ static pg_status decode_section(const Schema *s, const std::vector<SectionFile> 
 // ---- the single-file reader (FormatReaderFactory.createReader + readBatch): a section of one file
 
 struct PqReader {
-    const Schema *schema = nullptr;
-    Schema own_schema;
+    std::shared_ptr<const Schema> schema;
     pq::FileMetaData meta;
     std::vector<uint8_t> file;             // host copy: pg_parquet_open's caller may free its buffer
     int64_t n_rows = 0;
@@ -1728,12 +1727,11 @@ static Table<PqReader> g_pq(5);
 
 // open = footer + schema check + a host walk of the page headers, so that files the device would refuse are refused
 // here, before any device work (and on a box without a GPU)
-static pg_status pq_open(uint64_t schema_h, const uint8_t *bytes, int64_t size, uint64_t *out) {
-    Schema *s = g_schemas.get(schema_h);
+static pg_status pq_open(uint64_t schema, const uint8_t *bytes, int64_t size, uint64_t *out) {
+    std::shared_ptr<Schema> s = g_schemas.get(schema);
     if (!s || !bytes || !out) return fail(PG_ERR_INVALID, "bad schema handle or null argument");
     auto rd = std::make_unique<PqReader>();
-    rd->own_schema = *s;
-    rd->schema = &rd->own_schema;
+    rd->schema = s;
     try {
         rd->meta = pq::parse_footer(bytes, size);
     } catch (const std::exception &e) {
@@ -1741,7 +1739,7 @@ static pg_status pq_open(uint64_t schema_h, const uint8_t *bytes, int64_t size, 
     }
     const pq::FileMetaData &m = rd->meta;
     std::vector<int> file_col;
-    pg_status st = map_file_schema(s, m, nullptr, nullptr, &file_col);
+    pg_status st = map_file_schema(s.get(), m, nullptr, nullptr, &file_col);
     if (st) return st;
     const int nc = s->n_cols();
     rd->n_rows = m.num_rows;
@@ -1846,11 +1844,11 @@ __global__ void k_dv_copy_bytes(const uint8_t *data, const int32_t *offs, const 
 }
 
 static pg_status apply_deletion_vector(uint64_t run_h, const uint8_t *deleted, int64_t n_bits, uint64_t *out_run) {
-    Run *in = g_runs.get(run_h);
+    std::shared_ptr<Run> in = g_runs.get(run_h);
     if (!in || !out_run || (n_bits > 0 && !deleted)) return fail(PG_ERR_INVALID, "unknown run handle or null argument");
     pg_status st = ensure_device();
     if (st) return st;
-    const Schema *s = in->schema;
+    const Schema *s = in->schema.get();
     const int nc = s->n_cols();
     const int64_t n = in->n_rows;
     if (n_bits < 0) return fail(PG_ERR_INVALID, "negative deletion vector size");
@@ -1878,7 +1876,7 @@ static pg_status apply_deletion_vector(uint64_t run_h, const uint8_t *deleted, i
     if (!d_src) return oom("deletion vector", "the row sources", sizeof(int32_t) * (size_t)m);
     if (n > 0) k_dv_sources<<<(int)((n + 255) / 256), 256, 0, sm>>>(d_incl, n, d_src);
     // ---- the kept rows of the columns the input has, with the bitmaps the input has
-    RunBuilder b(*s, 1, scratch, "deletion vector");
+    RunBuilder b(in->schema, 1, scratch, "deletion vector");
     b.place_file(0, m);
     std::vector<uint8_t> bitmap(nc), no_zero(nc, 0);
     for (int c = 0; c < nc; c++) {
@@ -1933,30 +1931,30 @@ pg_status pg_parquet_open(uint64_t schema, const uint8_t *file_bytes, int64_t si
 }
 
 pg_status pg_parquet_describe(uint64_t reader, pg_parquet_info *out) {
-    const bool known = out && g_pq.with(reader, [&](PqReader &rd) {
-        out->n_rows = rd.n_rows;
-        out->n_row_groups = (int32_t)rd.meta.row_groups.size();
-        out->n_columns = rd.schema->n_cols();
-        out->n_data_pages = rd.n_data_pages;
-        out->n_dictionary_pages = rd.n_dict_pages;
-        out->ms_decode = rd.ms_decode;
-        out->launches = rd.launches;
-    });
-    return known ? PG_OK : fail(PG_ERR_INVALID, "unknown parquet reader handle");
+    std::shared_ptr<PqReader> rd = g_pq.get(reader);
+    if (!rd || !out) return fail(PG_ERR_INVALID, "unknown parquet reader handle");
+    out->n_rows = rd->n_rows;
+    out->n_row_groups = (int32_t)rd->meta.row_groups.size();
+    out->n_columns = rd->schema->n_cols();
+    out->n_data_pages = rd->n_data_pages;
+    out->n_dictionary_pages = rd->n_dict_pages;
+    out->ms_decode = rd->ms_decode;
+    out->launches = rd->launches;
+    return PG_OK;
 }
 
 pg_status pg_parquet_read_run(uint64_t reader, uint64_t *out_run) {
-    PqReader *rd = g_pq.get(reader);
+    std::shared_ptr<PqReader> rd = g_pq.get(reader);
     if (!rd || !out_run) return fail(PG_ERR_INVALID, "unknown parquet reader handle");
     pg_status st = ensure_device();           // fails loudly without pg_init / a CUDA device: no CPU fallback
     if (st) return st;
-    return pq_read_run(rd, out_run);
+    return pq_read_run(rd.get(), out_run);
 }
 
 pg_status pg_parquet_read_section(uint64_t schema, const pg_file_desc *files, int32_t n_files, int32_t n_runs,
                                   const char *const *column_names, const uint8_t *read_columns, uint64_t *out_runs,
                                   pg_section_info *info) {
-    Schema *s = g_schemas.get(schema);
+    std::shared_ptr<Schema> s = g_schemas.get(schema);
     if (!s || !out_runs || n_files < 0 || n_runs < 0 || (n_files > 0 && !files))
         return fail(PG_ERR_INVALID, "bad schema handle or null argument");
     if (n_runs == 0) return n_files == 0 ? PG_OK : fail(PG_ERR_INVALID, "files without runs");
@@ -1967,8 +1965,7 @@ pg_status pg_parquet_read_section(uint64_t schema, const pg_file_desc *files, in
         if (files[i].mem != PG_MEM_HOST && files[i].mem != PG_MEM_DEVICE) return fail(PG_ERR_INVALID, "bad memory kind");
         fs[i] = SectionFile{files[i].bytes, files[i].size, files[i].mem, files[i].run, nullptr};
     }
-    const Schema own = *s;                       // the schema handle may be freed while the runs live on
-    return decode_section(&own, fs, n_runs, column_names, read_columns, out_runs, info);
+    return decode_section(s, fs, n_runs, column_names, read_columns, out_runs, info);
 }
 
 pg_status pg_run_apply_deletion_vector(uint64_t run, const uint8_t *deleted_bitmap, int64_t n_bits, uint64_t *out_run) {

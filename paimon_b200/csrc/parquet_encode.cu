@@ -286,17 +286,17 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
                         const pg_parquet_write_options *opt, uint64_t *out_file) {
     pg_status st = ensure_device();
     if (st) return st;
-    const Schema *s = nullptr;
-    std::vector<DevColumn> dcols;
-    int64_t total_rows = 0;
-    st = batch_columns(source, &s, &dcols, &total_rows);
+    BatchColumns batch;                                      // held until the encode below is done
+    st = batch_columns(source, &batch);
     if (st) return st;
-    for (int c = 0; c < s->n_cols() && total_rows > 0; c++)
+    const Schema *s = batch.schema.get();
+    const std::vector<DevColumn> &dcols = batch.cols;
+    for (int c = 0; c < s->n_cols() && batch.n_rows > 0; c++)
         if (!dcols[c].data && !dcols[c].offsets)
             return fail(PG_ERR_INVALID, "parquet encode: the batch was produced under a read-type projection and has no "
                                         "column " + std::to_string(c) + "; a data file needs every column");
-    if (n_rows < 0) n_rows = total_rows - row0;
-    if (row0 < 0 || (row0 & 7) || row0 + n_rows > total_rows)
+    if (n_rows < 0) n_rows = batch.n_rows - row0;
+    if (row0 < 0 || (row0 & 7) || row0 + n_rows > batch.n_rows)
         return fail(PG_ERR_INVALID, "parquet encode: row range outside the batch or not starting at a multiple of 8");
     const int nc = s->n_cols();
     int64_t page_rows = opt && opt->page_rows > 0 ? opt->page_rows : 32768;
@@ -544,29 +544,27 @@ pg_status pg_parquet_encode(uint64_t source, const char *const *column_names, in
 }
 
 pg_status pg_parquet_file_meta(uint64_t file, pg_file_meta *out) {
-    const bool known = out && g_enc.with(file, [&](EncodedFile &ef) { *out = ef.meta; });
-    return known ? PG_OK : fail(PG_ERR_INVALID, "unknown encoded file handle");
+    std::shared_ptr<EncodedFile> ef = g_enc.get(file);
+    if (!ef || !out) return fail(PG_ERR_INVALID, "unknown encoded file handle");
+    *out = ef->meta;
+    return PG_OK;
 }
 
 pg_status pg_parquet_file_column_stats(uint64_t file, int32_t column, int64_t *null_count, int32_t *has_min_max,
                                        void *min8, void *max8) {
-    pg_status st = PG_OK;
-    const bool known = g_enc.with(file, [&](EncodedFile &ef) {
-        if (column < 0 || column >= (int32_t)ef.stats.size()) {
-            st = fail(PG_ERR_INVALID, "column out of range");
-            return;
-        }
-        const ColStats &cs = ef.stats[column];
-        if (null_count) *null_count = cs.null_count;
-        if (has_min_max) *has_min_max = cs.has_minmax;
-        if (min8) memcpy(min8, &cs.min, 8);
-        if (max8) memcpy(max8, &cs.max, 8);
-    });
-    return known ? st : fail(PG_ERR_INVALID, "unknown encoded file handle");
+    std::shared_ptr<EncodedFile> ef = g_enc.get(file);
+    if (!ef) return fail(PG_ERR_INVALID, "unknown encoded file handle");
+    if (column < 0 || column >= (int32_t)ef->stats.size()) return fail(PG_ERR_INVALID, "column out of range");
+    const ColStats &cs = ef->stats[column];
+    if (null_count) *null_count = cs.null_count;
+    if (has_min_max) *has_min_max = cs.has_minmax;
+    if (min8) memcpy(min8, &cs.min, 8);
+    if (max8) memcpy(max8, &cs.max, 8);
+    return PG_OK;
 }
 
 pg_status pg_parquet_file_fetch(uint64_t file, void *host_buffer, int64_t capacity) {
-    EncodedFile *ef = g_enc.get(file);
+    std::shared_ptr<EncodedFile> ef = g_enc.get(file);
     if (!ef || !host_buffer) return fail(PG_ERR_INVALID, "unknown encoded file handle");
     if (capacity < ef->file_bytes) return fail(PG_ERR_INVALID, "buffer smaller than the file");
     pg_status st = ensure_device();
@@ -578,7 +576,7 @@ pg_status pg_parquet_file_fetch(uint64_t file, void *host_buffer, int64_t capaci
 }
 
 pg_status pg_parquet_file_device_image(uint64_t file, const uint8_t **device_bytes, int64_t *size) {
-    EncodedFile *ef = g_enc.get(file);
+    std::shared_ptr<EncodedFile> ef = g_enc.get(file);
     if (!ef || !device_bytes || !size) return fail(PG_ERR_INVALID, "unknown encoded file handle");
     pg_status st = ensure_device();
     if (st) return st;

@@ -65,8 +65,7 @@ struct Schema {
 };
 
 struct Spec {
-    uint64_t schema_h = 0;
-    const Schema *schema = nullptr;
+    std::shared_ptr<const Schema> schema;
     int engine = 0, ignore_delete = 0, remove_record_on_delete = 0, drop_delete = 0;
     std::vector<int32_t> seq_fields;
     int seq_ascending = 1;
@@ -119,18 +118,18 @@ class DeviceBuffer {
 inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
 struct Run {
-    Run(const Schema &s, int64_t rows)
-        : schema(&own_schema), own_schema(s), n_rows(rows), cols(s.n_cols()), varlen_bytes(s.n_cols(), 0),
-          varlen_base(s.n_cols(), 0) {}
+    Run(std::shared_ptr<const Schema> s, int64_t rows)
+        : schema(std::move(s)), n_rows(rows), cols(schema->n_cols()), varlen_bytes(schema->n_cols(), 0),
+          varlen_base(schema->n_cols(), 0) {}
     Run(const Run &) = delete;
     Run &operator=(const Run &) = delete;
-    const Schema *schema;
-    Schema own_schema;                   // copy: a run may outlive the schema handle it was opened with
+    std::shared_ptr<const Schema> schema;
     int64_t n_rows;
     std::vector<DevColumn> cols;
     std::vector<int64_t> varlen_bytes;   // per column: payload bytes of a var-len column (offsets[n_rows] - offsets[0])
     std::vector<int64_t> varlen_base;    // per column: offsets[0] (data points at byte 0 of the offsets' space)
     std::vector<DeviceBuffer> bufs;      // device memory the run owns (none for device-memory runs and slices)
+    std::shared_ptr<const Run> source;   // a slice of a run: that run (a slice of a merge batch holds no merge: no cycle)
     int64_t bytes_h2d = 0;
 };
 
@@ -169,8 +168,8 @@ struct OutColumn {
 // read column; after the caller's read-back of the exact sizes, one payload buffer per run for its var-len columns.
 // The runs stay in scratch.runs until finish() registers them.  `who` prefixes the error messages.
 struct RunBuilder {
-    RunBuilder(const Schema &s, int n_runs, Scratch &scratch, const char *who)
-        : schema(s), nc(s.n_cols()), scratch(scratch), who(who), read(s.n_cols(), 1), run_rows(n_runs, 0) {}
+    RunBuilder(std::shared_ptr<const Schema> s, int n_runs, Scratch &scratch, const char *who)
+        : schema(std::move(s)), nc(schema->n_cols()), scratch(scratch), who(who), read(nc, 1), run_rows(n_runs, 0) {}
     // read[c] from a read-column mask (NULL = every column); the key, sequence number and kind columns are always read
     pg_status read_columns(const uint8_t *read_cols);
     // the rows of a file land behind those of the files in front of it in its run: returns its first row
@@ -188,7 +187,7 @@ struct RunBuilder {
     // registers the runs; *info (if any) is zeroed but for n_rows, n_runs and decoded_bytes
     void finish(uint64_t *out_runs, int64_t bytes_h2d, pg_section_info *info);
 
-    const Schema &schema;
+    const std::shared_ptr<const Schema> schema;
     const int nc;
     Scratch &scratch;
     const char *who;
@@ -215,42 +214,34 @@ struct SectionTimer {
 // ---- handle tables: one per handle kind.  A handle carries its kind's tag in the top byte (1 schema, 2 merge spec,
 // 3 run, 4 merge; 5 Parquet reader, 6 encoded Parquet file, 7 upload), so a handle of one kind is never found by
 // another kind's entry points.
+// The table holds one reference to each object; get() hands out a lease that an entry point holds until it returns, and
+// objects hold leases on what they use, so freeing a handle never frees an object in use.  No object holds a lease on
+// a Merge.  Scratch's ordering rule holds wherever a last lease is dropped: a lease may be dropped when its call
+// returns, because the call's device work is finished by then (every entry point synchronises before it returns).
 template <typename T>
 class Table {
  public:
     explicit Table(uint64_t tag) : tag_(tag << 56) {}
-    uint64_t put(std::unique_ptr<T> p) {
+    uint64_t put(std::shared_ptr<T> p) {
         std::lock_guard<std::mutex> g(mu_);
         const uint64_t h = tag_ | next_++;
         map_[h] = std::move(p);
         return h;
     }
-    T *get(uint64_t h) {
+    std::shared_ptr<T> get(uint64_t h) {     // NULL = unknown handle
         std::lock_guard<std::mutex> g(mu_);
         auto it = map_.find(h);
-        return it == map_.end() ? nullptr : it->second.get();
+        return it == map_.end() ? nullptr : it->second;
     }
-    // fn(T &) with the table locked, so that a concurrent take() cannot free the object meanwhile; false = unknown
-    template <typename F>
-    bool with(uint64_t h, F &&fn) {
+    std::shared_ptr<T> take(uint64_t h) {    // removes the handle: the table's reference, NULL = unknown handle
         std::lock_guard<std::mutex> g(mu_);
-        auto it = map_.find(h);
-        if (it == map_.end()) return false;
-        fn(*it->second);
-        return true;
-    }
-    std::unique_ptr<T> take(uint64_t h) {
-        std::lock_guard<std::mutex> g(mu_);
-        auto it = map_.find(h);
-        if (it == map_.end()) return nullptr;
-        std::unique_ptr<T> p = std::move(it->second);
-        map_.erase(it);
-        return p;
+        auto node = map_.extract(h);
+        return node.empty() ? nullptr : std::move(node.mapped());
     }
 
  private:
     std::mutex mu_;
-    std::unordered_map<uint64_t, std::unique_ptr<T>> map_;
+    std::unordered_map<uint64_t, std::shared_ptr<T>> map_;
     uint64_t next_ = 1;
     const uint64_t tag_;
 };
@@ -260,8 +251,17 @@ extern Table<Run> g_runs;
 // ---- the rest of api.cu that the format readers and writers use
 pg_status ensure_device();           // pg_init has been called; binds the calling thread to the device
 cudaStream_t copy_stream();          // the calling thread's non-blocking stream
-// the columns of a merge handle's current batch, or of a run
-pg_status batch_columns(uint64_t handle, const Schema **schema, std::vector<DevColumn> *cols, int64_t *n_rows);
+// the columns of a merge handle's current batch, or of a run, with leases on the schema and on the source that the
+// caller keeps for its whole call
+struct Merge;
+struct BatchColumns {
+    std::shared_ptr<const Schema> schema;
+    std::vector<DevColumn> cols;
+    int64_t n_rows = 0;
+    std::shared_ptr<const Run> run;      // the source: a run,
+    std::shared_ptr<Merge> merge;        // or a merge handle
+};
+pg_status batch_columns(uint64_t handle, BatchColumns *out);
 
 // ---- device-side descriptors (copied to device memory once per merge handle) ----
 

@@ -62,7 +62,7 @@ extern "C" pg_status pg_files_upload_begin(const pg_file_desc *files, int32_t n_
 }
 
 extern "C" pg_status pg_files_upload_wait(uint64_t upload, pg_file_desc *out_files, int32_t n_files) {
-    Upload *up = g_up.get(upload);
+    std::shared_ptr<Upload> up = g_up.get(upload);
     if (!up) return fail(PG_ERR_INVALID, "unknown upload handle");
     if (n_files != (int32_t)up->files.size() || (n_files > 0 && !out_files)) return fail(PG_ERR_INVALID, "upload: one descriptor per file");
     PG_CUDA(cudaEventSynchronize(up->done));
@@ -71,7 +71,7 @@ extern "C" pg_status pg_files_upload_wait(uint64_t upload, pg_file_desc *out_fil
 }
 
 extern "C" pg_status pg_files_upload_free(uint64_t upload) {
-    std::unique_ptr<Upload> up = g_up.take(upload);
+    std::shared_ptr<Upload> up = g_up.take(upload);
     if (!up) return fail(PG_ERR_INVALID, "unknown upload handle");
     // the copy itself, and the decode launches of the calling thread that read the bytes, must be done before the
     // buffers go back to the cache

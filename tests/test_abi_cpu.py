@@ -99,9 +99,14 @@ def test_handle_validation_without_device():
             assert b"unknown" in lib.pg_last_error()
             assert alive is None or alive(), (tag, other)
     assert (n_key.value, n_val.value) == (1, 0)
-    for tag, h, _ in reversed(live):
+    for tag, h, _ in live:                                 # the schema first: the spec and the reader keep it alive
         assert frees[tag](h) == 0, tag
         assert frees[tag](h) == 1, tag                     # freed once
+        assert b"unknown" in lib.pg_last_error(), tag
+        if tag == 1:
+            info = N.PgParquetInfo()
+            assert lib.pg_parquet_describe(reader.value, C.byref(info)) == 0, lib.pg_last_error()
+            assert (info.n_columns, info.n_rows) == (3, 3)
 
 
 def test_interval_partition_host_logic_matches_oracle():

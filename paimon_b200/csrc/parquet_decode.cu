@@ -833,10 +833,12 @@ k_pq_walk_dicts(const PqPage *dicts, int n_dicts, const PqChunk *chunks, int32_t
 // lanes of a warp walk streams of similar length.
 // Reading the length words straight from global memory makes every lane miss a 32-byte sector on nearly every value
 // (32 scattered sector fetches per warp step, one round trip each), so the warp works in ROUNDS: it
-// loads the next kWvWin bytes of all 32 streams into shared memory with coalesced 16-byte loads (16 lanes per stream,
-// 8 KiB in flight per warp), then every lane walks the values whose length word lies inside its window at
-// shared-memory latency.  Rows of the window buffer are XOR-swizzled per 16-byte chunk (lanes walk their rows at
-// similar offsets: without it every access is a 32-way bank conflict).
+// loads the next kWvWin bytes of all 32 streams into shared memory with coalesced 16-byte loads (32 KiB in flight per
+// warp), then every lane walks the values whose length word lies inside its window at shared-memory latency.  A round
+// costs about one round trip whatever its size, so the window is as large as the shared memory allows: 1 KiB windows
+// took the C3 walk from 15.3 to 12.1 ms beside the expansion (H100, DESIGN.md §5), 512 B ones did not help.  Rows of the
+// window buffer are XOR-swizzled per 16-byte chunk (lanes walk their rows at similar offsets: without it every access
+// is a 32-way bank conflict).
 __device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
 }
@@ -845,7 +847,8 @@ __device__ __forceinline__ void cp_async4(void *smem_dst, const void *gsrc) {
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-constexpr int kWvWarps = 4, kWvWin = 256;
+constexpr int kWvWarps = 1, kWvWin = 1024;
+static_assert(kWvWin % 16 == 0 && kWvWarps * 32 * kWvWin <= 48 * 1024, "whole 16-byte chunks, static shared memory");
 __global__ void __launch_bounds__(kWvWarps * 32)
 k_pq_walk_values(PqPage *pages, int n_pages, const PqChunk *chunks, int32_t *vstart, int32_t *err) {
     __shared__ __align__(16) uint8_t s_win[kWvWarps][32][kWvWin];
@@ -872,11 +875,12 @@ k_pq_walk_values(PqPage *pages, int n_pages, const PqChunk *chunks, int32_t *vst
         // ---- load every live lane's window [wb, wb + kWvWin): wb = the 16-byte boundary at or below its position
         const uint8_t *wb = done ? nullptr : (const uint8_t *)((uintptr_t)(stream + q) & ~(uintptr_t)15);
         const uint8_t *wend = done ? nullptr : stream + slen;
-        // (16 async 16-byte copies per lane, all in flight together: one round trip per round; chunks past the stream's
-        // end are not loaded — the walk never reads a length word it has not bounds-checked against the stream)
+        // (kWvWin / 16 async 16-byte copies per lane, all in flight together: one round trip per round; chunks past the
+        // stream's end are not loaded — the walk never reads a length word it has not bounds-checked against the stream)
+        constexpr int kChunks = kWvWin / 16;                          // 16-byte chunks per window
 #pragma unroll 4
-        for (int i = 0; i < 16; i++) {
-            const int w = 2 * i + (lane >> 4), c = lane & 15;
+        for (int i = 0; i < kChunks; i++) {
+            const int f = 32 * i + lane, w = f / kChunks, c = f % kChunks;
             const uint8_t *wbw = (const uint8_t *)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)wb, w);
             const uint8_t *wew = (const uint8_t *)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)wend, w);
             if (wbw != nullptr && wbw + 16 * c < wew) cp_async16(&rows[w][((c ^ (w & 15)) << 4)], wbw + 16 * c);   // (<= 15 bytes past the page)
@@ -940,23 +944,30 @@ __device__ __forceinline__ uint64_t pq_load_unaligned(const uint8_t *p, int w) {
     return sh ? (uint64_t)((lo >> sh) | (q[1] << (32 - sh))) : (uint64_t)lo;
 }
 
+// Shared-memory staging of the PLAIN BYTE_ARRAY payload copy.  Only the instantiation that expands those pages has it:
+// without its 29 KB, the expansion of the other pages fits on an SM beside the value walk's windows.
+template <bool kPlainStrings> struct PqPlainStage {
+    int vs[2][kExpThreads + 4];
+    int bnd[kPayBatches + 1];
+    alignas(16) uint8_t in[2][kPayIn];
+    alignas(16) uint8_t out[kPayOut];
+};
+template <> struct PqPlainStage<false> {};
+
+// kPlainStrings: the PLAIN BYTE_ARRAY pages (after the value walk), else every other page
+template <bool kPlainStrings>
 __global__ void __launch_bounds__(kExpThreads, 6)
 k_pq_expand(const PqPage *pages, const PqPage *dicts, const PqChunk *chunks, const PqOut *outs, int n_cols,
-            const int32_t *ids, const int32_t *vstart, const int32_t *dict_off, const int32_t *dict_len, int32_t *err,
-            int kind) {
+            const int32_t *ids, const int32_t *vstart, const int32_t *dict_off, const int32_t *dict_len) {
     __shared__ uint32_t s_bits[kExpThreads];
     __shared__ int s_rank[kExpThreads];
     __shared__ int s_wlen[kExpThreads];
     __shared__ int s_ws[34];
-    __shared__ int s_vs[2][kExpThreads + 4];
-    __shared__ int s_bnd[kPayBatches + 1];
-    __shared__ __align__(16) uint8_t s_in[2][kPayIn];
-    __shared__ __align__(16) uint8_t s_out[kPayOut];
+    __shared__ PqPlainStage<kPlainStrings> stage;
     const PqPage pg = pages[blockIdx.x];
     if (pg.bad || pg.num_values == 0) return;
     const PqChunk ch = chunks[pg.chunk];
-    // kind 1: pages that do not need the value walk's offsets; kind 2: PLAIN BYTE_ARRAY pages (they do); 0: all
-    if (kind != 0 && (kind == 2) != (ch.phys == pq::T_BYTE_ARRAY && pg.enc == ENC_PLAIN)) return;
+    if (kPlainStrings != (ch.phys == pq::T_BYTE_ARRAY && pg.enc == ENC_PLAIN)) return;
     const PqOut out = outs[ch.run * n_cols + ch.col];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int64_t row0 = pg.row0, row1 = pg.row0 + pg.num_values;
@@ -1155,7 +1166,11 @@ k_pq_expand(const PqPage *pages, const PqPage *dicts, const PqChunk *chunks, con
         __syncthreads();
     }
     if (varlen) {
-        if (!is_dict) {
+        if constexpr (kPlainStrings) {
+            auto &s_vs = stage.vs;
+            auto &s_bnd = stage.bnd;
+            auto &s_in = stage.in;
+            auto &s_out = stage.out;
             // PLAIN: the page's payload is its value stream with the 4-byte length words squeezed out.  Batches of
             // kExpThreads values: the batch's stretch of the stream comes into shared memory with 16-byte async copies
             // (the NEXT batch is in flight while this one is worked on), every thread moves ONE value byte by byte
@@ -1471,8 +1486,8 @@ static pg_status expand_pages(cudaStream_t sm, bool byte_arrays, PqPage *d_pages
                               const PqChunk *d_chunks, const PqOut *d_outs, int nc, const int32_t *d_ids, int32_t *d_vstart,
                               const int32_t *d_dict_off, const int32_t *d_dict_len, int32_t *d_err, int *launches) {
     if (!byte_arrays) {
-        k_pq_expand<<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                                d_dict_len, d_err, 0);
+        k_pq_expand<false><<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart,
+                                                       d_dict_off, d_dict_len);
         (*launches)++;
         return PG_OK;
     }
@@ -1492,11 +1507,11 @@ static pg_status expand_pages(cudaStream_t sm, bool byte_arrays, PqPage *d_pages
     k_pq_walk_values<<<(np + kWvWarps * 32 - 1) / (kWvWarps * 32), kWvWarps * 32, 0, side>>>(
         d_pages, np, d_chunks, d_vstart, d_err);
     // the PLAIN BYTE_ARRAY pages follow their walk on the side stream; everything else expands on the main one
-    k_pq_expand<<<np, kExpThreads, 0, side>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                              d_dict_len, d_err, 2);
+    k_pq_expand<true><<<np, kExpThreads, 0, side>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
+                                                    d_dict_len);
     PG_CUDA(cudaEventRecord(ev_join, side));
-    k_pq_expand<<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                            d_dict_len, d_err, 1);
+    k_pq_expand<false><<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
+                                                   d_dict_len);
     PG_CUDA(cudaStreamWaitEvent(sm, ev_join, 0));
     *launches += 3;
     return PG_OK;

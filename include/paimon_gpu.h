@@ -312,11 +312,15 @@ pg_status pg_parquet_free(uint64_t reader);
  * GPUDirect storage or produced by pg_parquet_encode; must stay valid during the call only).  Only the footers are
  * parsed on the host; page headers are parsed on the device.
  * `column_names` (n_key + 2 + n_val entries, or NULL = positional) are the names the read schema's fields have in the
- * files: columns are resolved BY NAME like the reference does (ParquetReaderFactory.java:113-148 clipParquetSchema):
- * a nullable read field the file does not have decodes as all-NULL (file written before ADD COLUMN), file columns
- * the read schema does not name are ignored (DROP COLUMN), and a file column that is narrower than the read field is
- * widened on the fly (INT-family -> BIGINT, FLOAT -> DOUBLE: the casts of DataFileRecordReader.java:55-57 that need
- * no rewrite).  Anything else (renames without the old name, other casts) is refused with PG_ERR_UNSUPPORTED.
+ * files; this holds for pg_orc_read_section too.  Columns are resolved BY NAME like the reference does
+ * (ParquetReaderFactory.java:113-148 clipParquetSchema): a nullable read field the file does not have decodes as
+ * all-NULL (file written before ADD COLUMN), file columns the read schema does not name are ignored (DROP COLUMN; of
+ * two equal names in a file the first counts), and a file column that is narrower than the read field is widened on
+ * the fly (INT-family -> BIGINT, FLOAT -> DOUBLE: the casts of DataFileRecordReader.java:55-57 that need no rewrite).
+ * A positional read needs files with exactly n_key + 2 + n_val columns.  Anything else (renames without the old name,
+ * other casts, a var-len field that only some files with rows of one run have) is refused with PG_ERR_UNSUPPORTED; a
+ * NULL entry in `column_names`, and a descriptor with another `mem`, a negative `size`, NULL `bytes` for a non-empty
+ * file or a `run` outside [0, n_runs), are PG_ERR_INVALID.
  * `read_columns` ([n_key + 2 + n_val] bytes, or NULL = all) is the read-type projection pushed into the decoder
  * (MergeFileSplitRead.withReadType, operation/MergeFileSplitRead.java:133-163): columns with 0 are not decoded and the
  * runs carry no buffers for them; key, sequence-number and kind columns are always read (keys are never projected

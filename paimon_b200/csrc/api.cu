@@ -232,7 +232,41 @@ pg_status oom(const char *who, const char *what, size_t bytes) {
                                  " MiB wanted, " + std::to_string(fr >> 20) + " of " + std::to_string(tot >> 20) + " MiB free)");
 }
 
-pg_status RunBuilder::read_columns(const uint8_t *read_cols) {
+pg_status check_file_desc(const pg_file_desc &f) {
+    if (f.mem != PG_MEM_HOST && f.mem != PG_MEM_DEVICE)
+        return fail(PG_ERR_INVALID, "file descriptor: memory kind " + std::to_string(f.mem) + " is neither host nor device");
+    if (f.size < 0) return fail(PG_ERR_INVALID, "file descriptor: negative size");
+    if (f.size > 0 && !f.bytes) return fail(PG_ERR_INVALID, "file descriptor: no bytes for a file of " + std::to_string(f.size) + " bytes");
+    return PG_OK;
+}
+
+pg_status check_section_args(uint64_t schema, const pg_file_desc *files, int n_files, int n_runs, const uint64_t *out_runs,
+                             std::shared_ptr<const Schema> *s) {
+    *s = g_schemas.get(schema);
+    if (!*s || !out_runs || n_files < 0 || n_runs < 0 || (n_files > 0 && !files))
+        return fail(PG_ERR_INVALID, "bad schema handle or null argument");
+    for (int i = 0; i < n_files; i++) {
+        pg_status st = check_file_desc(files[i]);
+        if (st) return st;
+        if (files[i].run < 0 || files[i].run >= n_runs)
+            return fail(PG_ERR_INVALID, "file descriptor: run index " + std::to_string(files[i].run) + " out of range");
+    }
+    return PG_OK;
+}
+
+pg_status file_image(Scratch &scratch, const uint8_t *bytes, int64_t size, const char *who, const uint8_t **out) {
+    uint8_t *d = (uint8_t *)scratch.take((size_t)size + 64);
+    if (!d) return oom(who, "a file image", (size_t)size);
+    PG_CUDA(cudaMemcpyAsync(d, bytes, (size_t)size, cudaMemcpyHostToDevice, scratch.stream));
+    *out = d;
+    return PG_OK;
+}
+
+pg_status RunBuilder::read_columns(const uint8_t *read_cols, const char *const *column_names) {
+    names = column_names;
+    if (names)
+        for (int c = 0; c < nc; c++)
+            if (!names[c]) return fail(PG_ERR_INVALID, std::string(who) + ": column name " + std::to_string(c) + " is NULL");
     if (!read_cols) return PG_OK;
     for (int c = 0; c < schema->n_key + 2; c++)
         if (!read_cols[c]) return fail(PG_ERR_INVALID, std::string(who) + ": key, sequence number and kind columns are always read");
@@ -240,9 +274,39 @@ pg_status RunBuilder::read_columns(const uint8_t *read_cols) {
     return PG_OK;
 }
 
-pg_status RunBuilder::check_rows() const {
+pg_status RunBuilder::add_file(int run, int64_t rows, const std::vector<std::string> &cols) {
+    if (!names && (int)cols.size() != nc)
+        return fail(PG_ERR_UNSUPPORTED, std::string(who) + ": the file has " + std::to_string(cols.size()) + " columns and the "
+                                        "read schema " + std::to_string(nc) + " (pass the field names)");
+    std::unordered_map<std::string, int> by_name;
+    if (names) for (int i = 0; i < (int)cols.size(); i++) by_name.emplace(cols[i], i);
+    std::vector<int> fc(nc, -2);
+    for (int c = 0; c < nc; c++) {
+        if (!read[c]) continue;
+        fc[c] = c;
+        if (names) {
+            auto it = by_name.find(names[c]);               // (of two equal names in a file, the first counts)
+            fc[c] = it == by_name.end() ? -1 : it->second;
+        }
+        if (fc[c] == -1 && (c < schema->n_key + 2 || !schema->field(c).nullable))
+            return fail(PG_ERR_UNSUPPORTED, std::string(who) + ": the file has no column '" + names[c] + "' and the read "
+                                            "schema does not allow NULL for it");
+        const size_t i = (size_t)run * nc + c;
+        if (fc[c] == -1) missing[i] = 1;
+        if (rows > 0) with_rows[i] |= fc[c] == -1 ? 2 : 1;
+    }
+    file_col.push_back(std::move(fc));
+    file_row0.push_back(place_file(run, rows));
+    return PG_OK;
+}
+
+pg_status RunBuilder::check_runs() const {
     for (int64_t n : run_rows)
         if (n > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, std::string(who) + ": more than 2^31 rows in one run");
+    for (size_t i = 0; i < with_rows.size(); i++)
+        if (with_rows[i] == 3 && is_varlen(schema->field((int)(i % nc)).type))
+            return fail(PG_ERR_UNSUPPORTED, std::string(who) + ": a var-len column exists in some files with rows of a sorted "
+                                            "run only (mixed table schemas inside one run: not decoded on device)");
     return PG_OK;
 }
 

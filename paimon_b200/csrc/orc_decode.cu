@@ -15,7 +15,6 @@
 #include <cstring>
 #include <memory>
 #include <stdexcept>
-#include <unordered_map>
 
 #include "inflate_device.cuh"
 #include "orc_device.cuh"
@@ -150,23 +149,17 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
     PG_CUDA(cudaEventCreate(&tm.e0));
     PG_CUDA(cudaEventCreate(&tm.e1));
     PG_CUDA(cudaEventRecord(tm.e0, sm));
-    { pg_status st = b.read_columns(read_cols); if (st) return st; }
-    const std::vector<uint8_t> &wanted = b.read;
+    { pg_status st = b.read_columns(read_cols, names); if (st) return st; }
 
-    // ---- file tails, schema mapping by name, plans
+    // ---- file tails, column resolution, plans
     std::vector<orc::FileTail> tails(nf);
     std::vector<orc::Plan> plans(nf);
     std::vector<const uint8_t *> d_file(nf, nullptr);
-    std::vector<int64_t> file_row0(nf, 0);
     int64_t file_bytes = 0, page_bytes = 0;
     bool any_compressed = false, any_zstd = false;
-    std::vector<uint8_t> col_missing((size_t)n_runs * nc, 0);
-    std::vector<int> files_of_run(n_runs, 0);
     for (int f = 0; f < nf; f++) {
         if (files[f].mem != PG_MEM_HOST)
             return fail(PG_ERR_UNSUPPORTED, "orc: the file bytes must be host memory (the footers and chunk headers are walked on the host)");
-        if (files[f].run < 0 || files[f].run >= n_runs) return fail(PG_ERR_INVALID, "orc section: run index out of range");
-        std::vector<int> file_col(nc, -1);
         try {
             tails[f] = orc::parse_file(files[f].bytes, files[f].size);
             const orc::FileTail &t = tails[f];
@@ -178,67 +171,34 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
             if (t.compression == orc::C_ZSTD) any_zstd = true;
             if (t.block_size > (1u << 30)) return fail(PG_ERR_UNSUPPORTED, "orc: compression block size above 1 GiB");
             const orc::Type &root = t.types[0];
-            std::unordered_map<std::string, int> by_name;
-            for (size_t i = 0; i < root.field_names.size() && i < root.subtypes.size(); i++) by_name.emplace(root.field_names[i], (int)i);
+            if (root.field_names.size() != root.subtypes.size())
+                return fail(PG_ERR_FORMAT, "orc: the root struct's field names do not match its fields");
+            { pg_status st = b.add_file(files[f].run, (int64_t)t.rows, root.field_names); if (st) return st; }
+            const std::vector<int> &file_col = b.file_col[f];
             for (int c = 0; c < nc; c++) {
-                if (!wanted[c]) continue;
-                int fc = -1;
-                if (names) {
-                    auto it = by_name.find(names[c] ? names[c] : "");
-                    if (it != by_name.end()) fc = it->second;
-                } else if ((size_t)c < root.subtypes.size()) fc = c;
-                if (fc < 0) {
-                    if (c < s->n_key + 2 || !s->field(c).nullable)
-                        return fail(PG_ERR_UNSUPPORTED, std::string("orc: the file has no column '") + (names ? names[c] : "?") +
-                                                        "' and the read schema does not allow NULL for it");
-                    col_missing[(size_t)files[f].run * nc + c] |= 1;
-                    continue;
-                }
-                const uint32_t tid = root.subtypes[fc];
+                if (file_col[c] < 0) continue;
+                const uint32_t tid = root.subtypes[file_col[c]];
                 if (tid >= t.types.size() || !orc_type_ok(s->field(c).type, t.types[tid]))
                     return fail(PG_ERR_UNSUPPORTED, "orc: column " + std::to_string(c) + " has an ORC type the device decoder does "
                                                     "not map to the table type (timestamps, DECIMAL(p > 18), nested types: Java side)");
-                file_col[c] = fc;
             }
-            if (!names && (int)root.subtypes.size() != nc)
-                return fail(PG_ERR_UNSUPPORTED, "orc: the file's column count differs from the read schema (pass the field names)");
             plans[f] = orc::plan_file(t, files[f].bytes, files[f].size, file_col);
         } catch (const std::exception &e) {
             // (a codec or type this decoder does not cover is a refusal, not a malformed file)
             const bool refusal = strstr(e.what(), "is not decoded") != nullptr || strstr(e.what(), "not supported") != nullptr;
             return fail(refusal ? PG_ERR_UNSUPPORTED : PG_ERR_FORMAT, e.what());
         }
-        file_row0[f] = b.place_file(files[f].run, (int64_t)tails[f].rows);
-        files_of_run[files[f].run]++;
         file_bytes += files[f].size;
-        uint8_t *d = (uint8_t *)scratch.take((size_t)files[f].size + 64);
-        if (!d) return oom("orc", "a file image", (size_t)files[f].size);
-        PG_CUDA(cudaMemcpyAsync(d, files[f].bytes, (size_t)files[f].size, cudaMemcpyHostToDevice, sm));
-        d_file[f] = d;
+        { pg_status st = file_image(scratch, files[f].bytes, files[f].size, "orc", &d_file[f]); if (st) return st; }
     }
-    { pg_status st = b.check_rows(); if (st) return st; }
-    // a var-len column that only some files of a run have would need offsets filled for the other files' rows
-    {
-        std::vector<int> present_files((size_t)n_runs * nc, 0);
-        for (int f = 0; f < nf; f++)
-            for (const orc::PlanTask &t : plans[f].tasks) if (t.stripe == 0) present_files[(size_t)files[f].run * nc + t.col]++;
-        for (int f = 0; f < nf; f++) {
-            if (!tails[f].stripes.empty()) continue;       // a file without stripes has no tasks: it lacks nothing
-            for (int c = 0; c < nc; c++) if (wanted[c]) present_files[(size_t)files[f].run * nc + c]++;
-        }
-        for (int r = 0; r < n_runs; r++)
-            for (int c = 0; c < nc; c++)
-                if (wanted[c] && is_varlen(s->field(c).type) && col_missing[(size_t)r * nc + c] && present_files[(size_t)r * nc + c] > 0 &&
-                    present_files[(size_t)r * nc + c] < files_of_run[r])
-                    return fail(PG_ERR_UNSUPPORTED, "orc: a var-len column exists in some files of a sorted run only");
-    }
+    { pg_status st = b.check_runs(); if (st) return st; }
 
     // ---- output columns.  ORC columns are nullable by format: every column the read schema calls nullable gets a
     // bitmap.  Var-len lengths are scanned in place: rows nobody writes must read 0; missing columns are all NULL.
     {
         std::vector<uint8_t> bitmap(nc), zero((size_t)n_runs * nc);
         for (int c = 0; c < nc; c++) bitmap[c] = s->field(c).nullable;
-        for (size_t i = 0; i < zero.size(); i++) zero[i] = is_varlen(s->field((int)(i % nc)).type) || col_missing[i];
+        for (size_t i = 0; i < zero.size(); i++) zero[i] = is_varlen(s->field((int)(i % nc)).type) || b.missing[i];
         pg_status st = b.alloc(bitmap, zero);
         if (st) return st;
     }
@@ -274,7 +234,7 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
             const OutColumn &o = b.out[(size_t)r * nc + p.col];
             orcdev::Task k;
             memset(&k, 0, sizeof(k));
-            k.row0 = file_row0[f] + p.row0;
+            k.row0 = b.file_row0[f] + p.row0;
             k.rows = p.rows;
             k.kind = p.kind; k.enc = p.enc; k.dict_size = (int32_t)p.dict_size; k.scale = p.scale;
             k.out_width = type_width(s->field(p.col).type);
@@ -382,11 +342,10 @@ using namespace pg;
 extern "C" pg_status pg_orc_read_section(uint64_t schema, const pg_file_desc *files, int32_t n_files, int32_t n_runs,
                                          const char *const *column_names, const uint8_t *read_columns, uint64_t *out_runs,
                                          pg_section_info *info) {
-    std::shared_ptr<Schema> s = g_schemas.get(schema);
-    if (!s || !out_runs || n_files < 0 || n_runs < 0 || (n_files > 0 && !files))
-        return fail(PG_ERR_INVALID, "bad schema handle or null argument");
-    if (n_runs == 0) return n_files == 0 ? PG_OK : fail(PG_ERR_INVALID, "files without runs");
-    pg_status st = ensure_device();
+    std::shared_ptr<const Schema> s;
+    pg_status st = check_section_args(schema, files, n_files, n_runs, out_runs, &s);
+    if (st || n_runs == 0) return st;
+    st = ensure_device();
     if (st) return st;
     return orc_decode_section(s, files, n_files, n_runs, column_names, read_columns, out_runs, info);
 }

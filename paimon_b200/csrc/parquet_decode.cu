@@ -30,7 +30,6 @@
 #include <cstring>
 #include <memory>
 #include <stdexcept>
-#include <unordered_map>
 
 #include "device_utils.cuh"
 #include "parquet_meta.h"
@@ -1279,50 +1278,25 @@ static int phys_width_of(int phys) {
     return phys == pq::T_INT32 || phys == pq::T_FLOAT ? 4 : (phys == pq::T_INT64 || phys == pq::T_DOUBLE ? 8 : 0);
 }
 
-// The file's columns against the read schema [_KEY_*, _SEQUENCE_NUMBER, _VALUE_KIND, value...].
-//   names == NULL: positional — same column count, compatible physical types (the single-file reader).
-//   names != NULL: BY NAME, as the reference resolves them (ParquetReaderFactory.clipParquetSchema -> containsField):
-//     a read column the file does not have becomes an all-NULL column (a file written before ADD COLUMN; the field
-//     must be nullable, key / sequence / kind columns must exist), extra file columns are ignored (DROP COLUMN), the
-//     order in the file does not matter.  Renames are resolved by field id above this layer (SchemaEvolutionUtil):
-//     the caller passes the names the field had in the file's schema.
-// file_col[c] = the file's leaf column of read column c, -1 = not in the file, -2 = not requested (read_cols[c] == 0)
-static pg_status map_file_schema(const Schema *s, const pq::FileMetaData &m, const char *const *names,
-                                 const uint8_t *read_cols, std::vector<int> *file_col) {
-    const int nc = s->n_cols();
+// A file of run `run` against the read schema [_KEY_*, _SEQUENCE_NUMBER, _VALUE_KIND, value...]: a flat schema, whose
+// columns b.add_file resolves, with physical types that map to the read types and codecs the device decodes.
+static pg_status map_file_schema(RunBuilder &b, const pq::FileMetaData &m, int run) {
     if (m.schema.empty()) return fail(PG_ERR_FORMAT, "parquet: empty schema");
     const int nleaf = (int)m.schema.size() - 1;
     if (m.schema[0].num_children != nleaf)
         return fail(PG_ERR_UNSUPPORTED, "parquet: nested columns are not decoded on device (flat KeyValue file schemas are)");
-    for (int i = 1; i <= nleaf; i++)
+    std::vector<std::string> cols(nleaf);
+    for (int i = 1; i <= nleaf; i++) {
         if (m.schema[i].num_children != 0 || m.schema[i].repetition == pq::R_REPEATED)
             return fail(PG_ERR_UNSUPPORTED, "parquet: nested / repeated column " + m.schema[i].name);
-    file_col->assign(nc, -1);
-    if (!names) {
-        if (nleaf != nc)
-            return fail(PG_ERR_UNSUPPORTED, "parquet: only flat schemas whose columns match the KeyValue file schema "
-                                            "[_KEY_*, _SEQUENCE_NUMBER, _VALUE_KIND, value...] are decoded on device");
-        for (int c = 0; c < nc; c++) (*file_col)[c] = c;
-    } else {
-        std::unordered_map<std::string, int> by_name;
-        for (int i = 0; i < nleaf; i++) by_name.emplace(m.schema[i + 1].name, i);
-        for (int c = 0; c < nc; c++) {
-            if (!names[c]) return fail(PG_ERR_INVALID, "parquet: null column name");
-            auto it = by_name.find(names[c]);
-            if (it != by_name.end()) { (*file_col)[c] = it->second; continue; }
-            if (read_cols && !read_cols[c]) continue;
-            if (c < s->n_key + 2 || !s->field(c).nullable)
-                return fail(PG_ERR_UNSUPPORTED, std::string("parquet: the file has no column '") + names[c] + "' and the read "
-                                                "schema does not allow NULL for it (a file written under another table "
-                                                "schema needs the Java-side schema-evolution mapping)");
-        }
+        cols[i - 1] = m.schema[i].name;
     }
-    for (int c = 0; c < nc; c++) {
-        if (read_cols && !read_cols[c]) { (*file_col)[c] = -2; continue; }
-        const int fc = (*file_col)[c];
+    { pg_status st = b.add_file(run, m.num_rows, cols); if (st) return st; }
+    for (int c = 0; c < b.nc; c++) {
+        const int fc = b.file_col.back()[c];
         if (fc < 0) continue;
         const pq::SchemaElement &e = m.schema[fc + 1];
-        if (phys_cast(s->field(c).type, e.type) < 0)
+        if (phys_cast(b.schema->field(c).type, e.type) < 0)
             return fail(PG_ERR_UNSUPPORTED, "parquet: column " + e.name + " has a physical type the device decoder "
                                             "does not map to the table type");
     }
@@ -1409,36 +1383,24 @@ static pg_status fetch_footers(const std::vector<SectionFile> &files, cudaStream
 struct ChunkTables {
     std::vector<PqChunk> chunks;
     std::vector<PqPair> pairs;
-    std::vector<uint8_t> col_missing;     // per (run, column): 1 = some, 2 = every file of the run lacks the column
     bool any_snappy = false, any_delta = false, any_zstd = false;
     int64_t pair_rows = 0;
 };
 
 static pg_status build_chunk_tables(const Schema *s, const std::vector<SectionFile> &files,
                                     const std::vector<const uint8_t *> &d_file, const std::vector<const pq::FileMetaData *> &meta,
-                                    const std::vector<std::vector<int>> &file_col, const std::vector<int64_t> &file_row0,
                                     const RunBuilder &b, ChunkTables &t) {
     const int nc = s->n_cols();
     const int n_runs = (int)b.run_rows.size();
     std::vector<std::vector<int>> run_files(n_runs);
     for (int f = 0; f < (int)files.size(); f++) run_files[files[f].run].push_back(f);
-    // (run, column) pairs some / all of whose files lack the column: the rows of those files are NULL
-    t.col_missing.assign((size_t)n_runs * nc, 0);
     for (int r = 0; r < n_runs; r++) {
         for (int c = 0; c < nc; c++) {
             if (!b.read[c]) continue;
             const int chunk0 = (int)t.chunks.size();
-            int n_missing = 0;
-            for (int f : run_files[r]) if (file_col[f][c] < 0) n_missing++;
-            if (n_missing > 0) {
-                t.col_missing[(size_t)r * nc + c] = n_missing == (int)run_files[r].size() ? 2 : 1;
-                if (n_missing != (int)run_files[r].size() && is_varlen(s->field(c).type))
-                    return fail(PG_ERR_UNSUPPORTED, "parquet: a var-len column exists in some files of a sorted run only "
-                                                    "(mixed table schemas inside one run: not decoded on device)");
-            }
             for (int f : run_files[r]) {
                 const pq::FileMetaData &m = *meta[f];
-                const int fc = file_col[f][c];
+                const int fc = b.file_col[f][c];
                 int64_t rg_row0 = 0;
                 int64_t rows = 0;
                 if (fc < 0) continue;
@@ -1454,7 +1416,7 @@ static pg_status build_chunk_tables(const Schema *s, const std::vector<SectionFi
                     ch.avail = std::min<int64_t>(cc.total_compressed_size > 0 ? cc.total_compressed_size : files[f].size,
                                                  files[f].size - start);
                     ch.num_values = cc.num_values;
-                    ch.row0 = file_row0[f] + rg_row0;
+                    ch.row0 = b.file_row0[f] + rg_row0;
                     ch.col = c; ch.run = r; ch.file = f; ch.codec = cc.codec;
                     ch.max_def = m.schema[fc + 1].repetition == pq::R_OPTIONAL ? 1 : 0;
                     ch.phys = cc.type;
@@ -1529,6 +1491,7 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const st
     SectionTimer tm;
     PG_CUDA(cudaEventCreate(&tm.e0));
     PG_CUDA(cudaEventCreate(&tm.e1));
+    { pg_status st = b.read_columns(read_cols, names); if (st) return st; }
 
     // ---- file bytes on the device, footers on the host
     std::vector<const uint8_t *> d_file(nf, nullptr);
@@ -1538,39 +1501,31 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const st
     PG_CUDA(cudaEventRecord(tm.e0, sm));
     for (int f = 0; f < nf; f++) {
         const SectionFile &sf = files[f];
-        if (!sf.bytes || sf.size < 12) return fail(PG_ERR_FORMAT, "parquet: missing PAR1 magic (encrypted or not a Parquet file)");
-        if (sf.run < 0 || sf.run >= n_runs) return fail(PG_ERR_INVALID, "parquet section: run index out of range");
+        if (sf.size < 12) return fail(PG_ERR_FORMAT, "parquet: missing PAR1 magic (encrypted or not a Parquet file)");
         file_bytes += sf.size;
         if (sf.mem == PG_MEM_DEVICE) d_file[f] = sf.bytes;
         else {
-            uint8_t *d = (uint8_t *)scratch.take((size_t)sf.size + 64);
-            if (!d) return oom("parquet", "a file image", (size_t)sf.size);
-            PG_CUDA(cudaMemcpyAsync(d, sf.bytes, (size_t)sf.size, cudaMemcpyHostToDevice, sm));
-            d_file[f] = d;
+            { pg_status st = file_image(scratch, sf.bytes, sf.size, "parquet", &d_file[f]); if (st) return st; }
             h2d += sf.size;
         }
     }
     { pg_status st = fetch_footers(files, sm, own_meta, meta); if (st) return st; }
-    { pg_status st = b.read_columns(read_cols); if (st) return st; }
     std::vector<uint8_t> any_optional(nc, 0);
-    std::vector<std::vector<int>> file_col(nf);
     for (int f = 0; f < nf; f++) {
-        pg_status st = map_file_schema(s.get(), *meta[f], names, read_cols, &file_col[f]);
+        pg_status st = map_file_schema(b, *meta[f], files[f].run);
         if (st) return st;
         for (int c = 0; c < nc; c++) {
-            const int fc = file_col[f][c];
+            const int fc = b.file_col[f][c];
             if (fc == -1 || (fc >= 0 && meta[f]->schema[fc + 1].repetition == pq::R_OPTIONAL)) any_optional[c] = 1;
         }
     }
-    std::vector<int64_t> file_row0(nf, 0);
-    for (int f = 0; f < nf; f++) file_row0[f] = b.place_file(files[f].run, meta[f]->num_rows);
-    { pg_status st = b.check_rows(); if (st) return st; }
+    { pg_status st = b.check_runs(); if (st) return st; }
     ChunkTables ct;
-    { pg_status st = build_chunk_tables(s.get(), files, d_file, meta, file_col, file_row0, b, ct); if (st) return st; }
+    { pg_status st = build_chunk_tables(s.get(), files, d_file, meta, b, ct); if (st) return st; }
     const int n_chunks = (int)ct.chunks.size(), n_pairs = (int)ct.pairs.size();
 
     // ---- output columns (the rows of files that lack a column stay NULL and get defined contents)
-    { pg_status st = b.alloc(any_optional, ct.col_missing); if (st) return st; }
+    { pg_status st = b.alloc(any_optional, b.missing); if (st) return st; }
     std::vector<PqOut> outs((size_t)n_runs * nc);
     auto fill_outs = [&] {
         for (size_t i = 0; i < outs.size(); i++) {
@@ -1753,8 +1708,9 @@ static pg_status pq_open(uint64_t schema, const uint8_t *bytes, int64_t size, ui
         return fail(PG_ERR_FORMAT, e.what());
     }
     const pq::FileMetaData &m = rd->meta;
-    std::vector<int> file_col;
-    pg_status st = map_file_schema(s.get(), m, nullptr, nullptr, &file_col);
+    Scratch scratch(nullptr);                          // (stays empty: the columns are resolved by position on the host)
+    RunBuilder b(s, 1, scratch, "parquet");
+    pg_status st = map_file_schema(b, m, 0);
     if (st) return st;
     const int nc = s->n_cols();
     rd->n_rows = m.num_rows;
@@ -1969,17 +1925,13 @@ pg_status pg_parquet_read_run(uint64_t reader, uint64_t *out_run) {
 pg_status pg_parquet_read_section(uint64_t schema, const pg_file_desc *files, int32_t n_files, int32_t n_runs,
                                   const char *const *column_names, const uint8_t *read_columns, uint64_t *out_runs,
                                   pg_section_info *info) {
-    std::shared_ptr<Schema> s = g_schemas.get(schema);
-    if (!s || !out_runs || n_files < 0 || n_runs < 0 || (n_files > 0 && !files))
-        return fail(PG_ERR_INVALID, "bad schema handle or null argument");
-    if (n_runs == 0) return n_files == 0 ? PG_OK : fail(PG_ERR_INVALID, "files without runs");
-    pg_status st = ensure_device();
+    std::shared_ptr<const Schema> s;
+    pg_status st = check_section_args(schema, files, n_files, n_runs, out_runs, &s);
+    if (st || n_runs == 0) return st;
+    st = ensure_device();
     if (st) return st;
     std::vector<SectionFile> fs(n_files);
-    for (int i = 0; i < n_files; i++) {
-        if (files[i].mem != PG_MEM_HOST && files[i].mem != PG_MEM_DEVICE) return fail(PG_ERR_INVALID, "bad memory kind");
-        fs[i] = SectionFile{files[i].bytes, files[i].size, files[i].mem, files[i].run, nullptr};
-    }
+    for (int i = 0; i < n_files; i++) fs[i] = SectionFile{files[i].bytes, files[i].size, files[i].mem, files[i].run, nullptr};
     return decode_section(s, fs, n_runs, column_names, read_columns, out_runs, info);
 }
 

@@ -163,22 +163,38 @@ struct OutColumn {
     uint32_t *validity = nullptr;
 };
 
+// The arguments of a section read, checked before any device work (api.cu), PG_ERR_INVALID when wrong.  A file
+// descriptor: PG_MEM_HOST or PG_MEM_DEVICE, size >= 0, bytes when size > 0.  A section: the schema handle (*s receives
+// its lease), out_runs, the counts, and every file's descriptor with 0 <= run < n_runs.
+pg_status check_file_desc(const pg_file_desc &f);
+pg_status check_section_args(uint64_t schema, const pg_file_desc *files, int n_files, int n_runs, const uint64_t *out_runs,
+                             std::shared_ptr<const Schema> *s);
+// *out = a device copy of a host file in scratch, size + 64 bytes (the readers look past a page's end)
+pg_status file_image(Scratch &scratch, const uint8_t *bytes, int64_t size, const char *who, const uint8_t **out);
+
 // The runs a section decode or a deletion vector builds (api.cu), in the layout of DESIGN.md §3: per run one buffer
 // with the validity bitmaps first and contiguous (one memset clears them), then the values or int32 offsets of each
 // read column; after the caller's read-back of the exact sizes, one payload buffer per run for its var-len columns.
 // The runs stay in scratch.runs until finish() registers them.  `who` prefixes the error messages.
 struct RunBuilder {
     RunBuilder(std::shared_ptr<const Schema> s, int n_runs, Scratch &scratch, const char *who)
-        : schema(std::move(s)), nc(schema->n_cols()), scratch(scratch), who(who), read(nc, 1), run_rows(n_runs, 0) {}
-    // read[c] from a read-column mask (NULL = every column); the key, sequence number and kind columns are always read
-    pg_status read_columns(const uint8_t *read_cols);
+        : schema(std::move(s)), nc(schema->n_cols()), scratch(scratch), who(who), read(nc, 1), run_rows(n_runs, 0),
+          missing((size_t)n_runs * nc, 0), with_rows((size_t)n_runs * nc, 0) {}
+    // read[c] from a read-column mask (NULL = every column); the key, sequence number and kind columns are always read.
+    // names: the names the read schema's columns have in the files (NULL = by position), none of them NULL
+    pg_status read_columns(const uint8_t *read_cols, const char *const *names);
+    // The next file of the section: `rows` rows of run `run`, top-level columns `cols`.  Resolves the read columns in it
+    // by the `column_names` rule of paimon_gpu.h (file_col.back()) and places its rows (file_row0.back()).
+    pg_status add_file(int run, int64_t rows, const std::vector<std::string> &cols);
     // the rows of a file land behind those of the files in front of it in its run: returns its first row
     int64_t place_file(int run, int64_t rows) {
         const int64_t row0 = run_rows[run];
         run_rows[run] += rows;
         return row0;
     }
-    pg_status check_rows() const;    // no run holds more than 2^31 rows
+    // after the last add_file: no run holds more than 2^31 rows, and no var-len column is in some of the files with rows
+    // of a run but not in others (the offsets of the other files' rows would have to be filled)
+    pg_status check_runs() const;
     // one buffer per run (validity cleared); bitmap[c]: a read column carries validity, zero[r * nc + c]: clear the
     // values / offsets of that column of that run as well
     pg_status alloc(const std::vector<uint8_t> &bitmap, const std::vector<uint8_t> &zero);
@@ -192,7 +208,12 @@ struct RunBuilder {
     Scratch &scratch;
     const char *who;
     std::vector<uint8_t> read;       // per column: part of the read type (a run has no buffers for the others)
+    const char *const *names = nullptr;
     std::vector<int64_t> run_rows;
+    std::vector<std::vector<int>> file_col;  // per file and column: the file's column, -1 = absent (NULL rows), -2 = not read
+    std::vector<int64_t> file_row0;          // per file: its first row in its run
+    std::vector<uint8_t> missing;    // per (run, column): some file of the run lacks the column
+    std::vector<uint8_t> with_rows;  // per (run, column), bits: 1 = a file with rows has the column, 2 = one lacks it
     std::vector<OutColumn> out;
     int64_t decoded_bytes = 0;       // validity (n + 7) / 8, values n * width, offsets 4 (n + 1), payload bytes
 };

@@ -34,6 +34,10 @@ using namespace pg;
 
 extern "C" pg_status pg_files_upload_begin(const pg_file_desc *files, int32_t n_files, uint64_t *out_upload) {
     if (!out_upload || n_files < 0 || (n_files > 0 && !files)) return fail(PG_ERR_INVALID, "null argument");
+    for (int i = 0; i < n_files; i++) {
+        pg_status st = check_file_desc(files[i]);
+        if (st) return st;
+    }
     pg_status st = ensure_device();
     if (st) return st;
     auto up = std::make_unique<Upload>();
@@ -44,13 +48,10 @@ extern "C" pg_status pg_files_upload_begin(const pg_file_desc *files, int32_t n_
     PG_CUDA(cudaEventCreateWithFlags(&up->done, cudaEventDisableTiming));
     Scratch scratch(g_up_stream);                      // the buffers until the upload is registered
     for (int i = 0; i < n_files; i++) {
-        if (files[i].size < 0 || (files[i].size > 0 && !files[i].bytes)) return fail(PG_ERR_INVALID, "upload: bad file descriptor");
         pg_file_desc d = files[i];
-        if (files[i].mem == PG_MEM_HOST) {
-            void *b = scratch.take((size_t)files[i].size + 64);                    // (readers may look 8 bytes past a page)
-            if (!b) return fail(PG_ERR_CUDA, "upload: out of device memory (" + std::to_string(files[i].size) + " bytes)");
-            PG_CUDA(cudaMemcpyAsync(b, files[i].bytes, (size_t)files[i].size, cudaMemcpyHostToDevice, g_up_stream));
-            d.bytes = (const uint8_t *)b;
+        if (d.mem == PG_MEM_HOST) {
+            st = file_image(scratch, d.bytes, d.size, "upload", &d.bytes);
+            if (st) return st;
             d.mem = PG_MEM_DEVICE;
         }
         up->files.push_back(d);

@@ -109,6 +109,36 @@ def test_handle_validation_without_device():
             assert (info.n_columns, info.n_rows) == (3, 3)
 
 
+def test_bad_file_descriptors_are_refused_before_device_work():
+    """A section read checks every file descriptor (memory kind, size, bytes, run index) before it touches the device,
+    and an upload checks the same but for the run index."""
+    lib = N.load()
+    field = N.PgField(4, 0)                                # PG_INT64
+    desc = N.PgSchemaDesc(1, 0, C.pointer(field), None)
+    schema = C.c_uint64(0)
+    assert lib.pg_schema_create(C.byref(desc), C.byref(schema)) == 0
+    blob = (C.c_uint8 * 100)()
+    bad = {"no bytes": N.PgFileDesc(None, 100, N.PG_MEM_HOST, 0),
+           "negative size": N.PgFileDesc(C.addressof(blob), -1, N.PG_MEM_HOST, 0),
+           "memory kind": N.PgFileDesc(C.addressof(blob), 100, 5, 0),
+           "run index": N.PgFileDesc(C.addressof(blob), 100, N.PG_MEM_HOST, 1)}
+    try:
+        for case, d in bad.items():
+            files = (N.PgFileDesc * 1)(d)
+            runs = (C.c_uint64 * 1)()
+            for read_section in (lib.pg_parquet_read_section, lib.pg_orc_read_section):
+                assert read_section(schema.value, files, 1, 1, None, None, runs, None) == 1, case
+                err = lib.pg_last_error()
+                assert b"descriptor" in err or b"run index" in err, (case, err)
+                assert b"pg_init" not in err, case
+            if case != "run index":
+                upload = C.c_uint64(0)
+                assert lib.pg_files_upload_begin(files, 1, C.byref(upload)) == 1, case
+                assert b"descriptor" in lib.pg_last_error() and b"pg_init" not in lib.pg_last_error(), case
+    finally:
+        assert lib.pg_schema_free(schema.value) == 0
+
+
 def test_interval_partition_host_logic_matches_oracle():
     import random
     import numpy as np

@@ -379,18 +379,6 @@ def test_section_from_an_asynchronous_upload(tmp_path):
         N.check(N.load().pg_files_upload_free(12345))
 
 
-def test_section_of_empty_files(tmp_path):
-    from paimon_b200.format import read_section
-    schema = datagen.schema_c3(n_i64=1, n_f64=1, n_str=1)
-    path = str(tmp_path / "empty.parquet")
-    write_kv_parquet(KeyValueBatch.from_rows(schema, []), path)
-    blob = open(path, "rb").read()
-    readers, info = read_section(schema, [(blob, 0), (blob, 1)], 2)
-    assert info.n_rows == 0
-    for b in _fetch_and_close(readers):
-        assert b is None or b.n_rows == 0
-
-
 def test_boolean_columns_plain_and_rle(tmp_path):
     """BOOLEAN: PLAIN pages are bit-packed LSB first (VectorizedPlainValuesReader.java:68-84); data page V2 writers
     use RLE for booleans."""
@@ -405,27 +393,6 @@ def test_boolean_columns_plain_and_rle(tmp_path):
         for opts in (dict(), dict(data_page_version="2.0"), dict(use_dictionary=False, data_page_size=128),
                      dict(data_page_version="2.0", compression="snappy", data_page_size=200)):
             check_file(schema, batch, str(tmp_path / f"bool{n}.parquet"), **opts)
-
-
-def test_columns_are_resolved_by_name_not_position(tmp_path):
-    """The reference resolves file columns by NAME (ParquetReaderFactory.clipParquetSchema): a read schema that lists
-    the value fields in another order gets every field's own values — never the positional neighbour's."""
-    from paimon_b200.format import read_section
-    vt_a = RowType((DataField("pk", "BIGINT", False), DataField("a", "BIGINT", True), DataField("b", "BIGINT", True)))
-    vt_b = RowType((DataField("pk", "BIGINT", False), DataField("b", "BIGINT", True), DataField("a", "BIGINT", True)))
-    sa, sb = KeyValueSchema.of(vt_a, ["pk"]), KeyValueSchema.of(vt_b, ["pk"])
-    batch = KeyValueBatch.from_rows(sa, [(k, k, 0, k, k * 2, k * 3) for k in range(100)])
-    path = str(tmp_path / "a.parquet")
-    write_kv_parquet(batch, path)
-    blob = open(path, "rb").read()
-    readers, _ = read_section(sa, [(blob, 0)], 1)
-    assert _fetch_and_close(readers)[0].equals(batch)
-    readers, _ = read_section(sb, [(blob, 0)], 1)
-    swapped = KeyValueBatch.from_rows(sb, [(k, k, 0, k, k * 3, k * 2) for k in range(100)])
-    assert _fetch_and_close(readers)[0].equals(swapped)
-    # positional reading (no names) of a file whose types line up is what the single-file reader does
-    readers, _ = read_section(sb, [(blob, 0)], 1, check_names=False)
-    assert _fetch_and_close(readers)[0].equals(KeyValueBatch.from_rows(sb, [(k, k, 0, k, k * 2, k * 3) for k in range(100)]))
 
 
 def test_section_from_device_resident_file_images(tmp_path):
@@ -506,7 +473,7 @@ def test_wide_fan_in_of_files_is_few_runs(tmp_path):
     assert got.equals(want), got.first_difference(want)
 
 
-# ------------------------------------------------------------------ read-type projection, schema evolution by name
+# ------------------------------------------------------------------ read-type projection
 
 def _drain(rd):
     from paimon_b200.merge_tree_readers import concat_batches
@@ -563,49 +530,6 @@ def test_read_type_projection_is_pushed_into_decode_and_merge(tmp_path, engine):
     from paimon_b200.sort_merge_reader import merge_runs
     got2 = merge_runs(schema, spec.with_read_fields(mask), runs)
     assert got2.equals(want), got2.first_difference(want)
-
-
-def test_schema_evolution_columns_resolve_by_name(tmp_path):
-    """Files written under older table schemas (ParquetReaderFactory.clipParquetSchema resolves by NAME;
-    DataFileRecordReader.java:55-57 casts): an added column is NULL in old files, a dropped column is ignored, column
-    order does not matter, INT widened to BIGINT and FLOAT to DOUBLE are cast on the fly."""
-    from paimon_b200.format import read_section
-    from paimon_b200.merge_tree_readers import concat_batches
-    read_vt = RowType((DataField("pk", "BIGINT", False), DataField("a", "BIGINT", True), DataField("f", "DOUBLE", True),
-                       DataField("b", "STRING", True), DataField("c", "DOUBLE", True)))
-    read_schema = KeyValueSchema.of(read_vt, ["pk"])
-    # v1: a INT, f FLOAT, b, no c, plus a column z that was dropped later; v2: another column order
-    v1 = KeyValueSchema.of(RowType((DataField("pk", "BIGINT", False), DataField("z", "INT", True), DataField("a", "INT", True),
-                                    DataField("f", "FLOAT", True), DataField("b", "STRING", True))), ["pk"])
-    v2 = KeyValueSchema.of(RowType((DataField("pk", "BIGINT", False), DataField("c", "DOUBLE", True), DataField("b", "STRING", True),
-                                    DataField("a", "BIGINT", True), DataField("f", "DOUBLE", True))), ["pk"])
-    rng = random.Random(4)
-
-    def opt(v):
-        return None if rng.random() < 0.3 else v
-    rows1 = [(k, k, 0, k, opt(k * 3), opt(rng.randrange(-2 ** 31, 2 ** 31)), opt(np.float32(rng.uniform(-9, 9)).item()),
-              opt("s%d" % k)) for k in range(0, 3000)]
-    rows2 = [(k, k, 0, k, opt(k / 7.0), opt("t%d" % k), opt(rng.randrange(-2 ** 62, 2 ** 62)), opt(rng.uniform(-1e9, 1e9)))
-             for k in range(5000, 9001)]
-    p1, p2 = str(tmp_path / "v1.parquet"), str(tmp_path / "v2.parquet")
-    write_kv_parquet(KeyValueBatch.from_rows(v1, rows1), p1, data_page_size=2048)
-    write_kv_parquet(KeyValueBatch.from_rows(v2, rows2), p2, use_dictionary=False)
-    want1 = KeyValueBatch.from_rows(read_schema, [(r[0], r[1], r[2], r[3], r[5], r[6], r[7], None) for r in rows1])
-    want2 = KeyValueBatch.from_rows(read_schema, [(r[0], r[1], r[2], r[3], r[6], r[7], r[5], r[4]) for r in rows2])
-    # each file as its own run, and both files as ONE run (a fixed-width column that only some files have)
-    readers, _ = read_section(read_schema, [(open(p1, "rb").read(), 0), (open(p2, "rb").read(), 1)], 2)
-    g1, g2 = _fetch_and_close(readers)
-    assert g1.equals(want1), g1.first_difference(want1)
-    assert g2.equals(want2), g2.first_difference(want2)
-    # in ONE run: column c exists in the second file only — allowed for fixed-width columns
-    readers, _ = read_section(read_schema, [(open(p1, "rb").read(), 0), (open(p2, "rb").read(), 0)], 1)
-    both = _fetch_and_close(readers)[0]
-    want = concat_batches(read_schema, [want1, want2])
-    assert both.equals(want), both.first_difference(want)
-    # a NOT NULL read field the file lacks, or a narrowing, is refused
-    bad_vt = RowType((DataField("pk", "BIGINT", False), DataField("a", "INT", True), DataField("nn", "BIGINT", False)))
-    with pytest.raises(N.UnsupportedOnDevice):
-        read_section(KeyValueSchema.of(bad_vt, ["pk"]), [(open(p2, "rb").read(), 0)], 1)
 
 
 @pytest.mark.parametrize("engine", ["dedup", "dedup-ignore-delete", "first-row", "partial-update"])

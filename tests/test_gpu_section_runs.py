@@ -1,7 +1,8 @@
 """The decoded runs of a section: the Parquet and the ORC decoder lay out the same runs from the same rows (read columns,
-NULL rows of a field some files lack, absent unread columns, `decoded_bytes`), and a deletion vector applied to a
-projected run keeps the projection."""
+NULL rows of a field some files lack, absent unread columns, `decoded_bytes`), both resolve the files' columns against
+the read schema by the same rule, and a deletion vector applied to a projected run keeps the projection."""
 import ctypes as C
+import random
 
 import numpy as np
 import pyarrow.orc as orc
@@ -14,7 +15,8 @@ from paimon_b200 import datagen
 from paimon_b200.columnar import KeyValueBatch
 from paimon_b200.format import read_section
 from paimon_b200.merge_function import DeduplicateMergeFunction
-from paimon_b200.sort_merge_reader import apply_deletion_vector
+from paimon_b200.merge_tree_readers import concat_batches
+from paimon_b200.sort_merge_reader import _SchemaHandle, apply_deletion_vector
 from paimon_b200.types import DataField, KeyValueSchema, RowType, is_varlen
 
 from parquet_util import to_arrow
@@ -76,6 +78,147 @@ def _layout(handle):
 def _filter(batch, deleted):
     gone = set(deleted)
     return KeyValueBatch.from_rows(batch.schema, [row for i, row in enumerate(batch.to_rows()) if i not in gone])
+
+
+def _fetch_and_close(readers):
+    out = []
+    for r in readers:
+        try:
+            out.append(r.read_batch())
+        finally:
+            r.close()
+    return out
+
+
+def _blob(tmp_path, name, batch, fmt):
+    path = str(tmp_path / f"{name}.{fmt}")
+    _write(batch, path, fmt)
+    return open(path, "rb").read()
+
+
+@pytest.mark.parametrize("fmt", ["parquet", "orc"])
+def test_section_of_empty_files(tmp_path, fmt):
+    schema = datagen.schema_c3(n_i64=1, n_f64=1, n_str=1)
+    blob = _blob(tmp_path, "empty", KeyValueBatch.from_rows(schema, []), fmt)
+    readers, info = read_section(schema, [(blob, 0), (blob, 1)], 2, file_format=fmt)
+    assert info.n_rows == 0
+    for b in _fetch_and_close(readers):
+        assert b is None or b.n_rows == 0
+
+
+@pytest.mark.parametrize("fmt", ["parquet", "orc"])
+def test_columns_are_resolved_by_name_not_position(tmp_path, fmt):
+    """The reference resolves file columns by NAME (ParquetReaderFactory.clipParquetSchema): a read schema that lists
+    the value fields in another order gets every field's own values — never the positional neighbour's."""
+    vt_a = RowType((DataField("pk", "BIGINT", False), DataField("a", "BIGINT", True), DataField("b", "BIGINT", True)))
+    vt_b = RowType((DataField("pk", "BIGINT", False), DataField("b", "BIGINT", True), DataField("a", "BIGINT", True)))
+    sa, sb = KeyValueSchema.of(vt_a, ["pk"]), KeyValueSchema.of(vt_b, ["pk"])
+    batch = KeyValueBatch.from_rows(sa, [(k, k, 0, k, k * 2, k * 3) for k in range(100)])
+    blob = _blob(tmp_path, "a", batch, fmt)
+    readers, _ = read_section(sa, [(blob, 0)], 1, file_format=fmt)
+    assert _fetch_and_close(readers)[0].equals(batch)
+    readers, _ = read_section(sb, [(blob, 0)], 1, file_format=fmt)
+    swapped = KeyValueBatch.from_rows(sb, [(k, k, 0, k, k * 3, k * 2) for k in range(100)])
+    assert _fetch_and_close(readers)[0].equals(swapped)
+    # positional reading (no names) of a file whose types line up is what the single-file reader does
+    readers, _ = read_section(sb, [(blob, 0)], 1, check_names=False, file_format=fmt)
+    assert _fetch_and_close(readers)[0].equals(KeyValueBatch.from_rows(sb, [(k, k, 0, k, k * 2, k * 3) for k in range(100)]))
+
+
+@pytest.mark.parametrize("fmt", ["parquet", "orc"])
+def test_schema_evolution_columns_resolve_by_name(tmp_path, fmt):
+    """Files written under older table schemas (ParquetReaderFactory.clipParquetSchema resolves by NAME;
+    DataFileRecordReader.java:55-57 casts): an added column is NULL in old files, a dropped column is ignored, column
+    order does not matter, INT widened to BIGINT and FLOAT to DOUBLE are cast on the fly."""
+    read_vt = RowType((DataField("pk", "BIGINT", False), DataField("a", "BIGINT", True), DataField("f", "DOUBLE", True),
+                       DataField("b", "STRING", True), DataField("c", "DOUBLE", True)))
+    read_schema = KeyValueSchema.of(read_vt, ["pk"])
+    # v1: a INT, f FLOAT, b, no c, plus a column z that was dropped later; v2: another column order
+    v1 = KeyValueSchema.of(RowType((DataField("pk", "BIGINT", False), DataField("z", "INT", True), DataField("a", "INT", True),
+                                    DataField("f", "FLOAT", True), DataField("b", "STRING", True))), ["pk"])
+    v2 = KeyValueSchema.of(RowType((DataField("pk", "BIGINT", False), DataField("c", "DOUBLE", True), DataField("b", "STRING", True),
+                                    DataField("a", "BIGINT", True), DataField("f", "DOUBLE", True))), ["pk"])
+    rng = random.Random(4)
+
+    def opt(v):
+        return None if rng.random() < 0.3 else v
+    rows1 = [(k, k, 0, k, opt(k * 3), opt(rng.randrange(-2 ** 31, 2 ** 31)), opt(np.float32(rng.uniform(-9, 9)).item()),
+              opt("s%d" % k)) for k in range(0, 3000)]
+    rows2 = [(k, k, 0, k, opt(k / 7.0), opt("t%d" % k), opt(rng.randrange(-2 ** 62, 2 ** 62)), opt(rng.uniform(-1e9, 1e9)))
+             for k in range(5000, 9001)]
+    b1 = _blob(tmp_path, "v1", KeyValueBatch.from_rows(v1, rows1), fmt)
+    b2 = _blob(tmp_path, "v2", KeyValueBatch.from_rows(v2, rows2), fmt)
+    want1 = KeyValueBatch.from_rows(read_schema, [(r[0], r[1], r[2], r[3], r[5], r[6], r[7], None) for r in rows1])
+    want2 = KeyValueBatch.from_rows(read_schema, [(r[0], r[1], r[2], r[3], r[6], r[7], r[5], r[4]) for r in rows2])
+    # each file as its own run, and both files as ONE run (a fixed-width column that only some files have)
+    readers, _ = read_section(read_schema, [(b1, 0), (b2, 1)], 2, file_format=fmt)
+    g1, g2 = _fetch_and_close(readers)
+    assert g1.equals(want1), g1.first_difference(want1)
+    assert g2.equals(want2), g2.first_difference(want2)
+    # in ONE run: column c exists in the second file only — allowed for fixed-width columns
+    readers, _ = read_section(read_schema, [(b1, 0), (b2, 0)], 1, file_format=fmt)
+    both = _fetch_and_close(readers)[0]
+    want = concat_batches(read_schema, [want1, want2])
+    assert both.equals(want), both.first_difference(want)
+    # a NOT NULL read field the file lacks, or a narrowing, is refused
+    bad_vt = RowType((DataField("pk", "BIGINT", False), DataField("a", "INT", True), DataField("nn", "BIGINT", False)))
+    with pytest.raises(N.UnsupportedOnDevice):
+        read_section(KeyValueSchema.of(bad_vt, ["pk"]), [(b2, 0)], 1, file_format=fmt)
+
+
+WITH_T = KeyValueSchema.of(RowType((DataField("pk", "BIGINT", False), DataField("a", "BIGINT", True),
+                                    DataField("t", "STRING", True))), ["pk"])
+NO_T = KeyValueSchema.of(RowType((DataField("pk", "BIGINT", False), DataField("a", "BIGINT", True))), ["pk"])
+
+
+def _rows(k0, n, with_t):
+    return [(k, k, 0, k, None if k % 3 == 0 else k * 5) + ((None if k % 4 == 0 else "t" * (k % 11),) if with_t else ())
+            for k in range(k0, k0 + n)]
+
+
+@pytest.mark.parametrize("fmt", ["parquet", "orc"])
+def test_var_len_column_in_some_files_of_a_run(tmp_path, fmt):
+    """A run is judged by its files with rows: a file without rows has no rows to fill, whether or not it has a var-len
+    column.  Only a var-len column that some files with rows of the run have and others lack is refused."""
+    empty_t = _blob(tmp_path, "empty_t", KeyValueBatch.from_rows(WITH_T, []), fmt)
+    empty_no_t = _blob(tmp_path, "empty_no_t", KeyValueBatch.from_rows(NO_T, []), fmt)
+    no_t = _blob(tmp_path, "no_t", KeyValueBatch.from_rows(NO_T, _rows(0, 2345, False)), fmt)
+    has_t = _blob(tmp_path, "has_t", KeyValueBatch.from_rows(WITH_T, _rows(3000, 1717, True)), fmt)
+    # (a) the file with rows lacks t, the empty file has it: t is NULL in every row
+    readers, _ = read_section(WITH_T, [(no_t, 0), (empty_t, 0)], 1, file_format=fmt)
+    got = _fetch_and_close(readers)[0]
+    want = KeyValueBatch.from_rows(WITH_T, [r + (None,) for r in _rows(0, 2345, False)])
+    assert got.equals(want), got.first_difference(want)
+    # (b) the file with rows has t, the empty file lacks it
+    readers, _ = read_section(WITH_T, [(has_t, 0), (empty_no_t, 0)], 1, file_format=fmt)
+    got = _fetch_and_close(readers)[0]
+    want = KeyValueBatch.from_rows(WITH_T, _rows(3000, 1717, True))
+    assert got.equals(want), got.first_difference(want)
+    # (c) two files with rows, one of them without t
+    with pytest.raises(N.UnsupportedOnDevice):
+        read_section(WITH_T, [(no_t, 0), (has_t, 0)], 1, file_format=fmt)
+
+
+@pytest.mark.parametrize("fmt", ["parquet", "orc"])
+def test_null_column_name_and_positional_column_count(tmp_path, fmt):
+    """A NULL entry in column_names is an invalid argument; a positional read needs the read schema's column count."""
+    has_t = _blob(tmp_path, "has_t", KeyValueBatch.from_rows(WITH_T, _rows(0, 100, True)), fmt)
+    with pytest.raises(N.UnsupportedOnDevice):
+        read_section(NO_T, [(has_t, 0)], 1, check_names=False, file_format=fmt)
+    lib = N.init(0)
+    sh = _SchemaHandle(WITH_T, 0)
+    try:
+        arr = np.frombuffer(has_t, np.uint8)
+        files = (N.PgFileDesc * 1)(N.PgFileDesc(arr.ctypes.data, len(arr), N.PG_MEM_HOST, 0))
+        nm = [f.name.encode() for f in WITH_T.file_fields()]
+        nm[-1] = None
+        names = (C.c_char_p * len(nm))(*nm)
+        runs = (C.c_uint64 * 1)()
+        fn = lib.pg_parquet_read_section if fmt == "parquet" else lib.pg_orc_read_section
+        assert fn(sh.handle, files, 1, 1, names, None, runs, None) == 1
+        assert b"NULL" in lib.pg_last_error()
+    finally:
+        sh.close()
 
 
 def test_parquet_and_orc_build_the_same_runs(tmp_path):

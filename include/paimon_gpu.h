@@ -407,6 +407,15 @@ typedef struct {
 
 pg_status pg_parquet_encode(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
                             const pg_parquet_write_options *options, uint64_t *out_file);
+/* The same file with its page bodies compressed.  `codec` is Parquet's CompressionCodec number: 0 UNCOMPRESSED (the
+ * bytes of pg_parquet_encode), 6 ZSTD (one frame per page body, written on the device; `level` is Paimon's
+ * file.compression.zstd-level: 1 and the negative fast levels are accepted and share one level-1-class strategy,
+ * 0 and levels >= 2 return PG_ERR_UNSUPPORTED).  The other codecs return PG_ERR_UNSUPPORTED, numbers outside the
+ * enum PG_ERR_INVALID.  Page headers carry both sizes, ColumnMetaData.codec is ZSTD and its
+ * total_uncompressed_size / total_compressed_size differ; pg_file_meta.ms_encode and launches cover the compression. */
+pg_status pg_parquet_encode_compressed(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
+                                       const pg_parquet_write_options *options, int32_t codec, int32_t level,
+                                       uint64_t *out_file);
 pg_status pg_parquet_file_meta(uint64_t file, pg_file_meta *out);
 /* whole-file statistics of one column: null count; min / max for fixed-width columns (integers and BOOLEAN as
  * int64, FLOAT / DOUBLE as double; absent when every value is NULL or a NaN was seen) */

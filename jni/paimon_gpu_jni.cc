@@ -275,6 +275,20 @@ JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetEncode(JNI
     PG_CHECK(pg_parquet_encode((uint64_t)source, ptrs.data(), row0, nRows, &opt, &h));
     return (jlong)h;
 }
+// The same with the page bodies compressed: codec = Parquet CompressionCodec (0 UNCOMPRESSED, 6 ZSTD), level =
+// file.compression.zstd-level
+JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetEncodeCompressed(JNIEnv *env, jclass, jlong source,
+                                                                                       jobjectArray names, jlong row0,
+                                                                                       jlong nRows, jlong rowGroupRows,
+                                                                                       jlong pageRows, jint codec,
+                                                                                       jint level) {
+    std::vector<std::string> keep;
+    std::vector<const char *> ptrs = utf_names(env, names, keep);
+    pg_parquet_write_options opt{rowGroupRows, pageRows};
+    uint64_t h = 0;
+    PG_CHECK(pg_parquet_encode_compressed((uint64_t)source, ptrs.data(), row0, nRows, &opt, codec, level, &h));
+    return (jlong)h;
+}
 JNIEXPORT jlongArray JNICALL Java_org_apache_paimon_gpu_NativeMerge_fileMeta(JNIEnv *env, jclass, jlong file) {
     pg_file_meta m{};
     pg_status fst = pg_parquet_file_meta((uint64_t)file, &m);

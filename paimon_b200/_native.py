@@ -150,6 +150,9 @@ _SIGNATURES = {
     "pg_run_apply_deletion_vector": (C.c_int32, [C.c_uint64, C.c_void_p, C.c_int64, C.POINTER(C.c_uint64)]),
     "pg_parquet_encode": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,
                                       C.POINTER(PgParquetWriteOptions), C.POINTER(C.c_uint64)]),
+    "pg_parquet_encode_compressed": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,
+                                                 C.POINTER(PgParquetWriteOptions), C.c_int32, C.c_int32,
+                                                 C.POINTER(C.c_uint64)]),
     "pg_parquet_file_meta": (C.c_int32, [C.c_uint64, C.POINTER(PgFileMeta)]),
     "pg_parquet_file_column_stats": (C.c_int32, [C.c_uint64, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int32),
                                                  C.c_void_p, C.c_void_p]),

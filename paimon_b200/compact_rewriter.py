@@ -14,7 +14,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 from dataclasses import dataclass, field
-from typing import List, Optional, Sequence
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -43,6 +43,37 @@ class WrittenFile:
     n_pages: int
 
 
+# Parquet CompressionCodec numbers (parquet.thrift) by the names Paimon's options use
+PARQUET_CODECS = {"none": 0, "uncompressed": 0, "snappy": 1, "gzip": 2, "lzo": 3, "brotli": 4, "lz4": 5, "zstd": 6,
+                  "lz4_raw": 7}
+
+
+def _per_level(value) -> Dict[int, str]:
+    """'file.compression.per.level' as a map: a dict, or the option's string form '0:lz4,5:zstd'."""
+    if isinstance(value, dict):
+        return {int(k): str(v) for k, v in value.items()}
+    out = {}
+    for item in str(value).split(","):
+        if item.strip():
+            k, v = item.split(":", 1)
+            out[int(k.strip())] = v.strip()
+    return out
+
+
+def compression_for_level(options: Optional[Dict[str, object]], level: int) -> Tuple[str, int]:
+    """(codec name, zstd level) of a data file written at `level`, the way the reference chooses them:
+    'file.compression.per.level' for the level, else 'file.compression' (default zstd) (KeyValueFileWriterFactory.java
+    :312-321, CoreOptions.java:299-323), overridden by 'parquet.compression' (RowDataParquetBuilder.java:121-122); the
+    level is 'parquet.compression.codec.zstd.level', else 'file.compression.zstd-level' (default 1;
+    ParquetFileFormat.java:98-101, CoreOptions.java:325-330)."""
+    options = options or {}
+    per_level = _per_level(options.get("file.compression.per.level", {}))
+    codec = per_level.get(level, options.get("file.compression", "zstd"))
+    codec = str(options.get("parquet.compression", codec)).lower()
+    zstd_level = int(options.get("parquet.compression.codec.zstd.level", options.get("file.compression.zstd-level", 1)))
+    return codec, zstd_level
+
+
 def file_column_names(schema: KeyValueSchema) -> List[str]:
     """[_KEY_*, _SEQUENCE_NUMBER, _VALUE_KIND, value...] (KeyValue.schema, KeyValue.java:130-138)."""
     return [f.name for f in schema.file_fields()]
@@ -50,22 +81,31 @@ def file_column_names(schema: KeyValueSchema) -> List[str]:
 
 class KeyValueDataFileWriter:
     """Encodes rows [row0, row0 + n_rows) of a device batch (a merge handle holding a batch, or a run handle) as
-    one Parquet data file and returns its DataFileMeta."""
+    one Parquet data file and returns its DataFileMeta.  `compression` names the page codec ('none' or 'zstd', compressed
+    on the device; the other Parquet codecs are refused by the library), `zstd_level` is file.compression.zstd-level."""
 
     def __init__(self, schema: KeyValueSchema, path: str, level: int, file_io: Optional[LocalFileIO] = None,
-                 row_group_rows: int = 0, page_rows: int = 0):
+                 row_group_rows: int = 0, page_rows: int = 0, compression: str = "none", zstd_level: int = 1):
         self.schema = schema
         self.path = path
         self.level = level
         self.file_io = file_io or LocalFileIO()
         self.opts = N.PgParquetWriteOptions(row_group_rows, page_rows)
         self.lib = N.load()
+        if compression.lower() not in PARQUET_CODECS:
+            raise ValueError(f"unknown file compression {compression!r}")
+        self.codec = PARQUET_CODECS[compression.lower()]
+        self.zstd_level = int(zstd_level)
 
     def write(self, source_handle: int, row0: int = 0, n_rows: int = -1) -> WrittenFile:
         names = file_column_names(self.schema)
         arr = (C.c_char_p * len(names))(*[n.encode() for n in names])
         fh = C.c_uint64(0)
-        N.check(self.lib.pg_parquet_encode(source_handle, arr, row0, n_rows, C.byref(self.opts), C.byref(fh)))
+        if self.codec == 0:
+            N.check(self.lib.pg_parquet_encode(source_handle, arr, row0, n_rows, C.byref(self.opts), C.byref(fh)))
+        else:
+            N.check(self.lib.pg_parquet_encode_compressed(source_handle, arr, row0, n_rows, C.byref(self.opts),
+                                                          self.codec, self.zstd_level, C.byref(fh)))
         try:
             meta = N.PgFileMeta()
             N.check(self.lib.pg_parquet_file_meta(fh.value, C.byref(meta)))
@@ -143,11 +183,13 @@ class CompactResult:
 
 class MergeTreeCompactRewriter:
     """rewriteCompaction(outputLevel, dropDelete, sections): every section is merged on the device, the merged
-    batch never leaves HBM before it is encoded (MergeTreeCompactRewriter.java:78-116)."""
+    batch never leaves HBM before it is encoded (MergeTreeCompactRewriter.java:78-116).  With `options` (table
+    options), the page codec of the files written at the output level is compression_for_level(options, level);
+    without, the files are uncompressed."""
 
     def __init__(self, schema: KeyValueSchema, mf_factory: MergeFunctionFactory, directory: str,
                  user_defined_seq_comparator=None, file_io: Optional[LocalFileIO] = None, device: int = 0,
-                 target_file_rows: int = 4 << 20, **writer_args):
+                 target_file_rows: int = 4 << 20, options: Optional[Dict[str, object]] = None, **writer_args):
         self.schema = schema
         self.mf_factory = mf_factory
         self.directory = directory
@@ -156,6 +198,7 @@ class MergeTreeCompactRewriter:
         self.file_io = file_io
         self.device = device
         self.target_file_rows = target_file_rows
+        self.options = options
         self.writer_args = writer_args
 
     def rewrite(self, output_level: int, drop_delete: bool, sections: Sequence[Sequence[SortedRun]]) -> CompactResult:
@@ -165,8 +208,11 @@ class MergeTreeCompactRewriter:
                            sections: Sequence[Sequence[SortedRun]]) -> CompactResult:
         result = CompactResult()
         spec = self.mf_factory.create().with_drop_delete(drop_delete)
+        writer_args = dict(self.writer_args)
+        if self.options is not None:
+            writer_args["compression"], writer_args["zstd_level"] = compression_for_level(self.options, output_level)
         rolling = RollingFileWriter(self.schema, self.directory, output_level, self.target_file_rows, self.file_io,
-                                    prefix=f"compact-l{output_level}", **self.writer_args)
+                                    prefix=f"compact-l{output_level}", **writer_args)
         for section in sections:
             for run in section:
                 result.before += run.files

@@ -12,7 +12,8 @@
 //       (TINYINT / SMALLINT / INT -> INT32 with INT_8 / INT_16 annotations, BIGINT -> INT64, STRING -> BYTE_ARRAY UTF8,
 //        nullable -> OPTIONAL (max definition level 1), NOT NULL -> REQUIRED)
 //
-// Layout written: PAR1 | per row group, per column: data pages V1, PLAIN, uncompressed | FileMetaData | len | PAR1.
+// Layout written: PAR1 | per row group, per column: data pages V1, PLAIN, uncompressed or one zstd frame per page
+// body (pg_parquet_encode_compressed) | FileMetaData | len | PAR1.
 // Pages start at multiples of 8 rows, so a nullable column's definition levels (bit width 1, bit-packed LSB first)
 // ARE the bytes of the Arrow validity bitmap: they are copied, not re-encoded.  Values of non-null rows are
 // compacted by a block-wide scan; BYTE_ARRAY values are written as [len:int32][bytes].
@@ -21,6 +22,7 @@
 
 #include "device_utils.cuh"
 #include "parquet_meta.h"
+#include "zstd_encode_device.cuh"
 
 namespace pg {
 
@@ -229,6 +231,65 @@ __global__ void k_pw_patch(const PatchJob *jobs, int n, const uint8_t *bytes, ui
     for (int i = lane; i < pj.len; i += 32) file[pj.dst + i] = bytes[pj.src + i];
 }
 
+// ------------------------------------------------------------------ zstd page compression
+// The page bodies are written into a scratch image, every 128 KiB block of every body is compressed by one warp, the
+// per-page frame sizes go back to the host (which lays out the file and writes the page headers), and a gather places
+// the frames at their file offsets.
+
+struct ZsBlockJob {
+    int64_t src;                  // offset of the block in the body image
+    int64_t out;                  // offset of its payload slot (n bytes)
+    int64_t seq;                  // first sequence slot (n / 4 + 1 of them)
+    int32_t n;                    // input bytes (<= 128 KiB)
+    int32_t page;
+};
+struct ZsPage {
+    int64_t raw;                  // body bytes
+    int32_t first_block, n_blocks;
+};
+
+constexpr size_t kZsSmem = (sizeof(int32_t) << zs::kHashLog) + sizeof(zs::EncWork);
+
+__global__ void __launch_bounds__(32)
+k_zs_block(const ZsBlockJob *jobs, const uint8_t *img, uint8_t *out, zs::Seq *seqs, uint8_t *lits, int2 *res) {
+    extern __shared__ __align__(16) uint8_t zs_smem[];
+    int32_t *htab = (int32_t *)zs_smem;
+    zs::EncWork &W = *(zs::EncWork *)(zs_smem + (sizeof(int32_t) << zs::kHashLog));
+    const ZsBlockJob j = jobs[blockIdx.x];
+    const zs::BlockOut r = zs::compress_block(img + j.src, j.n, out + j.out, htab, seqs + j.seq, lits + j.src, W);
+    if (threadIdx.x == 0) res[blockIdx.x] = make_int2(r.type, r.size);
+}
+
+// per page: where each block's header goes inside the frame, and the frame size
+__global__ void k_zs_page_sizes(const ZsPage *pages, int n_pages, const int2 *res, int32_t *boff, int64_t *frame_bytes) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= n_pages) return;
+    const ZsPage pg = pages[p];
+    int64_t off = zs::frame_header_size((uint64_t)pg.raw);
+    for (int b = 0; b < pg.n_blocks; b++) {
+        boff[pg.first_block + b] = (int32_t)off;
+        off += 3 + res[pg.first_block + b].y;
+    }
+    frame_bytes[p] = off;
+}
+
+// one CTA per block: frame header (first block of a page), block header, payload at the frame's file offset
+__global__ void k_zs_gather(const ZsBlockJob *jobs, const ZsPage *pages, const int2 *res, const int32_t *boff,
+                            const int64_t *frame_off, const uint8_t *img, const uint8_t *out, uint8_t *file) {
+    const ZsBlockJob j = jobs[blockIdx.x];
+    const ZsPage pg = pages[j.page];
+    const int2 r = res[blockIdx.x];
+    uint8_t *frame = file + frame_off[j.page];
+    uint8_t *dst = frame + boff[blockIdx.x];
+    if (threadIdx.x == 0) {
+        if ((int)blockIdx.x == pg.first_block) zs::write_frame_header(frame, (uint64_t)pg.raw);
+        zs::write_block_header(dst, (int)blockIdx.x == pg.first_block + pg.n_blocks - 1, r.x,
+                               r.x == 2 ? (uint32_t)r.y : (uint32_t)j.n);
+    }
+    const uint8_t *pay = r.x == 0 ? img + j.src : out + j.out;
+    for (int i = threadIdx.x; i < r.y; i += blockDim.x) dst[3 + i] = pay[i];
+}
+
 // ------------------------------------------------------------------ Thrift compact protocol writer
 
 struct ThriftWriter {
@@ -283,7 +344,7 @@ static int parquet_type_of(int t) {
 }
 
 static pg_status encode(uint64_t source, const char *const *names, int64_t row0, int64_t n_rows,
-                        const pg_parquet_write_options *opt, uint64_t *out_file) {
+                        const pg_parquet_write_options *opt, int codec, uint64_t *out_file) {
     pg_status st = ensure_device();
     if (st) return st;
     BatchColumns batch;                                      // held until the encode below is done
@@ -350,21 +411,21 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         PG_CUDA(cudaMemcpy(stats.data(), d_stats, sizeof(int64_t) * 4 * nsj, cudaMemcpyDeviceToHost));
     }
 
-    // ---- layout: page headers (Thrift), level prefixes, value regions
+    // ---- page bodies: level prefix (host-built) + values, per page
     auto ef = std::make_unique<EncodedFile>();
     ef->stats.assign(nc, ColStats{});
     for (int c = 0; c < nc; c++) { ef->stats[c].min = INT64_MAX; ef->stats[c].max = INT64_MIN; }
-    int64_t pos = 4;                                         // after "PAR1"
-    ef->host_parts.push_back({0, {'P', 'A', 'R', '1'}});
-    struct ChunkInfo { int64_t first_page, total_size, num_values, nn; ColStats st; };
+    struct ChunkInfo { int64_t first_page, total_uncompressed, total_compressed, num_values, nn; size_t page0, page1; ColStats st; };
+    struct PageInfo { std::vector<uint8_t> prefix; int64_t def_bytes, body, stored; };
     std::vector<ChunkInfo> chunks(nsj);
+    std::vector<PageInfo> pages;
+    pages.reserve(nj);
     size_t ji = 0;
-    int n_pages = 0;
     for (size_t sj = 0; sj < nsj; sj++) {
         const int c = sjobs[sj].col;
         const EncColumn &ec = cols[c];
         ChunkInfo &ci = chunks[sj];
-        ci.first_page = pos;
+        ci.page0 = ji;
         ci.num_values = sjobs[sj].n_rows;
         ci.nn = stats[4 * sj + 2];
         ci.st.null_count = ci.num_values - ci.nn;
@@ -405,10 +466,99 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
             else val_bytes = nn * (ec.width == 8 ? 8 : 4);
             const int64_t body = def_bytes + val_bytes;
             if (body > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet encode: page larger than 2 GiB");
+            pages.push_back(PageInfo{std::move(prefix), def_bytes, body, body});
+        }
+        ci.page1 = ji;
+    }
+    const int n_pages = (int)pages.size();
+
+    // ---- zstd: bodies into a scratch image, one frame per body; the frame sizes come back before the layout
+    int launches_zs = 0;
+    const bool zstd = codec == pq::C_ZSTD;
+    std::vector<ZsBlockJob> bjobs;
+    std::vector<ZsPage> zpages(zstd ? nj : 0);
+    uint8_t *d_img = nullptr, *d_zout = nullptr;
+    ZsBlockJob *d_bjobs = nullptr;
+    ZsPage *d_zpages = nullptr;
+    int2 *d_res = nullptr;
+    int32_t *d_boff = nullptr;
+    int64_t *d_frame = nullptr;
+    if (zstd && nj) {
+        std::vector<PatchJob> pjobs;
+        std::vector<uint8_t> pbytes;
+        int64_t img = 0, out = 0, seq = 0;
+        for (size_t p = 0; p < nj; p++) {
+            const PageInfo &pi = pages[p];
+            if (!pi.prefix.empty()) {
+                pjobs.push_back(PatchJob{img, (int32_t)pbytes.size(), (int32_t)pi.prefix.size()});
+                pbytes.insert(pbytes.end(), pi.prefix.begin(), pi.prefix.end());
+                jobs[p].def_off = img + (int64_t)pi.prefix.size();
+            }
+            jobs[p].val_off = img + pi.def_bytes;
+            zpages[p] = ZsPage{pi.body, (int32_t)bjobs.size(), 0};
+            for (int64_t b0 = 0; b0 == 0 || b0 < pi.body; b0 += zs::kMaxBlock) {
+                const int32_t n = (int32_t)std::min<int64_t>(zs::kMaxBlock, pi.body - b0);
+                bjobs.push_back(ZsBlockJob{img + b0, out, seq, n, (int32_t)p});
+                out += n;
+                seq += n / 4 + 1;
+                zpages[p].n_blocks++;
+            }
+            img += pi.body;
+        }
+        const size_t nb = bjobs.size();
+        d_img = (uint8_t *)scratch.take((size_t)img + 64);
+        d_zout = (uint8_t *)scratch.take((size_t)out + 64);
+        uint8_t *d_lits = (uint8_t *)scratch.take((size_t)img + 64);
+        zs::Seq *d_seqs = (zs::Seq *)scratch.take(sizeof(zs::Seq) * (size_t)seq);
+        d_bjobs = (ZsBlockJob *)scratch.take(sizeof(ZsBlockJob) * nb);
+        d_zpages = (ZsPage *)scratch.take(sizeof(ZsPage) * nj);
+        d_res = (int2 *)scratch.take(sizeof(int2) * nb);
+        d_boff = (int32_t *)scratch.take(sizeof(int32_t) * nb);
+        d_frame = (int64_t *)scratch.take(sizeof(int64_t) * nj);
+        PatchJob *d_pjobs = (PatchJob *)scratch.take(sizeof(PatchJob) * pjobs.size() + 16);
+        uint8_t *d_pbytes = (uint8_t *)scratch.take(pbytes.size() + 16);
+        if (!d_img || !d_zout || !d_lits || !d_seqs || !d_bjobs || !d_zpages || !d_res || !d_boff || !d_frame || !d_pjobs || !d_pbytes)
+            return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the zstd page images");
+        PG_CUDA(cudaMemsetAsync(d_img, 0, (size_t)img + 64, 0));
+        PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
+        PG_CUDA(cudaMemcpy(d_bjobs, bjobs.data(), sizeof(ZsBlockJob) * nb, cudaMemcpyHostToDevice));
+        PG_CUDA(cudaMemcpy(d_zpages, zpages.data(), sizeof(ZsPage) * nj, cudaMemcpyHostToDevice));
+        k_pw_encode<<<(unsigned)nj, 256>>>(d_cols, d_jobs, d_img);
+        launches_zs++;
+        if (!pjobs.empty()) {
+            PG_CUDA(cudaMemcpy(d_pjobs, pjobs.data(), sizeof(PatchJob) * pjobs.size(), cudaMemcpyHostToDevice));
+            PG_CUDA(cudaMemcpy(d_pbytes, pbytes.data(), pbytes.size(), cudaMemcpyHostToDevice));
+            k_pw_patch<<<(unsigned)((pjobs.size() * 32 + 127) / 128), 128>>>(d_pjobs, (int)pjobs.size(), d_pbytes, d_img);
+            launches_zs++;
+        }
+        k_zs_block<<<(unsigned)nb, 32, kZsSmem>>>(d_bjobs, d_img, d_zout, d_seqs, d_lits, d_res);
+        k_zs_page_sizes<<<(unsigned)((nj + 127) / 128), 128>>>(d_zpages, (int)nj, d_res, d_boff, d_frame);
+        launches_zs += 2;
+        std::vector<int64_t> frame_bytes(nj);
+        SmallReads rd(0);
+        if ((st = rd.add(frame_bytes.data(), d_frame, sizeof(int64_t) * nj))) return st;
+        launches_zs++;
+        if ((st = rd.finish())) return st;
+        cudaError_t le = cudaGetLastError();
+        if (le != cudaSuccess) return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(le));
+        for (size_t p = 0; p < nj; p++) pages[p].stored = frame_bytes[p];
+    }
+
+    // ---- layout: page headers (Thrift), level prefixes (uncompressed), stored bodies
+    int64_t pos = 4;                                         // after "PAR1"
+    ef->host_parts.push_back({0, {'P', 'A', 'R', '1'}});
+    std::vector<int64_t> frame_off(zstd ? nj : 0);
+    for (size_t sj = 0; sj < nsj; sj++) {
+        ChunkInfo &ci = chunks[sj];
+        ci.first_page = pos;
+        ci.total_uncompressed = ci.total_compressed = 0;
+        for (size_t p = ci.page0; p < ci.page1; p++) {
+            EncJob &j = jobs[p];
+            const PageInfo &pi = pages[p];
             ThriftWriter ph;                                   // PageHeader
             ph.i32(1, pq::P_DATA);
-            ph.i32(2, (int32_t)body);
-            ph.i32(3, (int32_t)body);
+            ph.i32(2, (int32_t)pi.body);
+            ph.i32(3, (int32_t)pi.stored);
             ph.struct_field(5);                                // DataPageHeader
             ph.i32(1, j.n_rows);
             ph.i32(2, pq::E_PLAIN);
@@ -418,15 +568,18 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
             ph.end();
             ef->host_parts.push_back({pos, ph.b});
             pos += (int64_t)ph.b.size();
-            if (!prefix.empty()) {
-                ef->host_parts.push_back({pos, prefix});
-                j.def_off = pos + (int64_t)prefix.size();
+            if (zstd) frame_off[p] = pos;
+            else {
+                if (!pi.prefix.empty()) {
+                    ef->host_parts.push_back({pos, pi.prefix});
+                    j.def_off = pos + (int64_t)pi.prefix.size();
+                }
+                j.val_off = pos + pi.def_bytes;
             }
-            j.val_off = pos + def_bytes;
-            pos += body;
-            n_pages++;
+            pos += pi.stored;
+            ci.total_uncompressed += (int64_t)ph.b.size() + pi.body;
+            ci.total_compressed += (int64_t)ph.b.size() + pi.stored;
         }
-        ci.total_size = pos - ci.first_page;
     }
     const int64_t data_end = pos;
 
@@ -458,7 +611,7 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         for (int c = 0; c < nc; c++) {
             const ChunkInfo &ci = chunks[(size_t)g * nc + c];
             const EncColumn &ec = cols[c];
-            group_bytes += ci.total_size;
+            group_bytes += ci.total_uncompressed;
             fw.struct_elem();                                  // ColumnChunk
             fw.i64(2, ci.first_page);
             fw.struct_field(3);                                // ColumnMetaData
@@ -466,10 +619,10 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
             fw.list(2, 5, 2); fw.zigzag(pq::E_PLAIN); fw.zigzag(pq::E_RLE);
             fw.list(3, 8, 1);
             { std::string nm = names && names[c] ? names[c] : ("c" + std::to_string(c)); fw.varint(nm.size()); fw.b.insert(fw.b.end(), nm.begin(), nm.end()); }
-            fw.i32(4, pq::C_UNCOMPRESSED);
+            fw.i32(4, zstd ? pq::C_ZSTD : pq::C_UNCOMPRESSED);
             fw.i64(5, ci.num_values);
-            fw.i64(6, ci.total_size);
-            fw.i64(7, ci.total_size);
+            fw.i64(6, ci.total_uncompressed);
+            fw.i64(7, ci.total_compressed);
             fw.i64(9, ci.first_page);
             fw.struct_field(12);                               // Statistics
             fw.i64(3, ci.st.null_count);
@@ -506,7 +659,12 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     // ---- page bodies on the device
     PG_CUDA(cudaMalloc(&ef->d_file, (size_t)ef->file_bytes + 64));
     PG_CUDA(cudaMemsetAsync(ef->d_file, 0, (size_t)ef->file_bytes + 64, 0));
-    if (nj) {
+    if (nj && zstd) {
+        // (the frame sizes have been read: their buffer takes the frame offsets)
+        PG_CUDA(cudaMemcpy(d_frame, frame_off.data(), sizeof(int64_t) * nj, cudaMemcpyHostToDevice));
+        k_zs_gather<<<(unsigned)bjobs.size(), 256>>>(d_bjobs, d_zpages, d_res, d_boff, d_frame, d_img, d_zout, ef->d_file);
+        launches += launches_zs + 1;
+    } else if (nj) {
         PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
         k_pw_encode<<<(unsigned)nj, 256>>>(d_cols, d_jobs, ef->d_file);
         launches++;
@@ -540,7 +698,22 @@ extern "C" {
 pg_status pg_parquet_encode(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
                             const pg_parquet_write_options *options, uint64_t *out_file) {
     if (!out_file) return fail(PG_ERR_INVALID, "null argument");
-    return encode(source, column_names, row0, n_rows, options, out_file);
+    return encode(source, column_names, row0, n_rows, options, pq::C_UNCOMPRESSED, out_file);
+}
+
+pg_status pg_parquet_encode_compressed(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
+                                       const pg_parquet_write_options *options, int32_t codec, int32_t level,
+                                       uint64_t *out_file) {
+    if (!out_file) return fail(PG_ERR_INVALID, "null argument");
+    if (codec < pq::C_UNCOMPRESSED || codec > pq::C_LZ4_RAW)
+        return fail(PG_ERR_INVALID, "parquet encode: codec " + std::to_string(codec) + " is not a Parquet CompressionCodec");
+    if (codec != pq::C_UNCOMPRESSED && codec != pq::C_ZSTD)
+        return fail(PG_ERR_UNSUPPORTED, "parquet encode: codec " + std::to_string(codec) +
+                                            " is not written on the device (UNCOMPRESSED and ZSTD are)");
+    if (codec == pq::C_ZSTD && (level == 0 || level > 1))
+        return fail(PG_ERR_UNSUPPORTED, "parquet encode: file.compression.zstd-level " + std::to_string(level) +
+                                            " is not written on the device (level 1 and the negative fast levels are)");
+    return encode(source, column_names, row0, n_rows, options, codec, out_file);
 }
 
 pg_status pg_parquet_file_meta(uint64_t file, pg_file_meta *out) {

@@ -28,6 +28,15 @@ namespace zs {
 
 constexpr int kMaxBlock = 128 * 1024;
 constexpr int kLLLog = 9, kOFLog = 8, kMLLog = 9, kHufLog = 11;
+constexpr int kLLDefLog = 6, kOFDefLog = 5, kMLDefLog = 6;
+
+// predefined distributions of the sequence codes (RFC 8878 §3.1.1.3.2.2), as initialisers of local arrays so that the
+// decoder and the encoder (zstd_encode_device.cuh) read the same numbers on the host and on the device
+#define ZS_LL_DEFAULT_NORM {4, 3, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 1, 1, 1, 2, 2, 2, 2, 2, 2, 2, 2, 2, 3, 2, 1, 1, 1, 1, 1, \
+                            -1, -1, -1, -1}
+#define ZS_ML_DEFAULT_NORM {1, 4, 3, 2, 2, 2, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, \
+                            1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1, -1, -1}
+#define ZS_OF_DEFAULT_NORM {1, 1, 1, 1, 1, 1, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1}
 
 struct FseEntry { uint16_t base; uint8_t sym; uint8_t nbits; };
 struct HufEntry { uint8_t sym; uint8_t nbits; };
@@ -511,10 +520,9 @@ ZS_HD inline int64_t decode_block(const uint8_t *p, int len, uint8_t *out, const
         const int modes = q[0];
         if (modes & 3) return -1;
         q++; left--;
-        const int8_t ll_def[36] = {4, 3, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 2, 1, 1, 1, 2, 2, 2, 2, 2, 2, 2, 2, 2, 3, 2, 1, 1, 1, 1, 1, -1, -1, -1, -1};
-        const int8_t ml_def[53] = {1, 4, 3, 2, 2, 2, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1,
-                                   1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1, -1, -1};
-        const int8_t of_def[29] = {1, 1, 1, 1, 1, 1, 2, 2, 2, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, 1, -1, -1, -1, -1, -1};
+        const int8_t ll_def[36] = ZS_LL_DEFAULT_NORM;
+        const int8_t ml_def[53] = ZS_ML_DEFAULT_NORM;
+        const int8_t of_def[29] = ZS_OF_DEFAULT_NORM;
         int u = 0;
         if (lane_id() == 0) u = read_seq_table((modes >> 6) & 3, q, left, kLLLog, 35, ll_def, 36, 6, T.ll, &T.ll_log, &T.have_ll, T);
         u = bcast0(u);

@@ -149,9 +149,11 @@ k_pw_encode(const EncColumn *cols, const EncJob *jobs, uint8_t *file) {
 }
 
 // per column chunk (one CTA): min / max of the non-null values of a fixed-width numeric column, as int64 / double
-// bit patterns; also used for the sequence number range and the delete count (kind column)
+// bit patterns (FLOAT / DOUBLE: of the non-NaN values, whichever zero comes first; the host applies the zero rule),
+// whether a non-null value is NaN; also used for the sequence number range and the delete count (kind column)
 struct StatJob { int32_t col; int32_t pad; int64_t row0; int64_t n_rows; };
-__global__ void k_pw_stats(const EncColumn *cols, const StatJob *jobs, int64_t *out /* [job][4]: min, max, nn, retracts */) {
+constexpr int kStatWords = 5;     // per job: min, max, non-null rows, retracts, NaN seen
+__global__ void k_pw_stats(const EncColumn *cols, const StatJob *jobs, int64_t *out /* [job][kStatWords] */) {
     const StatJob j = jobs[blockIdx.x];
     const EncColumn c = cols[j.col];
     const bool fp = c.type == PG_FLOAT || c.type == PG_DOUBLE;
@@ -212,13 +214,12 @@ __global__ void k_pw_stats(const EncColumn *cols, const StatJob *jobs, int64_t *
     atomicAdd((unsigned long long *)&s_n[1], (unsigned long long)retr);
     __syncthreads();
     if (threadIdx.x == 0) {
-        int64_t *o = out + 4 * (int64_t)blockIdx.x;
-        if (fp) {
-            o[0] = s_nan ? INT64_MAX : __double_as_longlong(s_d[0]);     // NaN present: no usable min / max
-            o[1] = s_nan ? INT64_MIN : __double_as_longlong(s_d[1]);
-        } else { o[0] = s_i[0]; o[1] = s_i[1]; }
+        int64_t *o = out + kStatWords * (int64_t)blockIdx.x;
+        if (fp) { o[0] = __double_as_longlong(s_d[0]); o[1] = __double_as_longlong(s_d[1]); }
+        else { o[0] = s_i[0]; o[1] = s_i[1]; }
         o[2] = s_n[0];
         o[3] = s_n[1];
+        o[4] = s_nan;
     }
 }
 
@@ -321,6 +322,14 @@ struct ThriftWriter {
 
 struct ColStats { int64_t min = 0, max = 0, null_count = 0; int has_minmax = 0; };
 
+// the bits of a FLOAT / DOUBLE bound (held as a double), a zero of either sign replaced by `zero`
+static int64_t zero_as(int64_t bits, double zero) {
+    double x;
+    memcpy(&x, &bits, 8);
+    if (x == 0) memcpy(&bits, &zero, 8);
+    return bits;
+}
+
 struct EncodedFile {
     unsigned char *d_file = nullptr;         // device image of the file (page bodies at their final offsets)
     int64_t file_bytes = 0;
@@ -390,13 +399,13 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         }
     }
     const size_t nj = jobs.size(), nsj = sjobs.size();
-    std::vector<int64_t> counts(2 * nj + 2), stats(4 * nsj + 4);
+    std::vector<int64_t> counts(2 * nj + 2), stats(kStatWords * (nsj + 1));
     Scratch scratch(0);                                      // temporaries, released on every path out of this function
     EncColumn *d_cols = (EncColumn *)scratch.take(sizeof(EncColumn) * nc);
     EncJob *d_jobs = (EncJob *)scratch.take(sizeof(EncJob) * std::max<size_t>(nj, 1));
     StatJob *d_sjobs = (StatJob *)scratch.take(sizeof(StatJob) * std::max<size_t>(nsj, 1));
     int64_t *d_counts = (int64_t *)scratch.take(sizeof(int64_t) * (2 * nj + 2));
-    int64_t *d_stats = (int64_t *)scratch.take(sizeof(int64_t) * (4 * nsj + 4));
+    int64_t *d_stats = (int64_t *)scratch.take(sizeof(int64_t) * kStatWords * (nsj + 1));
     if (!d_cols || !d_jobs || !d_sjobs || !d_counts || !d_stats)
         return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the page tables");
     PG_CUDA(cudaMemcpy(d_cols, cols.data(), sizeof(EncColumn) * nc, cudaMemcpyHostToDevice));
@@ -408,7 +417,7 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         k_pw_stats<<<(unsigned)nsj, 256>>>(d_cols, d_sjobs, d_stats);
         launches += 2;
         PG_CUDA(cudaMemcpy(counts.data(), d_counts, sizeof(int64_t) * 2 * nj, cudaMemcpyDeviceToHost));
-        PG_CUDA(cudaMemcpy(stats.data(), d_stats, sizeof(int64_t) * 4 * nsj, cudaMemcpyDeviceToHost));
+        PG_CUDA(cudaMemcpy(stats.data(), d_stats, sizeof(int64_t) * kStatWords * nsj, cudaMemcpyDeviceToHost));
     }
 
     // ---- page bodies: level prefix (host-built) + values, per page
@@ -420,22 +429,29 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     std::vector<ChunkInfo> chunks(nsj);
     std::vector<PageInfo> pages;
     pages.reserve(nj);
+    std::vector<char> file_nan(nc, 0);                       // per column: a chunk holds a NaN
     size_t ji = 0;
     for (size_t sj = 0; sj < nsj; sj++) {
         const int c = sjobs[sj].col;
         const EncColumn &ec = cols[c];
+        const int64_t *cs = &stats[kStatWords * sj];
+        const bool fp = ec.type == PG_FLOAT || ec.type == PG_DOUBLE, nan = cs[4] != 0;
         ChunkInfo &ci = chunks[sj];
         ci.page0 = ji;
         ci.num_values = sjobs[sj].n_rows;
-        ci.nn = stats[4 * sj + 2];
+        ci.nn = cs[2];
         ci.st.null_count = ci.num_values - ci.nn;
-        ci.st.has_minmax = ec.width > 0 && ci.nn > 0 && !(stats[4 * sj] == INT64_MAX && stats[4 * sj + 1] == INT64_MIN);
-        ci.st.min = stats[4 * sj];
-        ci.st.max = stats[4 * sj + 1];
+        ci.st.has_minmax = ec.width > 0 && ci.nn > 0 && !nan;   // a chunk with a NaN has no min / max
+        ci.st.min = cs[0];
+        ci.st.max = cs[1];
+        // parquet.thrift, Statistics: a zero min of a floating point column is written as -0.0, a zero max as +0.0,
+        // so that min <= v <= max holds for both zeros in the order readers compare with (Double.compare: -0.0 <
+        // +0.0).  The file-level merge below keeps the rule: the zero min it can take is -0.0, the zero max +0.0.
+        if (fp && ci.st.has_minmax) { ci.st.min = zero_as(ci.st.min, -0.0); ci.st.max = zero_as(ci.st.max, 0.0); }
+        file_nan[c] |= nan;
         ColStats &fs = ef->stats[c];
         fs.null_count += ci.st.null_count;
         if (ci.st.has_minmax) {
-            const bool fp = ec.type == PG_FLOAT || ec.type == PG_DOUBLE;
             if (!fs.has_minmax) { fs.min = ci.st.min; fs.max = ci.st.max; fs.has_minmax = 1; }
             else if (fp) {
                 double a, b, x, y;
@@ -444,7 +460,7 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
                 memcpy(&fs.min, &a, 8); memcpy(&fs.max, &b, 8);
             } else { fs.min = std::min(fs.min, ci.st.min); fs.max = std::max(fs.max, ci.st.max); }
         }
-        if (c == s->n_key + 1) ef->meta.delete_row_count += stats[4 * sj + 3];
+        if (c == s->n_key + 1) ef->meta.delete_row_count += cs[3];
         for (; ji < nj && jobs[ji].col == c && jobs[ji].row0 >= sjobs[sj].row0 &&
                jobs[ji].row0 < sjobs[sj].row0 + sjobs[sj].n_rows; ji++) {
             EncJob &j = jobs[ji];
@@ -470,6 +486,10 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         }
         ci.page1 = ji;
     }
+    // A file with a NaN in a FLOAT / DOUBLE column has no min / max for that column, though its other chunks have
+    // some: NaN sorts above every value (Double.compare), so a max taken around it would prune rows `x > max` matches.
+    for (int c = 0; c < nc; c++)
+        if (file_nan[c]) ef->stats[c] = ColStats{INT64_MAX, INT64_MIN, ef->stats[c].null_count, 0};
     const int n_pages = (int)pages.size();
 
     // ---- zstd: bodies into a scratch image, one frame per body; the frame sizes come back before the layout
@@ -649,6 +669,15 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         fw.end();
     }
     fw.str(6, "paimon-b200 (libpaimon_gpu)");
+    // column_orders: TYPE_ORDER (TypeDefinedOrder) for every column.  Readers take min_value / max_value only from a
+    // file that declares the order they were computed in; without it parquet-cpp (pyarrow) ignores them.
+    fw.list(7, 12, (size_t)nc);
+    for (int c = 0; c < nc; c++) {
+        fw.struct_elem();                                      // ColumnOrder (union)
+        fw.struct_field(1);                                    // TYPE_ORDER: TypeDefinedOrder, no fields
+        fw.end();
+        fw.end();
+    }
     fw.end();
     std::vector<uint8_t> tail = fw.b;
     const uint32_t flen = (uint32_t)fw.b.size();

@@ -291,33 +291,6 @@ __global__ void k_zs_gather(const ZsBlockJob *jobs, const ZsPage *pages, const i
     for (int i = threadIdx.x; i < r.y; i += blockDim.x) dst[3 + i] = pay[i];
 }
 
-// ------------------------------------------------------------------ Thrift compact protocol writer
-
-struct ThriftWriter {
-    std::vector<uint8_t> b;
-    std::vector<int> last{0};
-    void varint(uint64_t v) { while (v >= 0x80) { b.push_back((uint8_t)(v | 0x80)); v >>= 7; } b.push_back((uint8_t)v); }
-    void zigzag(int64_t v) { varint(((uint64_t)v << 1) ^ (uint64_t)(v >> 63)); }
-    void field(int id, int type) {
-        int d = id - last.back();
-        if (d > 0 && d <= 15) b.push_back((uint8_t)((d << 4) | type));
-        else { b.push_back((uint8_t)type); zigzag(id); }
-        last.back() = id;
-    }
-    void i32(int id, int32_t v) { field(id, 5); zigzag(v); }
-    void i64(int id, int64_t v) { field(id, 6); zigzag(v); }
-    void bin(int id, const void *p, size_t n) { field(id, 8); varint(n); b.insert(b.end(), (const uint8_t *)p, (const uint8_t *)p + n); }
-    void str(int id, const std::string &s) { bin(id, s.data(), s.size()); }
-    void list(int id, int elem_type, size_t n) {
-        field(id, 9);
-        if (n < 15) b.push_back((uint8_t)((n << 4) | elem_type));
-        else { b.push_back((uint8_t)(0xF0 | elem_type)); varint(n); }
-    }
-    void struct_field(int id) { field(id, 12); last.push_back(0); }
-    void struct_elem() { last.push_back(0); }           // list element
-    void end() { b.push_back(0); last.pop_back(); }
-};
-
 // ------------------------------------------------------------------ host orchestration
 
 struct ColStats { int64_t min = 0, max = 0, null_count = 0; int has_minmax = 0; };
@@ -330,10 +303,13 @@ static int64_t zero_as(int64_t bits, double zero) {
     return bits;
 }
 
+using Part = std::pair<int64_t, std::vector<uint8_t>>;  // a host-built piece of the file: (offset, bytes)
+
 struct EncodedFile {
     unsigned char *d_file = nullptr;         // device image of the file (page bodies at their final offsets)
     int64_t file_bytes = 0;
-    std::vector<std::pair<int64_t, std::vector<uint8_t>>> host_parts;   // (offset, bytes): headers, level prefixes, footer
+    int64_t data_end = 0;                    // end of the page data, where the footer starts
+    std::vector<Part> host_parts;            // headers, level prefixes, footer
     pg_file_meta meta{};
     std::vector<ColStats> stats;             // whole-file, per column
     bool image_complete = false;             // host_parts have been patched into d_file
@@ -350,6 +326,256 @@ static int parquet_type_of(int t) {
         case PG_DOUBLE: return pq::T_DOUBLE;
         default: return pq::T_BYTE_ARRAY;
     }
+}
+
+// The column chunks and data pages of a file, built in one pass over (row group, column, page).  jobs[p] and
+// sjobs[k] are what the kernels read for pages[p] and chunks[k], in arrays that go to the device as they are.
+struct Page {
+    std::vector<uint8_t> prefix;  // RLE-hybrid definition levels: [length:int32][run header varint]; empty = REQUIRED
+    int64_t def_bytes = 0;        // prefix and level bytes
+    int64_t body = 0;             // page body bytes
+    int64_t stored = 0;           // bytes in the file: the body, or its zstd frame
+};
+struct Chunk {
+    size_t page0, page1;          // its pages
+    ColStats st;                  // the footer's Statistics
+    int64_t first_page = 0, total_uncompressed = 0, total_compressed = 0;
+};
+struct Plan {
+    int64_t n_groups = 0;
+    std::vector<EncColumn> cols;
+    std::vector<EncJob> jobs;
+    std::vector<Page> pages;
+    std::vector<StatJob> sjobs;
+    std::vector<Chunk> chunks;    // row group major, then column
+};
+
+static Plan make_plan(const Schema &s, const std::vector<DevColumn> &dcols, int64_t row0, int64_t n_rows,
+                      const pg_parquet_write_options *opt) {
+    Plan pl;
+    int64_t page_rows = opt && opt->page_rows > 0 ? opt->page_rows : 32768;
+    page_rows = (page_rows + 7) & ~(int64_t)7;
+    int64_t group_rows = opt && opt->row_group_rows > 0 ? opt->row_group_rows : (int64_t)1 << 20;
+    group_rows = ((group_rows + page_rows - 1) / page_rows) * page_rows;
+    pl.n_groups = n_rows == 0 ? 0 : (n_rows + group_rows - 1) / group_rows;
+    const int nc = s.n_cols();
+    for (int c = 0; c < nc; c++) {
+        pg_field f = s.field(c);
+        pl.cols.push_back(EncColumn{dcols[c].data, dcols[c].offsets, dcols[c].validity, f.type, type_width(f.type),
+                                    (f.nullable || dcols[c].validity) ? 1 : 0, 0});
+    }
+    for (int64_t g = 0; g < pl.n_groups; g++) {
+        const int64_t g0 = row0 + g * group_rows, g1 = std::min(row0 + n_rows, g0 + group_rows);
+        for (int c = 0; c < nc; c++) {
+            pl.sjobs.push_back(StatJob{c, 0, g0, g1 - g0});
+            const size_t page0 = pl.jobs.size();
+            for (int64_t p0 = g0; p0 < g1; p0 += page_rows)
+                pl.jobs.push_back(EncJob{c, (int32_t)(std::min(g1, p0 + page_rows) - p0), p0, -1, 0});
+            pl.chunks.push_back(Chunk{page0, pl.jobs.size(), ColStats{}});
+        }
+    }
+    pl.pages.resize(pl.jobs.size());
+    return pl;
+}
+
+// The device's counts -> each page's level prefix and body size, each chunk's statistics, the file's statistics of
+// each column, and the count of retract rows in column `kind_col`.  counts: per page, non-null rows and payload
+// bytes (k_pw_count); stats: per chunk, kStatWords (k_pw_stats).
+static pg_status fold_counts(Plan &pl, const int64_t *counts, const int64_t *stats, int kind_col,
+                             std::vector<ColStats> &file, int64_t &deletes) {
+    const int nc = (int)pl.cols.size();
+    file.assign(nc, ColStats{INT64_MAX, INT64_MIN, 0, 0});
+    std::vector<char> file_nan(nc, 0);                       // per column: a chunk holds a NaN
+    for (size_t k = 0; k < pl.chunks.size(); k++) {
+        const int c = pl.sjobs[k].col;
+        const EncColumn &ec = pl.cols[c];
+        const int64_t *cs = &stats[kStatWords * k];
+        const bool fp = ec.type == PG_FLOAT || ec.type == PG_DOUBLE, nan = cs[4] != 0;
+        Chunk &ch = pl.chunks[k];
+        ch.st.null_count = pl.sjobs[k].n_rows - cs[2];
+        ch.st.has_minmax = ec.width > 0 && cs[2] > 0 && !nan;   // a chunk with a NaN has no min / max
+        ch.st.min = cs[0];
+        ch.st.max = cs[1];
+        // parquet.thrift, Statistics: a zero min of a floating point column is written as -0.0, a zero max as +0.0,
+        // so that min <= v <= max holds for both zeros in the order readers compare with (Double.compare: -0.0 <
+        // +0.0).  The file-level merge below keeps the rule: the zero min it can take is -0.0, the zero max +0.0.
+        if (fp && ch.st.has_minmax) { ch.st.min = zero_as(ch.st.min, -0.0); ch.st.max = zero_as(ch.st.max, 0.0); }
+        file_nan[c] |= nan;
+        ColStats &fs = file[c];
+        fs.null_count += ch.st.null_count;
+        if (ch.st.has_minmax) {
+            if (!fs.has_minmax) { fs.min = ch.st.min; fs.max = ch.st.max; fs.has_minmax = 1; }
+            else if (fp) {
+                double a, b, x, y;
+                memcpy(&a, &fs.min, 8); memcpy(&b, &fs.max, 8); memcpy(&x, &ch.st.min, 8); memcpy(&y, &ch.st.max, 8);
+                a = std::min(a, x); b = std::max(b, y);
+                memcpy(&fs.min, &a, 8); memcpy(&fs.max, &b, 8);
+            } else { fs.min = std::min(fs.min, ch.st.min); fs.max = std::max(fs.max, ch.st.max); }
+        }
+        if (c == kind_col) deletes += cs[3];
+        for (size_t p = ch.page0; p < ch.page1; p++) {
+            Page &pg = pl.pages[p];
+            const int64_t nn = counts[2 * p], vb = counts[2 * p + 1];
+            if (ec.optional) {                                 // one bit-packed run of bit width 1
+                const int64_t groups = (pl.jobs[p].n_rows + 7) / 8;
+                std::vector<uint8_t> run;
+                pq::put_varint(run, (uint64_t)(groups << 1) | 1);
+                const uint32_t len = (uint32_t)(run.size() + groups);
+                pg.prefix = {(uint8_t)len, (uint8_t)(len >> 8), (uint8_t)(len >> 16), (uint8_t)(len >> 24)};
+                pg.prefix.insert(pg.prefix.end(), run.begin(), run.end());
+                pg.def_bytes = (int64_t)pg.prefix.size() + groups;
+            }
+            int64_t val_bytes;
+            if (ec.width == 0) val_bytes = 4 * nn + vb;
+            else if (ec.type == PG_BOOL) val_bytes = (nn + 7) / 8;
+            else val_bytes = nn * (ec.width == 8 ? 8 : 4);
+            pg.body = pg.stored = pg.def_bytes + val_bytes;
+            if (pg.body > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet encode: page larger than 2 GiB");
+        }
+    }
+    // A file with a NaN in a FLOAT / DOUBLE column has no min / max for that column, though its other chunks have
+    // some: NaN sorts above every value (Double.compare), so a max taken around it would prune rows `x > max` matches.
+    for (int c = 0; c < nc; c++)
+        if (file_nan[c]) file[c] = ColStats{INT64_MAX, INT64_MIN, file[c].null_count, 0};
+    return PG_OK;
+}
+
+// Places the body of page p at base[p]: its level prefix, the definition-level bytes behind it, the values behind
+// those.  Sets the jobs' def_off / val_off and returns the prefixes, which the caller puts in place.
+static std::vector<Part> place_bodies(Plan &pl, const std::vector<int64_t> &base) {
+    std::vector<Part> prefixes;
+    for (size_t p = 0; p < pl.pages.size(); p++) {
+        const Page &pg = pl.pages[p];
+        if (!pg.prefix.empty()) {
+            prefixes.push_back({base[p], pg.prefix});
+            pl.jobs[p].def_off = base[p] + (int64_t)pg.prefix.size();
+        }
+        pl.jobs[p].val_off = base[p] + pg.def_bytes;
+    }
+    return prefixes;
+}
+
+// Copies host-built parts into the device image `dst` with one k_pw_patch launch, none when there are no parts.  The
+// staging buffers come from `scratch`; `what` names them when the device is out of memory.
+static pg_status patch(Scratch &scratch, const std::vector<Part> &parts, uint8_t *dst, const char *what) {
+    if (parts.empty()) return PG_OK;
+    std::vector<PatchJob> jobs;
+    std::vector<uint8_t> bytes;
+    for (const Part &p : parts) {
+        if (bytes.size() + p.second.size() > 0x7fffffffull) return fail(PG_ERR_UNSUPPORTED, "parquet encode: too many header bytes");
+        jobs.push_back(PatchJob{p.first, (int32_t)bytes.size(), (int32_t)p.second.size()});
+        bytes.insert(bytes.end(), p.second.begin(), p.second.end());
+    }
+    PatchJob *d_jobs = (PatchJob *)scratch.take(sizeof(PatchJob) * jobs.size() + 16);
+    uint8_t *d_bytes = (uint8_t *)scratch.take(bytes.size() + 16);
+    if (!d_jobs || !d_bytes) return fail(PG_ERR_CUDA, std::string("parquet encode: out of device memory for ") + what);
+    PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(PatchJob) * jobs.size(), cudaMemcpyHostToDevice));
+    PG_CUDA(cudaMemcpy(d_bytes, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
+    k_pw_patch<<<(unsigned)((jobs.size() * 32 + 127) / 128), 128>>>(d_jobs, (int)jobs.size(), d_bytes, dst);
+    return PG_OK;
+}
+
+// PageHeader of a data page V1: PLAIN values, RLE levels
+static std::vector<uint8_t> page_header(const Page &pg, int32_t n_rows) {
+    pq::ThriftWriter w;
+    w.i32(1, pq::P_DATA);
+    w.i32(2, (int32_t)pg.body);
+    w.i32(3, (int32_t)pg.stored);
+    w.struct_field(5);                                         // DataPageHeader
+    w.i32(1, n_rows);
+    w.i32(2, pq::E_PLAIN);
+    w.i32(3, pq::E_RLE);
+    w.i32(4, pq::E_RLE);
+    w.end();
+    w.end();
+    return std::move(w.b);
+}
+
+// Statistics max_value / min_value: a chunk's bounds, PLAIN-encoded in the column's physical type
+static void write_min_max(pq::ThriftWriter &w, const EncColumn &ec, const ColStats &st) {
+    uint8_t mn[8], mx[8];
+    size_t n = ec.width == 8 ? 8 : 4;
+    if (ec.type == PG_FLOAT) {
+        double a, b; memcpy(&a, &st.min, 8); memcpy(&b, &st.max, 8);
+        float fa = (float)a, fb = (float)b; memcpy(mn, &fa, 4); memcpy(mx, &fb, 4);
+    } else if (ec.type == PG_BOOL) {
+        n = 1; mn[0] = (uint8_t)st.min; mx[0] = (uint8_t)st.max;
+    } else if (n == 4) {
+        int32_t a = (int32_t)st.min, b = (int32_t)st.max; memcpy(mn, &a, 4); memcpy(mx, &b, 4);
+    } else { memcpy(mn, &st.min, 8); memcpy(mx, &st.max, 8); }
+    w.bin(5, mx, n);
+    w.bin(6, mn, n);
+}
+
+// FileMetaData, its length and "PAR1": the end of the file
+static std::vector<uint8_t> footer(const Plan &pl, const char *const *names, int64_t n_rows, bool zstd) {
+    const int nc = (int)pl.cols.size();
+    std::vector<std::string> col_names(nc);
+    for (int c = 0; c < nc; c++) col_names[c] = names && names[c] ? names[c] : "c" + std::to_string(c);
+    pq::ThriftWriter w;
+    w.i32(1, 1);                                               // version
+    w.list(2, pq::CT_STRUCT, (size_t)nc + 1);                  // schema
+    w.struct_elem();
+    w.str(4, "paimon_schema");
+    w.i32(5, nc);
+    w.end();
+    for (int c = 0; c < nc; c++) {
+        const EncColumn &ec = pl.cols[c];
+        w.struct_elem();
+        w.i32(1, parquet_type_of(ec.type));
+        w.i32(3, ec.optional ? pq::R_OPTIONAL : pq::R_REQUIRED);
+        w.str(4, col_names[c]);
+        if (ec.type == PG_STRING) w.i32(6, 0);                 // UTF8
+        else if (ec.type == PG_INT8) w.i32(6, 15);             // INT_8
+        else if (ec.type == PG_INT16) w.i32(6, 16);            // INT_16
+        w.end();
+    }
+    w.i64(3, n_rows);
+    w.list(4, pq::CT_STRUCT, (size_t)pl.n_groups);
+    for (int64_t g = 0; g < pl.n_groups; g++) {
+        w.struct_elem();                                       // RowGroup
+        w.list(1, pq::CT_STRUCT, (size_t)nc);
+        int64_t group_bytes = 0;
+        for (int c = 0; c < nc; c++) {
+            const size_t k = (size_t)g * nc + c;
+            const Chunk &ch = pl.chunks[k];
+            group_bytes += ch.total_uncompressed;
+            w.struct_elem();                                   // ColumnChunk
+            w.i64(2, ch.first_page);
+            w.struct_field(3);                                 // ColumnMetaData
+            w.i32(1, parquet_type_of(pl.cols[c].type));
+            w.list(2, pq::CT_I32, 2); w.zigzag(pq::E_PLAIN); w.zigzag(pq::E_RLE);
+            w.list(3, pq::CT_BINARY, 1); w.binary(col_names[c].data(), col_names[c].size());
+            w.i32(4, zstd ? pq::C_ZSTD : pq::C_UNCOMPRESSED);
+            w.i64(5, pl.sjobs[k].n_rows);
+            w.i64(6, ch.total_uncompressed);
+            w.i64(7, ch.total_compressed);
+            w.i64(9, ch.first_page);
+            w.struct_field(12);                                // Statistics
+            w.i64(3, ch.st.null_count);
+            if (ch.st.has_minmax) write_min_max(w, pl.cols[c], ch.st);
+            w.end();
+            w.end();                                           // ColumnMetaData
+            w.end();                                           // ColumnChunk
+        }
+        w.i64(2, group_bytes);
+        w.i64(3, pl.sjobs[(size_t)g * nc].n_rows);             // the rows of the group: those of any of its chunks
+        w.end();
+    }
+    w.str(6, "paimon-b200 (libpaimon_gpu)");
+    // column_orders: TYPE_ORDER (TypeDefinedOrder) for every column.  Readers take min_value / max_value only from a
+    // file that declares the order they were computed in; without it parquet-cpp (pyarrow) ignores them.
+    w.list(7, pq::CT_STRUCT, (size_t)nc);
+    for (int c = 0; c < nc; c++) {
+        w.struct_elem();                                       // ColumnOrder (union)
+        w.struct_field(1);                                     // TYPE_ORDER: TypeDefinedOrder, no fields
+        w.end();
+        w.end();
+    }
+    w.end();
+    const uint32_t flen = (uint32_t)w.b.size();
+    w.b.insert(w.b.end(), {(uint8_t)flen, (uint8_t)(flen >> 8), (uint8_t)(flen >> 16), (uint8_t)(flen >> 24), 'P', 'A', 'R', '1'});
+    return std::move(w.b);
 }
 
 static pg_status encode(uint64_t source, const char *const *names, int64_t row0, int64_t n_rows,
@@ -369,36 +595,14 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     if (row0 < 0 || (row0 & 7) || row0 + n_rows > batch.n_rows)
         return fail(PG_ERR_INVALID, "parquet encode: row range outside the batch or not starting at a multiple of 8");
     const int nc = s->n_cols();
-    int64_t page_rows = opt && opt->page_rows > 0 ? opt->page_rows : 32768;
-    page_rows = (page_rows + 7) & ~(int64_t)7;
-    int64_t group_rows = opt && opt->row_group_rows > 0 ? opt->row_group_rows : (int64_t)1 << 20;
-    group_rows = ((group_rows + page_rows - 1) / page_rows) * page_rows;
-    const int64_t n_groups = n_rows == 0 ? 0 : (n_rows + group_rows - 1) / group_rows;
 
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    struct EvGuard { cudaEvent_t &a, &b; ~EvGuard() { if (a) cudaEventDestroy(a); if (b) cudaEventDestroy(b); } } evg{e0, e1};
-    PG_CUDA(cudaEventCreate(&e0));
-    PG_CUDA(cudaEventCreate(&e1));
-    PG_CUDA(cudaEventRecord(e0, 0));
+    SectionTimer tm;
+    PG_CUDA(cudaEventCreate(&tm.e0));
+    PG_CUDA(cudaEventCreate(&tm.e1));
+    PG_CUDA(cudaEventRecord(tm.e0, 0));
 
-    std::vector<EncColumn> cols(nc);
-    for (int c = 0; c < nc; c++) {
-        pg_field f = s->field(c);
-        cols[c] = EncColumn{dcols[c].data, dcols[c].offsets, dcols[c].validity, f.type, type_width(f.type),
-                            (f.nullable || dcols[c].validity) ? 1 : 0, 0};
-    }
-    // jobs: row group major, column, page
-    std::vector<EncJob> jobs;
-    std::vector<StatJob> sjobs;
-    for (int64_t g = 0; g < n_groups; g++) {
-        const int64_t g0 = row0 + g * group_rows, g1 = std::min(row0 + n_rows, g0 + group_rows);
-        for (int c = 0; c < nc; c++) {
-            sjobs.push_back(StatJob{c, 0, g0, g1 - g0});
-            for (int64_t p0 = g0; p0 < g1; p0 += page_rows)
-                jobs.push_back(EncJob{c, (int32_t)(std::min(g1, p0 + page_rows) - p0), p0, -1, 0});
-        }
-    }
-    const size_t nj = jobs.size(), nsj = sjobs.size();
+    Plan pl = make_plan(*s, dcols, row0, n_rows, opt);
+    const size_t nj = pl.jobs.size(), nsj = pl.sjobs.size();
     std::vector<int64_t> counts(2 * nj + 2), stats(kStatWords * (nsj + 1));
     Scratch scratch(0);                                      // temporaries, released on every path out of this function
     EncColumn *d_cols = (EncColumn *)scratch.take(sizeof(EncColumn) * nc);
@@ -408,95 +612,24 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     int64_t *d_stats = (int64_t *)scratch.take(sizeof(int64_t) * kStatWords * (nsj + 1));
     if (!d_cols || !d_jobs || !d_sjobs || !d_counts || !d_stats)
         return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the page tables");
-    PG_CUDA(cudaMemcpy(d_cols, cols.data(), sizeof(EncColumn) * nc, cudaMemcpyHostToDevice));
+    PG_CUDA(cudaMemcpy(d_cols, pl.cols.data(), sizeof(EncColumn) * nc, cudaMemcpyHostToDevice));
     int launches = 0;
     if (nj) {
-        PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
-        PG_CUDA(cudaMemcpy(d_sjobs, sjobs.data(), sizeof(StatJob) * nsj, cudaMemcpyHostToDevice));
+        PG_CUDA(cudaMemcpy(d_jobs, pl.jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
+        PG_CUDA(cudaMemcpy(d_sjobs, pl.sjobs.data(), sizeof(StatJob) * nsj, cudaMemcpyHostToDevice));
         k_pw_count<<<(unsigned)nj, 256>>>(d_cols, d_jobs, d_counts);
         k_pw_stats<<<(unsigned)nsj, 256>>>(d_cols, d_sjobs, d_stats);
         launches += 2;
         PG_CUDA(cudaMemcpy(counts.data(), d_counts, sizeof(int64_t) * 2 * nj, cudaMemcpyDeviceToHost));
         PG_CUDA(cudaMemcpy(stats.data(), d_stats, sizeof(int64_t) * kStatWords * nsj, cudaMemcpyDeviceToHost));
     }
-
-    // ---- page bodies: level prefix (host-built) + values, per page
     auto ef = std::make_unique<EncodedFile>();
-    ef->stats.assign(nc, ColStats{});
-    for (int c = 0; c < nc; c++) { ef->stats[c].min = INT64_MAX; ef->stats[c].max = INT64_MIN; }
-    struct ChunkInfo { int64_t first_page, total_uncompressed, total_compressed, num_values, nn; size_t page0, page1; ColStats st; };
-    struct PageInfo { std::vector<uint8_t> prefix; int64_t def_bytes, body, stored; };
-    std::vector<ChunkInfo> chunks(nsj);
-    std::vector<PageInfo> pages;
-    pages.reserve(nj);
-    std::vector<char> file_nan(nc, 0);                       // per column: a chunk holds a NaN
-    size_t ji = 0;
-    for (size_t sj = 0; sj < nsj; sj++) {
-        const int c = sjobs[sj].col;
-        const EncColumn &ec = cols[c];
-        const int64_t *cs = &stats[kStatWords * sj];
-        const bool fp = ec.type == PG_FLOAT || ec.type == PG_DOUBLE, nan = cs[4] != 0;
-        ChunkInfo &ci = chunks[sj];
-        ci.page0 = ji;
-        ci.num_values = sjobs[sj].n_rows;
-        ci.nn = cs[2];
-        ci.st.null_count = ci.num_values - ci.nn;
-        ci.st.has_minmax = ec.width > 0 && ci.nn > 0 && !nan;   // a chunk with a NaN has no min / max
-        ci.st.min = cs[0];
-        ci.st.max = cs[1];
-        // parquet.thrift, Statistics: a zero min of a floating point column is written as -0.0, a zero max as +0.0,
-        // so that min <= v <= max holds for both zeros in the order readers compare with (Double.compare: -0.0 <
-        // +0.0).  The file-level merge below keeps the rule: the zero min it can take is -0.0, the zero max +0.0.
-        if (fp && ci.st.has_minmax) { ci.st.min = zero_as(ci.st.min, -0.0); ci.st.max = zero_as(ci.st.max, 0.0); }
-        file_nan[c] |= nan;
-        ColStats &fs = ef->stats[c];
-        fs.null_count += ci.st.null_count;
-        if (ci.st.has_minmax) {
-            if (!fs.has_minmax) { fs.min = ci.st.min; fs.max = ci.st.max; fs.has_minmax = 1; }
-            else if (fp) {
-                double a, b, x, y;
-                memcpy(&a, &fs.min, 8); memcpy(&b, &fs.max, 8); memcpy(&x, &ci.st.min, 8); memcpy(&y, &ci.st.max, 8);
-                a = std::min(a, x); b = std::max(b, y);
-                memcpy(&fs.min, &a, 8); memcpy(&fs.max, &b, 8);
-            } else { fs.min = std::min(fs.min, ci.st.min); fs.max = std::max(fs.max, ci.st.max); }
-        }
-        if (c == s->n_key + 1) ef->meta.delete_row_count += cs[3];
-        for (; ji < nj && jobs[ji].col == c && jobs[ji].row0 >= sjobs[sj].row0 &&
-               jobs[ji].row0 < sjobs[sj].row0 + sjobs[sj].n_rows; ji++) {
-            EncJob &j = jobs[ji];
-            const int64_t nn = counts[2 * ji], vb = counts[2 * ji + 1];
-            std::vector<uint8_t> prefix;                       // [def length:int32][hybrid header varint]
-            int64_t def_bytes = 0;
-            if (ec.optional) {
-                const int64_t groups = (j.n_rows + 7) / 8;
-                ThriftWriter tw;
-                tw.varint((uint64_t)(groups << 1) | 1);
-                const uint32_t len = (uint32_t)(tw.b.size() + groups);
-                prefix = {(uint8_t)len, (uint8_t)(len >> 8), (uint8_t)(len >> 16), (uint8_t)(len >> 24)};
-                prefix.insert(prefix.end(), tw.b.begin(), tw.b.end());
-                def_bytes = (int64_t)prefix.size() + groups;
-            }
-            int64_t val_bytes;
-            if (ec.width == 0) val_bytes = 4 * nn + vb;
-            else if (ec.type == PG_BOOL) val_bytes = (nn + 7) / 8;
-            else val_bytes = nn * (ec.width == 8 ? 8 : 4);
-            const int64_t body = def_bytes + val_bytes;
-            if (body > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet encode: page larger than 2 GiB");
-            pages.push_back(PageInfo{std::move(prefix), def_bytes, body, body});
-        }
-        ci.page1 = ji;
-    }
-    // A file with a NaN in a FLOAT / DOUBLE column has no min / max for that column, though its other chunks have
-    // some: NaN sorts above every value (Double.compare), so a max taken around it would prune rows `x > max` matches.
-    for (int c = 0; c < nc; c++)
-        if (file_nan[c]) ef->stats[c] = ColStats{INT64_MAX, INT64_MIN, ef->stats[c].null_count, 0};
-    const int n_pages = (int)pages.size();
+    if ((st = fold_counts(pl, counts.data(), stats.data(), s->n_key + 1, ef->stats, ef->meta.delete_row_count)))
+        return st;
 
     // ---- zstd: bodies into a scratch image, one frame per body; the frame sizes come back before the layout
-    int launches_zs = 0;
     const bool zstd = codec == pq::C_ZSTD;
-    std::vector<ZsBlockJob> bjobs;
-    std::vector<ZsPage> zpages(zstd ? nj : 0);
+    size_t nb = 0;
     uint8_t *d_img = nullptr, *d_zout = nullptr;
     ZsBlockJob *d_bjobs = nullptr;
     ZsPage *d_zpages = nullptr;
@@ -504,28 +637,25 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     int32_t *d_boff = nullptr;
     int64_t *d_frame = nullptr;
     if (zstd && nj) {
-        std::vector<PatchJob> pjobs;
-        std::vector<uint8_t> pbytes;
+        std::vector<ZsBlockJob> bjobs;
+        std::vector<ZsPage> zpages(nj);
+        std::vector<int64_t> img_off(nj);
         int64_t img = 0, out = 0, seq = 0;
         for (size_t p = 0; p < nj; p++) {
-            const PageInfo &pi = pages[p];
-            if (!pi.prefix.empty()) {
-                pjobs.push_back(PatchJob{img, (int32_t)pbytes.size(), (int32_t)pi.prefix.size()});
-                pbytes.insert(pbytes.end(), pi.prefix.begin(), pi.prefix.end());
-                jobs[p].def_off = img + (int64_t)pi.prefix.size();
-            }
-            jobs[p].val_off = img + pi.def_bytes;
-            zpages[p] = ZsPage{pi.body, (int32_t)bjobs.size(), 0};
-            for (int64_t b0 = 0; b0 == 0 || b0 < pi.body; b0 += zs::kMaxBlock) {
-                const int32_t n = (int32_t)std::min<int64_t>(zs::kMaxBlock, pi.body - b0);
+            const int64_t body = pl.pages[p].body;
+            img_off[p] = img;
+            zpages[p] = ZsPage{body, (int32_t)bjobs.size(), 0};
+            for (int64_t b0 = 0; b0 == 0 || b0 < body; b0 += zs::kMaxBlock) {
+                const int32_t n = (int32_t)std::min<int64_t>(zs::kMaxBlock, body - b0);
                 bjobs.push_back(ZsBlockJob{img + b0, out, seq, n, (int32_t)p});
                 out += n;
                 seq += n / 4 + 1;
                 zpages[p].n_blocks++;
             }
-            img += pi.body;
+            img += body;
         }
-        const size_t nb = bjobs.size();
+        const std::vector<Part> prefixes = place_bodies(pl, img_off);
+        nb = bjobs.size();
         d_img = (uint8_t *)scratch.take((size_t)img + 64);
         d_zout = (uint8_t *)scratch.take((size_t)out + 64);
         uint8_t *d_lits = (uint8_t *)scratch.take((size_t)img + 64);
@@ -535,180 +665,74 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         d_res = (int2 *)scratch.take(sizeof(int2) * nb);
         d_boff = (int32_t *)scratch.take(sizeof(int32_t) * nb);
         d_frame = (int64_t *)scratch.take(sizeof(int64_t) * nj);
-        PatchJob *d_pjobs = (PatchJob *)scratch.take(sizeof(PatchJob) * pjobs.size() + 16);
-        uint8_t *d_pbytes = (uint8_t *)scratch.take(pbytes.size() + 16);
-        if (!d_img || !d_zout || !d_lits || !d_seqs || !d_bjobs || !d_zpages || !d_res || !d_boff || !d_frame || !d_pjobs || !d_pbytes)
+        if (!d_img || !d_zout || !d_lits || !d_seqs || !d_bjobs || !d_zpages || !d_res || !d_boff || !d_frame)
             return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the zstd page images");
         PG_CUDA(cudaMemsetAsync(d_img, 0, (size_t)img + 64, 0));
-        PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
+        PG_CUDA(cudaMemcpy(d_jobs, pl.jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
         PG_CUDA(cudaMemcpy(d_bjobs, bjobs.data(), sizeof(ZsBlockJob) * nb, cudaMemcpyHostToDevice));
         PG_CUDA(cudaMemcpy(d_zpages, zpages.data(), sizeof(ZsPage) * nj, cudaMemcpyHostToDevice));
         k_pw_encode<<<(unsigned)nj, 256>>>(d_cols, d_jobs, d_img);
-        launches_zs++;
-        if (!pjobs.empty()) {
-            PG_CUDA(cudaMemcpy(d_pjobs, pjobs.data(), sizeof(PatchJob) * pjobs.size(), cudaMemcpyHostToDevice));
-            PG_CUDA(cudaMemcpy(d_pbytes, pbytes.data(), pbytes.size(), cudaMemcpyHostToDevice));
-            k_pw_patch<<<(unsigned)((pjobs.size() * 32 + 127) / 128), 128>>>(d_pjobs, (int)pjobs.size(), d_pbytes, d_img);
-            launches_zs++;
-        }
+        launches++;
+        if ((st = patch(scratch, prefixes, d_img, "the zstd page images"))) return st;
+        if (!prefixes.empty()) launches++;
         k_zs_block<<<(unsigned)nb, 32, kZsSmem>>>(d_bjobs, d_img, d_zout, d_seqs, d_lits, d_res);
         k_zs_page_sizes<<<(unsigned)((nj + 127) / 128), 128>>>(d_zpages, (int)nj, d_res, d_boff, d_frame);
-        launches_zs += 2;
+        launches += 2;
         std::vector<int64_t> frame_bytes(nj);
         SmallReads rd(0);
         if ((st = rd.add(frame_bytes.data(), d_frame, sizeof(int64_t) * nj))) return st;
-        launches_zs++;
+        launches++;
         if ((st = rd.finish())) return st;
         cudaError_t le = cudaGetLastError();
         if (le != cudaSuccess) return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(le));
-        for (size_t p = 0; p < nj; p++) pages[p].stored = frame_bytes[p];
+        for (size_t p = 0; p < nj; p++) pl.pages[p].stored = frame_bytes[p];
     }
 
-    // ---- layout: page headers (Thrift), level prefixes (uncompressed), stored bodies
-    int64_t pos = 4;                                         // after "PAR1"
+    // ---- layout: "PAR1", per page its header and its stored body, the footer
+    int64_t pos = 4;
     ef->host_parts.push_back({0, {'P', 'A', 'R', '1'}});
-    std::vector<int64_t> frame_off(zstd ? nj : 0);
-    for (size_t sj = 0; sj < nsj; sj++) {
-        ChunkInfo &ci = chunks[sj];
-        ci.first_page = pos;
-        ci.total_uncompressed = ci.total_compressed = 0;
-        for (size_t p = ci.page0; p < ci.page1; p++) {
-            EncJob &j = jobs[p];
-            const PageInfo &pi = pages[p];
-            ThriftWriter ph;                                   // PageHeader
-            ph.i32(1, pq::P_DATA);
-            ph.i32(2, (int32_t)pi.body);
-            ph.i32(3, (int32_t)pi.stored);
-            ph.struct_field(5);                                // DataPageHeader
-            ph.i32(1, j.n_rows);
-            ph.i32(2, pq::E_PLAIN);
-            ph.i32(3, pq::E_RLE);
-            ph.i32(4, pq::E_RLE);
-            ph.end();
-            ph.end();
-            ef->host_parts.push_back({pos, ph.b});
-            pos += (int64_t)ph.b.size();
-            if (zstd) frame_off[p] = pos;
-            else {
-                if (!pi.prefix.empty()) {
-                    ef->host_parts.push_back({pos, pi.prefix});
-                    j.def_off = pos + (int64_t)pi.prefix.size();
-                }
-                j.val_off = pos + pi.def_bytes;
-            }
-            pos += pi.stored;
-            ci.total_uncompressed += (int64_t)ph.b.size() + pi.body;
-            ci.total_compressed += (int64_t)ph.b.size() + pi.stored;
+    std::vector<int64_t> body_off(nj);
+    for (Chunk &ch : pl.chunks) {
+        ch.first_page = pos;
+        for (size_t p = ch.page0; p < ch.page1; p++) {
+            const Page &pg = pl.pages[p];
+            std::vector<uint8_t> header = page_header(pg, pl.jobs[p].n_rows);
+            const int64_t hb = (int64_t)header.size();
+            ef->host_parts.push_back({pos, std::move(header)});
+            body_off[p] = pos + hb;
+            pos += hb + pg.stored;
+            ch.total_uncompressed += hb + pg.body;
+            ch.total_compressed += hb + pg.stored;
         }
     }
-    const int64_t data_end = pos;
+    ef->data_end = pos;
+    ef->host_parts.push_back({pos, footer(pl, names, n_rows, zstd)});
+    ef->file_bytes = pos + (int64_t)ef->host_parts.back().second.size();
 
-    // ---- footer
-    ThriftWriter fw;
-    fw.i32(1, 1);                                              // version
-    fw.list(2, 12, (size_t)nc + 1);                            // schema
-    fw.struct_elem();
-    fw.str(4, "paimon_schema");
-    fw.i32(5, nc);
-    fw.end();
-    for (int c = 0; c < nc; c++) {
-        const EncColumn &ec = cols[c];
-        fw.struct_elem();
-        fw.i32(1, parquet_type_of(ec.type));
-        fw.i32(3, ec.optional ? pq::R_OPTIONAL : pq::R_REQUIRED);
-        fw.str(4, names && names[c] ? names[c] : ("c" + std::to_string(c)));
-        if (ec.type == PG_STRING) fw.i32(6, 0);               // UTF8
-        else if (ec.type == PG_INT8) fw.i32(6, 15);           // INT_8
-        else if (ec.type == PG_INT16) fw.i32(6, 16);          // INT_16
-        fw.end();
-    }
-    fw.i64(3, n_rows);
-    fw.list(4, 12, (size_t)n_groups);
-    for (int64_t g = 0; g < n_groups; g++) {
-        fw.struct_elem();                                      // RowGroup
-        fw.list(1, 12, (size_t)nc);
-        int64_t group_bytes = 0;
-        for (int c = 0; c < nc; c++) {
-            const ChunkInfo &ci = chunks[(size_t)g * nc + c];
-            const EncColumn &ec = cols[c];
-            group_bytes += ci.total_uncompressed;
-            fw.struct_elem();                                  // ColumnChunk
-            fw.i64(2, ci.first_page);
-            fw.struct_field(3);                                // ColumnMetaData
-            fw.i32(1, parquet_type_of(ec.type));
-            fw.list(2, 5, 2); fw.zigzag(pq::E_PLAIN); fw.zigzag(pq::E_RLE);
-            fw.list(3, 8, 1);
-            { std::string nm = names && names[c] ? names[c] : ("c" + std::to_string(c)); fw.varint(nm.size()); fw.b.insert(fw.b.end(), nm.begin(), nm.end()); }
-            fw.i32(4, zstd ? pq::C_ZSTD : pq::C_UNCOMPRESSED);
-            fw.i64(5, ci.num_values);
-            fw.i64(6, ci.total_uncompressed);
-            fw.i64(7, ci.total_compressed);
-            fw.i64(9, ci.first_page);
-            fw.struct_field(12);                               // Statistics
-            fw.i64(3, ci.st.null_count);
-            if (ci.st.has_minmax) {
-                uint8_t mn[8], mx[8];
-                size_t w = ec.width == 8 ? 8 : 4;
-                if (ec.type == PG_FLOAT) {
-                    double a, b; memcpy(&a, &ci.st.min, 8); memcpy(&b, &ci.st.max, 8);
-                    float fa = (float)a, fb = (float)b; memcpy(mn, &fa, 4); memcpy(mx, &fb, 4);
-                } else if (ec.type == PG_BOOL) {
-                    w = 1; mn[0] = (uint8_t)ci.st.min; mx[0] = (uint8_t)ci.st.max;
-                } else if (w == 4) {
-                    int32_t a = (int32_t)ci.st.min, b = (int32_t)ci.st.max; memcpy(mn, &a, 4); memcpy(mx, &b, 4);
-                } else { memcpy(mn, &ci.st.min, 8); memcpy(mx, &ci.st.max, 8); }
-                fw.bin(5, mx, w);
-                fw.bin(6, mn, w);
-            }
-            fw.end();
-            fw.end();                                          // ColumnMetaData
-            fw.end();                                          // ColumnChunk
-        }
-        fw.i64(2, group_bytes);
-        fw.i64(3, std::min(row0 + n_rows, row0 + (g + 1) * group_rows) - (row0 + g * group_rows));
-        fw.end();
-    }
-    fw.str(6, "paimon-b200 (libpaimon_gpu)");
-    // column_orders: TYPE_ORDER (TypeDefinedOrder) for every column.  Readers take min_value / max_value only from a
-    // file that declares the order they were computed in; without it parquet-cpp (pyarrow) ignores them.
-    fw.list(7, 12, (size_t)nc);
-    for (int c = 0; c < nc; c++) {
-        fw.struct_elem();                                      // ColumnOrder (union)
-        fw.struct_field(1);                                    // TYPE_ORDER: TypeDefinedOrder, no fields
-        fw.end();
-        fw.end();
-    }
-    fw.end();
-    std::vector<uint8_t> tail = fw.b;
-    const uint32_t flen = (uint32_t)fw.b.size();
-    tail.insert(tail.end(), {(uint8_t)flen, (uint8_t)(flen >> 8), (uint8_t)(flen >> 16), (uint8_t)(flen >> 24), 'P', 'A', 'R', '1'});
-    ef->host_parts.push_back({data_end, tail});
-    ef->file_bytes = data_end + (int64_t)tail.size();
-
-    // ---- page bodies on the device
+    // ---- page bodies on the device: the zstd frames gathered, or the bodies written in place behind their prefixes
     PG_CUDA(cudaMalloc(&ef->d_file, (size_t)ef->file_bytes + 64));
     PG_CUDA(cudaMemsetAsync(ef->d_file, 0, (size_t)ef->file_bytes + 64, 0));
     if (nj && zstd) {
         // (the frame sizes have been read: their buffer takes the frame offsets)
-        PG_CUDA(cudaMemcpy(d_frame, frame_off.data(), sizeof(int64_t) * nj, cudaMemcpyHostToDevice));
-        k_zs_gather<<<(unsigned)bjobs.size(), 256>>>(d_bjobs, d_zpages, d_res, d_boff, d_frame, d_img, d_zout, ef->d_file);
-        launches += launches_zs + 1;
+        PG_CUDA(cudaMemcpy(d_frame, body_off.data(), sizeof(int64_t) * nj, cudaMemcpyHostToDevice));
+        k_zs_gather<<<(unsigned)nb, 256>>>(d_bjobs, d_zpages, d_res, d_boff, d_frame, d_img, d_zout, ef->d_file);
+        launches++;
     } else if (nj) {
-        PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
+        for (Part &prefix : place_bodies(pl, body_off)) ef->host_parts.push_back(std::move(prefix));
+        PG_CUDA(cudaMemcpy(d_jobs, pl.jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
         k_pw_encode<<<(unsigned)nj, 256>>>(d_cols, d_jobs, ef->d_file);
         launches++;
     }
-    PG_CUDA(cudaEventRecord(e1, 0));
-    PG_CUDA(cudaEventSynchronize(e1));
-    float ms = 0;
-    cudaEventElapsedTime(&ms, e0, e1);
+    PG_CUDA(cudaEventRecord(tm.e1, 0));
+    PG_CUDA(cudaEventSynchronize(tm.e1));
+    const float ms = tm.ms();
     cudaError_t le = cudaGetLastError();
     if (le != cudaSuccess) return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(le));
 
     ef->meta.n_rows = n_rows;
     ef->meta.file_bytes = ef->file_bytes;
-    ef->meta.n_row_groups = (int32_t)n_groups;
-    ef->meta.n_pages = n_pages;
+    ef->meta.n_row_groups = (int32_t)pl.n_groups;
+    ef->meta.n_pages = (int)nj;
     ef->meta.ms_encode = ms;
     ef->meta.launches = launches;
     const ColStats &sq = ef->stats[s->n_key];
@@ -771,8 +795,7 @@ pg_status pg_parquet_file_fetch(uint64_t file, void *host_buffer, int64_t capaci
     if (capacity < ef->file_bytes) return fail(PG_ERR_INVALID, "buffer smaller than the file");
     pg_status st = ensure_device();
     if (st) return st;
-    const auto &tail = ef->host_parts.back();
-    PG_CUDA(cudaMemcpy(host_buffer, ef->d_file, (size_t)tail.first, cudaMemcpyDeviceToHost));
+    PG_CUDA(cudaMemcpy(host_buffer, ef->d_file, (size_t)ef->data_end, cudaMemcpyDeviceToHost));
     for (const auto &p : ef->host_parts) memcpy((uint8_t *)host_buffer + p.first, p.second.data(), p.second.size());
     return PG_OK;
 }
@@ -783,20 +806,8 @@ pg_status pg_parquet_file_device_image(uint64_t file, const uint8_t **device_byt
     pg_status st = ensure_device();
     if (st) return st;
     if (!ef->image_complete) {
-        std::vector<PatchJob> jobs;
-        std::vector<uint8_t> bytes;
-        for (const auto &p : ef->host_parts) {
-            if (bytes.size() + p.second.size() > 0x7fffffffull) return fail(PG_ERR_UNSUPPORTED, "parquet encode: too many header bytes");
-            jobs.push_back(PatchJob{p.first, (int32_t)bytes.size(), (int32_t)p.second.size()});
-            bytes.insert(bytes.end(), p.second.begin(), p.second.end());
-        }
         Scratch scratch(0);
-        PatchJob *d_jobs = (PatchJob *)scratch.take(sizeof(PatchJob) * jobs.size() + 16);
-        uint8_t *d_bytes = (uint8_t *)scratch.take(bytes.size() + 16);
-        if (!d_jobs || !d_bytes) return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the header patch");
-        PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(PatchJob) * jobs.size(), cudaMemcpyHostToDevice));
-        PG_CUDA(cudaMemcpy(d_bytes, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
-        k_pw_patch<<<(unsigned)((jobs.size() * 32 + 127) / 128), 128>>>(d_jobs, (int)jobs.size(), d_bytes, ef->d_file);
+        if ((st = patch(scratch, ef->host_parts, ef->d_file, "the header patch"))) return st;
         cudaError_t e = cudaDeviceSynchronize();
         if (e != cudaSuccess) return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(e));
         ef->image_complete = true;

@@ -1,4 +1,4 @@
-// parquet_meta.cc — Thrift compact protocol reader + Parquet footer / page-header parse (see parquet_meta.h).
+// parquet_meta.cc — Thrift compact protocol reader + Parquet footer parse (see parquet_meta.h).
 #include "parquet_meta.h"
 
 #include <stdexcept>
@@ -6,9 +6,6 @@
 namespace pq {
 
 namespace {
-
-enum TType { CT_STOP = 0, CT_TRUE = 1, CT_FALSE = 2, CT_BYTE = 3, CT_I16 = 4, CT_I32 = 5, CT_I64 = 6, CT_DOUBLE = 7,
-             CT_BINARY = 8, CT_LIST = 9, CT_SET = 10, CT_MAP = 11, CT_STRUCT = 12 };
 
 struct Reader {
     const uint8_t *p, *end;
@@ -220,65 +217,6 @@ FileMetaData parse_footer(const uint8_t *file, int64_t size) {
     const int64_t flen = footer_length(file + size - 8);
     if (flen + 12 > size) throw std::runtime_error("parquet: bad footer length");
     return parse_footer_thrift(file + size - 8 - flen, flen);
-}
-
-PageHeader parse_page_header(const uint8_t *p, int64_t avail) {
-    Reader r(p, avail);
-    PageHeader h;
-    int16_t id = 0;
-    int t;
-    while (r.field(id, t)) {
-        switch (id) {
-            case 1: h.type = (int32_t)r.zigzag(); break;
-            case 2: h.uncompressed_size = (int32_t)r.zigzag(); break;
-            case 3: h.compressed_size = (int32_t)r.zigzag(); break;
-            case 5: {                                   // DataPageHeader
-                int16_t i2 = 0;
-                int t2;
-                while (r.field(i2, t2)) {
-                    switch (i2) {
-                        case 1: h.num_values = (int32_t)r.zigzag(); break;
-                        case 2: h.encoding = (int32_t)r.zigzag(); break;
-                        case 3: h.def_level_encoding = (int32_t)r.zigzag(); break;
-                        default: r.skip(t2);
-                    }
-                }
-                break;
-            }
-            case 7: {                                   // DictionaryPageHeader
-                int16_t i2 = 0;
-                int t2;
-                while (r.field(i2, t2)) {
-                    switch (i2) {
-                        case 1: h.num_values = (int32_t)r.zigzag(); break;
-                        case 2: h.encoding = (int32_t)r.zigzag(); break;
-                        default: r.skip(t2);
-                    }
-                }
-                break;
-            }
-            case 8: {                                   // DataPageHeaderV2
-                int16_t i2 = 0;
-                int t2;
-                while (r.field(i2, t2)) {
-                    switch (i2) {
-                        case 1: h.num_values = (int32_t)r.zigzag(); break;
-                        case 2: h.num_nulls = (int32_t)r.zigzag(); break;
-                        case 3: h.num_rows = (int32_t)r.zigzag(); break;
-                        case 4: h.encoding = (int32_t)r.zigzag(); break;
-                        case 5: h.def_levels_byte_length = (int32_t)r.zigzag(); break;
-                        case 6: h.rep_levels_byte_length = (int32_t)r.zigzag(); break;
-                        case 7: h.is_compressed = (t2 == CT_TRUE); break;
-                        default: r.skip(t2);
-                    }
-                }
-                break;
-            }
-            default: r.skip(t);
-        }
-    }
-    h.header_size = (int32_t)(r.p - p);
-    return h;
 }
 
 }  // namespace pq

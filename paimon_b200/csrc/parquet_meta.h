@@ -1,7 +1,7 @@
-// parquet_meta.h — host-side Parquet metadata: Thrift compact-protocol reader, footer (FileMetaData) and
-// page headers.  Replaces what the reference takes from parquet-mr 1.16.0
-// (org.apache.parquet.format.* via PQ3P/hadoop/ParquetFileReader.java:277-334 footer read,
-// :1345 Chunk.readAllPages page-header loop).  The algorithm restated here is the public Parquet format
+// parquet_meta.h — host-side Parquet metadata: Thrift compact-protocol reader and writer, footer (FileMetaData).
+// Replaces what the reference takes from parquet-mr 1.16.0
+// (org.apache.parquet.format.* via PQ3P/hadoop/ParquetFileReader.java:277-334 footer read, and the page headers and
+// footer its writer serializes).  The algorithm restated here is the public Parquet format
 // specification (parquet-format: "Thrift Compact Protocol" + parquet.thrift field ids), which is what
 // parquet-mr implements; the dependency itself is not vendored in /root/reference.
 #pragma once
@@ -20,6 +20,9 @@ enum Encoding { E_PLAIN = 0, E_PLAIN_DICTIONARY = 2, E_RLE = 3, E_BIT_PACKED = 4
 enum Codec { C_UNCOMPRESSED = 0, C_SNAPPY = 1, C_GZIP = 2, C_LZO = 3, C_BROTLI = 4, C_LZ4 = 5, C_ZSTD = 6, C_LZ4_RAW = 7 };
 enum PageType { P_DATA = 0, P_INDEX = 1, P_DICTIONARY = 2, P_DATA_V2 = 3 };
 enum Repetition { R_REQUIRED = 0, R_OPTIONAL = 1, R_REPEATED = 2 };
+// Thrift compact protocol wire types
+enum TType { CT_STOP = 0, CT_TRUE = 1, CT_FALSE = 2, CT_BYTE = 3, CT_I16 = 4, CT_I32 = 5, CT_I64 = 6, CT_DOUBLE = 7,
+             CT_BINARY = 8, CT_LIST = 9, CT_SET = 10, CT_MAP = 11, CT_STRUCT = 12 };
 
 struct SchemaElement {
     int32_t type = -1;            // PhysType; -1 for groups
@@ -60,26 +63,43 @@ struct FileMetaData {
     std::string created_by;
 };
 
-struct PageHeader {
-    int32_t type = -1;
-    int32_t uncompressed_size = 0;
-    int32_t compressed_size = 0;
-    int32_t num_values = 0;
-    int32_t encoding = 0;
-    int32_t def_level_encoding = E_RLE;
-    // v2
-    int32_t num_nulls = 0, num_rows = 0;
-    int32_t def_levels_byte_length = 0, rep_levels_byte_length = 0;
-    bool is_compressed = true;
-    int32_t header_size = 0;      // bytes the Thrift header occupied
-};
-
 // Throws std::runtime_error on malformed input.
 FileMetaData parse_footer(const uint8_t *file, int64_t size);
 // the pieces of parse_footer, for files whose bytes live on the device: the last 8 bytes of the file
 // ([footer length:4 LE]["PAR1"]) -> footer length; the Thrift FileMetaData bytes in front of them -> metadata
 int64_t footer_length(const uint8_t *tail8);
 FileMetaData parse_footer_thrift(const uint8_t *footer, int64_t flen);
-PageHeader parse_page_header(const uint8_t *p, int64_t avail);
+
+inline void put_varint(std::vector<uint8_t> &b, uint64_t v) {
+    while (v >= 0x80) { b.push_back((uint8_t)(v | 0x80)); v >>= 7; }
+    b.push_back((uint8_t)v);
+}
+
+// Thrift compact protocol writer: the page headers and the footer of the files the device encoder writes
+struct ThriftWriter {
+    std::vector<uint8_t> b;
+    std::vector<int> last{0};                           // per open struct: the id of its last field
+    void varint(uint64_t v) { put_varint(b, v); }
+    void zigzag(int64_t v) { varint(((uint64_t)v << 1) ^ (uint64_t)(v >> 63)); }
+    void field(int id, int type) {
+        int d = id - last.back();
+        if (d > 0 && d <= 15) b.push_back((uint8_t)((d << 4) | type));
+        else { b.push_back((uint8_t)type); zigzag(id); }
+        last.back() = id;
+    }
+    void i32(int id, int32_t v) { field(id, CT_I32); zigzag(v); }
+    void i64(int id, int64_t v) { field(id, CT_I64); zigzag(v); }
+    void binary(const void *p, size_t n) { varint(n); b.insert(b.end(), (const uint8_t *)p, (const uint8_t *)p + n); }
+    void bin(int id, const void *p, size_t n) { field(id, CT_BINARY); binary(p, n); }
+    void str(int id, const std::string &s) { bin(id, s.data(), s.size()); }
+    void list(int id, int elem_type, size_t n) {
+        field(id, CT_LIST);
+        if (n < 15) b.push_back((uint8_t)((n << 4) | elem_type));
+        else { b.push_back((uint8_t)(0xF0 | elem_type)); varint(n); }
+    }
+    void struct_field(int id) { field(id, CT_STRUCT); last.push_back(0); }
+    void struct_elem() { last.push_back(0); }           // list element
+    void end() { b.push_back(CT_STOP); last.pop_back(); }
+};
 
 }  // namespace pq

@@ -99,7 +99,7 @@ def java_compare(a, b) -> int:
 # ---------------------------------------------------------------------------------------------- layout
 
 def writer_rows(page_rows: int = 0, row_group_rows: int = 0) -> Tuple[int, int]:
-    """(page rows, row-group rows) as the encoder rounds them (parquet_encode.cu, encode())."""
+    """(page rows, row-group rows) as the encoder rounds them (parquet_encode.cu, make_plan())."""
     page = page_rows if page_rows > 0 else 32768
     page = (page + 7) & ~7
     group = row_group_rows if row_group_rows > 0 else 1 << 20

@@ -18,7 +18,7 @@ from paimon_b200.compact_rewriter import KeyValueDataFileWriter, MergeTreeCompac
 from paimon_b200.format import FileFormat, FormatReaderContext, LocalFileIO
 from paimon_b200.merge_function import DeduplicateMergeFunction, PartialUpdateMergeFunction
 from paimon_b200.merge_tree_readers import DataFileMeta, IntervalPartition, concat_batches
-from paimon_b200.sort_merge_reader import SortedRunReader, _SchemaHandle
+from paimon_b200.sort_merge_reader import SortedRunReader, SortMergeReader, _SchemaHandle
 from paimon_b200.types import DataField, KeyValueSchema, PhysicalType, RowType, is_varlen
 
 from parquet_util import arrow_to_batch, write_kv_parquet
@@ -115,6 +115,56 @@ def test_device_decoder_reads_what_the_device_writes(tmp_path):
         rd.close()
     assert got.equals(run), got.first_difference(run)
     assert arrow_to_batch(schema, pq.read_table(path)).equals(run)
+
+
+def test_encoder_refuses_bad_arguments():
+    """Both entry points refuse, with PG_ERR_INVALID and the same message: a row range that does not start at a
+    multiple of 8 (the definition levels are the batch's bitmap bytes) or leaves the batch, a batch merged under a
+    read-type projection (it lacks columns a data file needs), and an unknown source handle."""
+    schema = all_types_schema()
+    batch = KeyValueBatch.from_rows(schema, random_rows(random.Random(5), 100))
+    lib = N.init(0)
+    names = file_column_names(schema)
+    arr = (C.c_char_p * len(names))(*[n.encode() for n in names])
+    opts = N.PgParquetWriteOptions(0, 0)
+
+    def encode_both(source, row0, n_rows):
+        out = []
+        for codec in (None, 6):
+            fh = C.c_uint64(0)
+            if codec is None:
+                st = lib.pg_parquet_encode(source, arr, row0, n_rows, C.byref(opts), C.byref(fh))
+            else:
+                st = lib.pg_parquet_encode_compressed(source, arr, row0, n_rows, C.byref(opts), codec, 1, C.byref(fh))
+            out.append((st, lib.pg_last_error().decode() if st else ""))
+            if st == 0:
+                lib.pg_parquet_file_free(fh.value)
+        return out
+
+    mask = [f.name in ("pk", "i") for f in schema.value_type.fields]
+    merge = SortMergeReader([SortedRunReader(schema, batch)], DeduplicateMergeFunction.factory().create()
+                            .with_read_fields(mask))
+    sh = _SchemaHandle(schema, 0)
+    run, gone = SortedRunReader(schema, batch), SortedRunReader(schema, batch)
+    try:
+        merge.execute()
+        assert merge.device_batch().n_rows > 0
+        h = run._open(sh.handle)
+        unknown = gone._open(sh.handle)
+        gone.close()
+        assert encode_both(h, 8, -1) == [(0, ""), (0, "")]
+        bad_range = "parquet encode: row range outside the batch or not starting at a multiple of 8"
+        cases = [(h, 3, -1, bad_range), (h, 3, 8, bad_range), (h, -8, 8, bad_range), (h, 0, 101, bad_range),
+                 (h, 96, 8, bad_range),
+                 (merge._merge_h, 0, -1, "parquet encode: the batch was produced under a read-type projection"),
+                 (unknown, 0, -1, "unknown run / merge handle")]
+        for source, row0, n_rows, message in cases:
+            for st, msg in encode_both(source, row0, n_rows):
+                assert st == 1 and msg.startswith(message), (row0, n_rows, st, msg)
+    finally:
+        run.close()
+        merge.close()
+        sh.close()
 
 
 @pytest.mark.parametrize("drop_delete", [True, False])

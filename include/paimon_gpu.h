@@ -428,6 +428,38 @@ pg_status pg_parquet_file_fetch(uint64_t file, void *host_buffer, int64_t capaci
 pg_status pg_parquet_file_device_image(uint64_t file, const uint8_t **device_bytes, int64_t *size);
 pg_status pg_parquet_file_free(uint64_t file);
 
+/* ---- compaction output encode: device batch -> ORC data file ----------------------------------------------
+ * The same rewrite step for tables whose 'file.format' (or 'file.format.per.level' at the output level) is orc: the
+ * writer behind KeyValueFileWriterFactory (paimon-core/.../io/KeyValueFileWriterFactory.java:301-310) is then
+ * OrcWriterFactory (paimon-format/.../orc/OrcWriterFactory.java), types mapped by OrcTypeUtil.convertToOrcType.
+ * `source`, `row0` (a multiple of 8) and `n_rows` mean what they mean for pg_parquet_encode, and a batch produced under
+ * a read-type projection is refused the same way.  The result is an encoded-file handle like Parquet's:
+ * pg_parquet_file_meta (n_row_groups counts stripes, n_pages streams), _column_stats (same meaning), _fetch,
+ * _device_image and _free accept it.
+ * Written: ORC v1 ("0.12"), a flat struct named by `column_names`, streams DIRECT / DIRECT_V2 (integer RLE v2 without
+ * PATCHED_BASE, byte RLE, PRESENT only in stripes with a null), no row indexes or bloom filters, per-stripe and file
+ * column statistics.  Compression kinds ZLIB / SNAPPY / LZO / LZ4 / BROTLI, zstd levels 0 and >= 2, TIMESTAMP, CHAR
+ * and nested kinds, and a VARCHAR(n) value longer than n characters return PG_ERR_UNSUPPORTED; a compression kind
+ * outside 0..6, a block size >= 2^23 or negative, and a kind that does not fit the column's physical type return
+ * PG_ERR_INVALID. */
+typedef struct {
+    int32_t kind;        /* ORC TypeKind (orc_proto): BOOLEAN 0, BYTE 1, SHORT 2, INT 3, LONG 4, FLOAT 5, DOUBLE 6,
+                            STRING 7, BINARY 8, DECIMAL 14, DATE 15, VARCHAR 16 */
+    int32_t precision, scale;   /* DECIMAL */
+    int32_t max_length;         /* VARCHAR */
+} pg_orc_column_type;
+
+typedef struct {
+    int64_t stripe_rows;             /* 0 = 1 Mi rows; rounded up to a multiple of 8 */
+    int32_t compression;             /* ORC CompressionKind: 0 NONE, 5 ZSTD */
+    int32_t zstd_level;              /* like pg_parquet_encode_compressed: 1 and the negative levels */
+    int64_t compression_block_size;  /* 0 = 256 KiB ('orc.compress.size') */
+    const pg_orc_column_type *types; /* [n_key + 2 + n_val], NULL = from the physical types */
+} pg_orc_write_options;
+
+pg_status pg_orc_encode(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
+                        const pg_orc_write_options *options, uint64_t *out_file);
+
 /* IntervalPartition over int64 (min,max) key bounds of data files: section and run id per file */
 pg_status pg_interval_partition(int32_t n_files, const int64_t *min_key, const int64_t *max_key,
                                 int32_t *section_of, int32_t *run_of, int32_t *n_sections);

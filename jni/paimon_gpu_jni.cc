@@ -289,6 +289,27 @@ JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetEncodeComp
     PG_CHECK(pg_parquet_encode_compressed((uint64_t)source, ptrs.data(), row0, nRows, &opt, codec, level, &h));
     return (jlong)h;
 }
+// The same rows as one ORC file: compression = ORC CompressionKind (0 NONE, 5 ZSTD), blockSize = orc.compress.size
+// (0 = 256 KiB); types = 4 ints per column (kind, precision, scale, max length; pg_orc_column_type), or null for the
+// kinds of the physical types.  The result is a file handle for fileMeta / fileFetch / fileFree like Parquet's.
+JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_orcEncode(JNIEnv *env, jclass, jlong source,
+                                                                         jobjectArray names, jlong row0, jlong nRows,
+                                                                         jlong stripeRows, jint compression, jint level,
+                                                                         jlong blockSize, jintArray types) {
+    std::vector<std::string> keep;
+    std::vector<const char *> ptrs = utf_names(env, names, keep);
+    std::vector<pg_orc_column_type> cols;
+    if (types) {
+        const jsize n = env->GetArrayLength(types);
+        std::vector<jint> v((size_t)n);
+        env->GetIntArrayRegion(types, 0, n, v.data());
+        for (jsize i = 0; i + 3 < n; i += 4) cols.push_back(pg_orc_column_type{v[i], v[i + 1], v[i + 2], v[i + 3]});
+    }
+    pg_orc_write_options opt{stripeRows, compression, level, blockSize, types ? cols.data() : nullptr};
+    uint64_t h = 0;
+    PG_CHECK(pg_orc_encode((uint64_t)source, ptrs.data(), row0, nRows, &opt, &h));
+    return (jlong)h;
+}
 JNIEXPORT jlongArray JNICALL Java_org_apache_paimon_gpu_NativeMerge_fileMeta(JNIEnv *env, jclass, jlong file) {
     pg_file_meta m{};
     pg_status fst = pg_parquet_file_meta((uint64_t)file, &m);

@@ -87,6 +87,15 @@ class PgFileMeta(C.Structure):
                 ("n_pages", C.c_int32), ("ms_encode", C.c_float), ("launches", C.c_int32)]
 
 
+class PgOrcColumnType(C.Structure):
+    _fields_ = [("kind", C.c_int32), ("precision", C.c_int32), ("scale", C.c_int32), ("max_length", C.c_int32)]
+
+
+class PgOrcWriteOptions(C.Structure):
+    _fields_ = [("stripe_rows", C.c_int64), ("compression", C.c_int32), ("zstd_level", C.c_int32),
+                ("compression_block_size", C.c_int64), ("types", C.POINTER(PgOrcColumnType))]
+
+
 class PaimonGpuError(RuntimeError):
     """A non-zero pg_status.  `.status` holds the code (PG_ERR_*)."""
 
@@ -153,6 +162,8 @@ _SIGNATURES = {
     "pg_parquet_encode_compressed": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,
                                                  C.POINTER(PgParquetWriteOptions), C.c_int32, C.c_int32,
                                                  C.POINTER(C.c_uint64)]),
+    "pg_orc_encode": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,
+                                  C.POINTER(PgOrcWriteOptions), C.POINTER(C.c_uint64)]),
     "pg_parquet_file_meta": (C.c_int32, [C.c_uint64, C.POINTER(PgFileMeta)]),
     "pg_parquet_file_column_stats": (C.c_int32, [C.c_uint64, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int32),
                                                  C.c_void_p, C.c_void_p]),

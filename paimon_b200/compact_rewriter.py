@@ -1,4 +1,4 @@
-"""The rewrite side of a compaction: merged device batch -> Parquet data files + DataFileMeta.
+"""The rewrite side of a compaction: merged device batch -> Parquet or ORC data files + DataFileMeta.
 
 Mirrors (same names, same argument meaning):
   KeyValueDataFileWriter.write / result      paimon-core/.../io/KeyValueDataFileWriter.java:108-184
@@ -6,7 +6,7 @@ Mirrors (same names, same argument meaning):
   MergeTreeCompactRewriter.rewriteCompaction paimon-core/.../mergetree/compact/MergeTreeCompactRewriter.java:78-116
   CompactResult(before, after)               paimon-core/.../compact/CompactResult.java
 
-The merge of a section, the drop-delete filter, the Parquet encode and the file statistics all happen on the
+The merge of a section, the drop-delete filter, the Parquet or ORC encode and the file statistics all happen on the
 device; the host writes the encoded bytes through the FileIO and assembles the DataFileMeta.
 """
 from __future__ import annotations
@@ -24,7 +24,7 @@ from .merge_function import MergeFunctionFactory
 from .merge_tree_readers import (DataFileMeta, IntervalPartition, KeyValueFileReaderFactory, MergeTreeReaders,
                                  SortedRun)
 from .sort_merge_reader import SortMergeReader
-from .types import KeyValueSchema, PhysicalType, is_varlen
+from .types import KeyValueSchema, PhysicalType, is_varlen, orc_column_type
 
 
 @dataclass
@@ -48,8 +48,15 @@ PARQUET_CODECS = {"none": 0, "uncompressed": 0, "snappy": 1, "gzip": 2, "lzo": 3
                   "lz4_raw": 7}
 
 
+# ORC CompressionKind numbers (orc_proto) by the names 'orc.compress' and 'file.compression' use
+ORC_CODECS = {"none": 0, "uncompressed": 0, "zlib": 1, "snappy": 2, "lzo": 3, "lz4": 4, "zstd": 5, "brotli": 6}
+
+FILE_FORMATS = ("parquet", "orc")
+
+
 def _per_level(value) -> Dict[int, str]:
-    """'file.compression.per.level' as a map: a dict, or the option's string form '0:lz4,5:zstd'."""
+    """'file.compression.per.level' / 'file.format.per.level' as a map: a dict, or the option's string form
+    '0:lz4,5:zstd'."""
     if isinstance(value, dict):
         return {int(k): str(v) for k, v in value.items()}
     out = {}
@@ -74,6 +81,27 @@ def compression_for_level(options: Optional[Dict[str, object]], level: int) -> T
     return codec, zstd_level
 
 
+def format_for_level(options: Optional[Dict[str, object]], level: int) -> str:
+    """The file format of a data file written at `level`: 'file.format.per.level' for the level, else 'file.format',
+    else parquet (KeyValueFileWriterFactory.java:301-310, CoreOptions.java:292-313)."""
+    options = options or {}
+    per_level = _per_level(options.get("file.format.per.level", {}))
+    return str(per_level.get(level, options.get("file.format", "parquet"))).lower()
+
+
+def orc_compression_for_level(options: Optional[Dict[str, object]], level: int) -> Tuple[str, int, int]:
+    """(codec name, zstd level, compression block size) of an ORC data file written at `level`: the codec is
+    'file.compression.per.level' for the level, else 'file.compression' (default zstd), overridden by 'orc.compress'
+    (OrcWriterFactory.java:101-104); the level is 'orc.compression.zstd.level', else 'file.compression.zstd-level'
+    (default 1; OrcFileFormat.java:158-175); the block size is 'orc.compress.size' (0 = the library's 256 KiB)."""
+    options = options or {}
+    per_level = _per_level(options.get("file.compression.per.level", {}))
+    codec = per_level.get(level, options.get("file.compression", "zstd"))
+    codec = str(options.get("orc.compress", codec)).lower()
+    zstd_level = int(options.get("orc.compression.zstd.level", options.get("file.compression.zstd-level", 1)))
+    return codec, zstd_level, int(options.get("orc.compress.size", 0))
+
+
 def file_column_names(schema: KeyValueSchema) -> List[str]:
     """[_KEY_*, _SEQUENCE_NUMBER, _VALUE_KIND, value...] (KeyValue.schema, KeyValue.java:130-138)."""
     return [f.name for f in schema.file_fields()]
@@ -81,27 +109,42 @@ def file_column_names(schema: KeyValueSchema) -> List[str]:
 
 class KeyValueDataFileWriter:
     """Encodes rows [row0, row0 + n_rows) of a device batch (a merge handle holding a batch, or a run handle) as
-    one Parquet data file and returns its DataFileMeta.  `compression` names the page codec ('none' or 'zstd', compressed
-    on the device; the other Parquet codecs are refused by the library), `zstd_level` is file.compression.zstd-level."""
+    one data file of `file_format` ('parquet' or 'orc') and returns its DataFileMeta.  `compression` names the codec
+    ('none' or 'zstd', compressed on the device; the library refuses the others), `zstd_level` is
+    file.compression.zstd-level.  Parquet takes `row_group_rows` / `page_rows`, ORC `stripe_rows` /
+    `compression_block_size` and writes the logical types of the schema (OrcTypeUtil.convertToOrcType)."""
 
     def __init__(self, schema: KeyValueSchema, path: str, level: int, file_io: Optional[LocalFileIO] = None,
-                 row_group_rows: int = 0, page_rows: int = 0, compression: str = "none", zstd_level: int = 1):
+                 row_group_rows: int = 0, page_rows: int = 0, compression: str = "none", zstd_level: int = 1,
+                 file_format: str = "parquet", stripe_rows: int = 0, compression_block_size: int = 0):
         self.schema = schema
         self.path = path
         self.level = level
         self.file_io = file_io or LocalFileIO()
-        self.opts = N.PgParquetWriteOptions(row_group_rows, page_rows)
-        self.lib = N.load()
-        if compression.lower() not in PARQUET_CODECS:
-            raise ValueError(f"unknown file compression {compression!r}")
-        self.codec = PARQUET_CODECS[compression.lower()]
+        self.file_format = file_format.lower()
+        if self.file_format not in FILE_FORMATS:
+            raise N.UnsupportedOnDevice(2, f"file format '{file_format}' is not written on the device (parquet and orc are)")
+        codecs = ORC_CODECS if self.file_format == "orc" else PARQUET_CODECS
+        if compression.lower() not in codecs:
+            raise ValueError(f"unknown {self.file_format} file compression {compression!r}")
+        self.codec = codecs[compression.lower()]
         self.zstd_level = int(zstd_level)
+        self.opts = N.PgParquetWriteOptions(row_group_rows, page_rows)
+        if self.file_format == "orc":
+            fields = schema.file_fields()
+            self._orc_types = (N.PgOrcColumnType * len(fields))(*[N.PgOrcColumnType(*orc_column_type(f.type))
+                                                                   for f in fields])
+            self.orc_opts = N.PgOrcWriteOptions(stripe_rows, self.codec, self.zstd_level, compression_block_size,
+                                                self._orc_types)
+        self.lib = N.load()
 
     def write(self, source_handle: int, row0: int = 0, n_rows: int = -1) -> WrittenFile:
         names = file_column_names(self.schema)
         arr = (C.c_char_p * len(names))(*[n.encode() for n in names])
         fh = C.c_uint64(0)
-        if self.codec == 0:
+        if self.file_format == "orc":
+            N.check(self.lib.pg_orc_encode(source_handle, arr, row0, n_rows, C.byref(self.orc_opts), C.byref(fh)))
+        elif self.codec == 0:
             N.check(self.lib.pg_parquet_encode(source_handle, arr, row0, n_rows, C.byref(self.opts), C.byref(fh)))
         else:
             N.check(self.lib.pg_parquet_encode_compressed(source_handle, arr, row0, n_rows, C.byref(self.opts),
@@ -164,11 +207,12 @@ class RollingFileWriter:
         self.file_io = file_io
         self.prefix = prefix
         self.writer_args = writer_args
+        self.suffix = writer_args.get("file_format", "parquet").lower()
         self.results: List[WrittenFile] = []
 
     def write(self, source_handle: int, n_rows: int) -> List[WrittenFile]:
         for i, r0 in enumerate(range(0, n_rows, self.target)):
-            path = os.path.join(self.directory, f"{self.prefix}-{len(self.results)}.parquet")
+            path = os.path.join(self.directory, f"{self.prefix}-{len(self.results)}.{self.suffix}")
             w = KeyValueDataFileWriter(self.schema, path, self.level, self.file_io, **self.writer_args)
             self.results.append(w.write(source_handle, r0, min(self.target, n_rows - r0)))
         return self.results
@@ -184,8 +228,9 @@ class CompactResult:
 class MergeTreeCompactRewriter:
     """rewriteCompaction(outputLevel, dropDelete, sections): every section is merged on the device, the merged
     batch never leaves HBM before it is encoded (MergeTreeCompactRewriter.java:78-116).  With `options` (table
-    options), the page codec of the files written at the output level is compression_for_level(options, level);
-    without, the files are uncompressed."""
+    options), the files written at the output level take the format format_for_level(options, level) and, for
+    parquet, the codec compression_for_level(options, level), for orc orc_compression_for_level(options, level);
+    without, they are uncompressed Parquet (or the writer arguments' file_format)."""
 
     def __init__(self, schema: KeyValueSchema, mf_factory: MergeFunctionFactory, directory: str,
                  user_defined_seq_comparator=None, file_io: Optional[LocalFileIO] = None, device: int = 0,
@@ -210,7 +255,16 @@ class MergeTreeCompactRewriter:
         spec = self.mf_factory.create().with_drop_delete(drop_delete)
         writer_args = dict(self.writer_args)
         if self.options is not None:
-            writer_args["compression"], writer_args["zstd_level"] = compression_for_level(self.options, output_level)
+            fmt = format_for_level(self.options, output_level)
+            if fmt not in FILE_FORMATS:
+                raise N.UnsupportedOnDevice(2, f"file format '{fmt}' of level {output_level} is not written on the "
+                                               f"device (parquet and orc are)")
+            writer_args["file_format"] = fmt
+            if fmt == "orc":
+                (writer_args["compression"], writer_args["zstd_level"],
+                 writer_args["compression_block_size"]) = orc_compression_for_level(self.options, output_level)
+            else:
+                writer_args["compression"], writer_args["zstd_level"] = compression_for_level(self.options, output_level)
         rolling = RollingFileWriter(self.schema, self.directory, output_level, self.target_file_rows, self.file_io,
                                     prefix=f"compact-l{output_level}", **writer_args)
         for section in sections:

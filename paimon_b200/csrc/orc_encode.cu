@@ -1,0 +1,715 @@
+// orc_encode.cu — compaction output encode: a device-resident columnar batch -> one ORC data file.
+//
+// The rewrite step of parquet_encode.cu for tables whose file format at the output level is orc
+// (KeyValueFileWriterFactory.java:301-310 picks the writer per level; OrcWriterFactory drives orc-core's writer, types
+// by OrcTypeUtil.convertToOrcType).  The byte layout is the public ORC v1 specification that orc_meta.h restates:
+//   "ORC" | stripes: per column PRESENT? DATA LENGTH|SECONDARY?, stripe footer | Metadata | Footer | PostScript | len
+// No row indexes, bloom filters or dictionaries.  Stripes start at multiples of 8 rows, so a PRESENT stream's bytes are
+// the bit-reversed bytes of the validity bitmap.
+//
+// Pipeline (the launch count does not depend on the number of columns; a task = one column of one stripe):
+//   1. k_oe_count + k_pw_stats per task: non-null values, payload bytes, exact sums, true count, VARCHAR lengths; min /
+//      max / NaN / retracts.  One read-back.
+//   2. k_oe_values (phase 0): the non-null values that are run-length coded are compacted into scratch (int64 values,
+//      string lengths, decimal scales; BYTE values, BOOLEAN bits; PRESENT bytes).
+//   3. k_oe_rle_size: one thread per integer RLE v2 run (kRunValues values) or byte-RLE group (kByteGroup bytes).  One
+//      read-back; the host lays out the streams.
+//   4. k_oe_rle_write and k_oe_values (phase 1): the runs, and the streams that are the values themselves (FLOAT /
+//      DOUBLE, string bytes, DECIMAL varints) straight from the batch, at their positions in the image.
+//   5. ZSTD: every stream cut into chunks of at most the block size, every chunk one frame of k_zs_block blocks; one
+//      read-back of the frame sizes; k_oe_zs_gather places each chunk, compressed or original, behind its header.
+// The stripe footers and the file tail are written on the host (orc_meta.cc) and patched in like Parquet's footer.
+#include <math.h>
+
+#include <algorithm>
+#include <memory>
+#include <string>
+
+#include "device_utils.cuh"
+#include "encoded_file.h"
+#include "orc_encode_device.cuh"
+#include "orc_meta.h"
+#include "zstd_encode_device.cuh"
+
+namespace pg {
+
+namespace {
+
+using orc::OutType;
+
+struct OeTask {                   // one column of one stripe
+    int32_t col, kind;            // batch column, ORC kind
+    int32_t max_len, scale;       // VARCHAR(n): n, else 0; DECIMAL: the scale
+    int64_t row0, rows;           // batch rows of the stripe (row0 a multiple of 8)
+    int64_t present;              // byte scratch: the PRESENT bytes, -1 = no PRESENT stream
+    int64_t bytes;                // byte scratch: BYTE values / BOOLEAN bits, -1 = none
+    int64_t ints;                 // int64 scratch: SHORT / INT / LONG / DATE values, string lengths, decimal scales; -1
+    int64_t direct;               // image offset of a DATA stream written from the values themselves, -1 = none
+};
+constexpr int kCountWords = 6;    // per task: non-null values, payload bytes, trues, sum (lo, hi), a VARCHAR too long
+
+struct RleJob {                   // one integer RLE v2 run or one byte-RLE group
+    int64_t src;                  // first value in the int64 / byte scratch
+    int64_t dst;                  // image offset
+    int32_t n;
+    int32_t mode;                 // 0 unsigned RLE v2, 1 signed RLE v2, 2 byte RLE
+};
+
+__device__ __forceinline__ bool is_int_rle(int k) {
+    return k == orc::K_SHORT || k == orc::K_INT || k == orc::K_LONG || k == orc::K_DATE;
+}
+__device__ __forceinline__ bool is_bytes(int k) { return k == orc::K_STRING || k == orc::K_VARCHAR || k == orc::K_BINARY; }
+
+__device__ __forceinline__ __int128 shfl_xor128(__int128 v, int d) {
+    const unsigned long long lo = __shfl_xor_sync(0xffffffffu, (unsigned long long)v, d);
+    const unsigned long long hi = __shfl_xor_sync(0xffffffffu, (unsigned long long)((unsigned __int128)v >> 64), d);
+    return (__int128)(((unsigned __int128)hi << 64) | lo);
+}
+
+__global__ void __launch_bounds__(256)
+k_oe_count(const EncColumn *cols, const OeTask *tasks, int64_t *out) {
+    const OeTask t = tasks[blockIdx.x];
+    const EncColumn c = cols[t.col];
+    long long nn = 0, payload = 0, trues = 0, too_long = 0;
+    __int128 sum = 0;
+    for (int64_t i = threadIdx.x; i < t.rows; i += blockDim.x) {
+        const int64_t row = t.row0 + i;
+        if (!valid_bit(c.validity, row)) continue;
+        nn++;
+        if (c.width == 0) {
+            const int32_t s = c.offsets[row], len = c.offsets[row + 1] - s;
+            payload += len;
+            if (t.max_len) {                               // characters = UTF-8 bytes that are not continuation bytes
+                const uint8_t *p = (const uint8_t *)c.data + s;
+                int chars = 0;
+                for (int b = 0; b < len; b++) chars += (p[b] & 0xC0) != 0x80;
+                too_long |= chars > t.max_len;
+            }
+            continue;
+        }
+        const int64_t x = sext(load_fixed(c.data, c.width, row), c.width);
+        if (t.kind == orc::K_BOOLEAN) trues += x != 0;
+        else if (t.kind != orc::K_FLOAT && t.kind != orc::K_DOUBLE && t.kind != orc::K_DATE) sum += x;
+        if (t.kind == orc::K_DECIMAL) payload += orcdev::varint_size(orcdev::zigzag(x));
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        nn += __shfl_xor_sync(0xffffffffu, nn, d);
+        payload += __shfl_xor_sync(0xffffffffu, payload, d);
+        trues += __shfl_xor_sync(0xffffffffu, trues, d);
+        too_long |= __shfl_xor_sync(0xffffffffu, too_long, d);
+        sum += shfl_xor128(sum, d);
+    }
+    __shared__ long long s_w[8][4];
+    __shared__ __int128 s_sum[8];
+    const int warp = threadIdx.x >> 5;
+    if ((threadIdx.x & 31) == 0) {
+        s_w[warp][0] = nn; s_w[warp][1] = payload; s_w[warp][2] = trues; s_w[warp][3] = too_long;
+        s_sum[warp] = sum;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        long long a = 0, b = 0, e = 0, f = 0;
+        __int128 s = 0;
+        for (int w = 0; w < (int)(blockDim.x >> 5); w++) {
+            a += s_w[w][0]; b += s_w[w][1]; e += s_w[w][2]; f |= s_w[w][3];
+            s += s_sum[w];
+        }
+        int64_t *o = out + kCountWords * (int64_t)blockIdx.x;
+        o[0] = a; o[1] = b; o[2] = e;
+        o[3] = (int64_t)(uint64_t)s;
+        o[4] = (int64_t)(s >> 64);
+        o[5] = f;
+    }
+}
+
+// phase 0: PRESENT bytes and the compacted values the run-length coders read; phase 1: the DATA streams that are the
+// values themselves, at t.direct in the image.  One CTA per task; ranks and byte offsets by block-wide scans.
+__global__ void __launch_bounds__(256)
+k_oe_values(const EncColumn *cols, const OeTask *tasks, int phase, int64_t *ints, uint8_t *bytes, uint8_t *image) {
+    const OeTask t = tasks[blockIdx.x];
+    const EncColumn c = cols[t.col];
+    const int k = t.kind;
+    if (phase == 0 && t.present >= 0) {
+        const int64_t nb = (t.rows + 7) >> 3;
+        for (int64_t b = threadIdx.x; b < nb; b += blockDim.x) {
+            uint32_t v = c.validity ? c.validity[(t.row0 >> 3) + b] : 0xFFu;
+            const int64_t rem = t.rows - b * 8;
+            if (rem < 8) v &= (1u << rem) - 1;
+            bytes[t.present + b] = orcdev::bit_reverse8(v);
+        }
+    }
+    const bool work = phase == 0 ? (t.bytes >= 0 || t.ints >= 0) : t.direct >= 0;
+    if (!work) return;
+    __shared__ int ws[33];
+    int64_t base_rank = 0, base_bytes = 0;
+    for (int64_t i0 = 0; i0 < t.rows; i0 += blockDim.x) {
+        const int64_t i = i0 + threadIdx.x;
+        const int64_t row = t.row0 + i;
+        const bool v = i < t.rows && valid_bit(c.validity, row);
+        int len = 0;
+        int32_t st = 0;
+        int64_t x = 0;
+        if (v && c.width == 0) { st = c.offsets[row]; len = c.offsets[row + 1] - st; }
+        else if (v) x = sext(load_fixed(c.data, c.width, row), c.width);
+        if (phase == 1 && v && k == orc::K_DECIMAL) len = orcdev::varint_size(orcdev::zigzag(x));
+        int n_valid, n_bytes;
+        const int64_t rank = base_rank + block_scan_excl(v ? 1 : 0, ws, &n_valid);
+        const int64_t boff = base_bytes + block_scan_excl(phase == 1 ? len : 0, ws, &n_bytes);
+        if (v) {
+            if (phase == 0) {
+                if (k == orc::K_BYTE) bytes[t.bytes + rank] = (uint8_t)x;
+                else if (k == orc::K_BOOLEAN) {
+                    // bits most significant first; the scratch is zeroed, the aligned word may hold neighbouring bytes
+                    if (x) {
+                        uint8_t *byte = bytes + t.bytes + (rank >> 3);
+                        unsigned int *word = (unsigned int *)((uintptr_t)byte & ~(uintptr_t)3);
+                        atomicOr(word, 1u << ((((uintptr_t)byte & 3) << 3) + (7 - (rank & 7))));
+                    }
+                } else if (is_int_rle(k)) ints[t.ints + rank] = x;
+                else if (is_bytes(k)) ints[t.ints + rank] = len;
+                else if (k == orc::K_DECIMAL) ints[t.ints + rank] = t.scale;
+            } else {
+                uint8_t *d = image + t.direct;
+                if (k == orc::K_FLOAT) { const uint32_t u = (uint32_t)x; memcpy(d + 4 * rank, &u, 4); }
+                else if (k == orc::K_DOUBLE) { const uint64_t u = (uint64_t)x; memcpy(d + 8 * rank, &u, 8); }
+                else if (k == orc::K_DECIMAL) {
+                    orcdev::Out o{d + boff, 0};
+                    orcdev::put_varint(o, orcdev::zigzag(x));
+                } else {
+                    const uint8_t *s = (const uint8_t *)c.data + st;
+                    for (int b = 0; b < len; b++) d[boff + b] = s[b];
+                }
+            }
+        }
+        base_rank += n_valid;
+        base_bytes += n_bytes;
+    }
+}
+
+__global__ void k_oe_rle_size(const RleJob *jobs, int n, const int64_t *ints, const uint8_t *bytes, int32_t *sizes) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const RleJob r = jobs[j];
+    sizes[j] = r.mode == 2 ? orcdev::brle_size(bytes + r.src, r.n) : orcdev::rle2_plan(ints + r.src, r.n, r.mode).size;
+}
+
+__global__ void k_oe_rle_write(const RleJob *jobs, int n, const int64_t *ints, const uint8_t *bytes, uint8_t *image) {
+    const int j = blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const RleJob r = jobs[j];
+    if (r.mode == 2) orcdev::brle_write(bytes + r.src, r.n, image + r.dst);
+    else {
+        const orcdev::Rle2Plan p = orcdev::rle2_plan(ints + r.src, r.n, r.mode);
+        orcdev::rle2_write(ints + r.src, r.n, r.mode, p, image + r.dst);
+    }
+}
+
+// One CTA per zstd block: places its compression chunk at chunk_off (3-byte header, then the frame, or the original
+// bytes when the frame is not smaller: stored == raw)
+__global__ void k_oe_zs_gather(const ZsBlockJob *jobs, const ZsPage *chunks, const int2 *res, const int32_t *boff,
+                               const int64_t *chunk_off, const int64_t *stored, const uint8_t *img, const uint8_t *zout,
+                               uint8_t *file) {
+    const ZsBlockJob j = jobs[blockIdx.x];
+    const ZsPage ch = chunks[j.page];
+    const int64_t len = stored[j.page];
+    const bool original = len == ch.raw;
+    uint8_t *hdr = file + chunk_off[j.page];
+    const bool first = (int)blockIdx.x == ch.first_block;
+    if (threadIdx.x == 0 && first) {
+        const uint32_t h = (uint32_t)len << 1 | (original ? 1u : 0u);
+        hdr[0] = (uint8_t)h; hdr[1] = (uint8_t)(h >> 8); hdr[2] = (uint8_t)(h >> 16);
+    }
+    if (original) {
+        uint8_t *dst = hdr + 3 + (j.src - jobs[ch.first_block].src);
+        for (int i = threadIdx.x; i < j.n; i += blockDim.x) dst[i] = img[j.src + i];
+        return;
+    }
+    const int2 r = res[blockIdx.x];
+    uint8_t *frame = hdr + 3;
+    uint8_t *dst = frame + boff[blockIdx.x];
+    if (threadIdx.x == 0) {
+        if (first) zs::write_frame_header(frame, (uint64_t)ch.raw);
+        zs::write_block_header(dst, (int)blockIdx.x == ch.first_block + ch.n_blocks - 1, r.x,
+                               r.x == 2 ? (uint32_t)r.y : (uint32_t)j.n);
+    }
+    const uint8_t *pay = r.x == 0 ? img + j.src : zout + j.out;
+    for (int i = threadIdx.x; i < r.y; i += blockDim.x) dst[3 + i] = pay[i];
+}
+
+// ------------------------------------------------------------------ host side
+
+int default_kind(int t) {
+    switch (t) {
+        case PG_INT8: return orc::K_BYTE;
+        case PG_INT16: return orc::K_SHORT;
+        case PG_INT32: return orc::K_INT;
+        case PG_INT64: return orc::K_LONG;
+        case PG_FLOAT: return orc::K_FLOAT;
+        case PG_DOUBLE: return orc::K_DOUBLE;
+        case PG_BOOL: return orc::K_BOOLEAN;
+        case PG_STRING: return orc::K_STRING;
+        default: return orc::K_BINARY;
+    }
+}
+
+// the ORC type of every column: the caller's, checked against the physical types, or the default for each
+pg_status resolve_types(const Schema &s, const pg_orc_column_type *in, std::vector<OutType> &out) {
+    const int nc = s.n_cols();
+    out.assign(nc, OutType{});
+    for (int c = 0; c < nc; c++) {
+        const int t = s.field(c).type;
+        OutType &o = out[c];
+        if (!in) { o.kind = default_kind(t); continue; }
+        const pg_orc_column_type &x = in[c];
+        const std::string who = "orc encode: column " + std::to_string(c) + ": ";
+        if (x.kind < 0 || x.kind > orc::K_TIMESTAMP_INSTANT)
+            return fail(PG_ERR_INVALID, who + "kind " + std::to_string(x.kind) + " is not an ORC TypeKind");
+        if (x.kind == orc::K_TIMESTAMP || x.kind == orc::K_TIMESTAMP_INSTANT || x.kind == orc::K_CHAR ||
+            (x.kind >= orc::K_LIST && x.kind <= orc::K_UNION))
+            return fail(PG_ERR_UNSUPPORTED, who + "kind " + std::to_string(x.kind) +
+                                                " is not written on the device (TIMESTAMP, CHAR and nested kinds are not)");
+        bool fits;
+        switch (x.kind) {
+            case orc::K_BYTE: fits = t == PG_INT8; break;
+            case orc::K_SHORT: fits = t == PG_INT16; break;
+            case orc::K_INT: case orc::K_DATE: fits = t == PG_INT32; break;
+            case orc::K_LONG: fits = t == PG_INT64; break;
+            case orc::K_DECIMAL: fits = t == PG_INT64 && x.precision >= 1 && x.precision <= 18 && x.scale >= 0 &&
+                                        x.scale <= x.precision; break;
+            case orc::K_FLOAT: fits = t == PG_FLOAT; break;
+            case orc::K_DOUBLE: fits = t == PG_DOUBLE; break;
+            case orc::K_BOOLEAN: fits = t == PG_BOOL; break;
+            case orc::K_STRING: fits = t == PG_STRING; break;
+            case orc::K_VARCHAR: fits = t == PG_STRING && x.max_length >= 1; break;
+            default: fits = t == PG_BINARY; break;       // K_BINARY
+        }
+        if (!fits)
+            return fail(PG_ERR_INVALID, who + "kind " + std::to_string(x.kind) + " (precision " + std::to_string(x.precision) +
+                                            ", scale " + std::to_string(x.scale) + ", max_length " + std::to_string(x.max_length) +
+                                            ") does not fit physical type " + std::to_string(t));
+        o.kind = x.kind;
+        if (x.kind == orc::K_DECIMAL) { o.precision = (uint32_t)x.precision; o.scale = (uint32_t)x.scale; }
+        if (x.kind == orc::K_VARCHAR) o.max_length = (uint32_t)x.max_length;
+    }
+    return PG_OK;
+}
+
+bool is_int_kind(int k) { return k == orc::K_BYTE || k == orc::K_SHORT || k == orc::K_INT || k == orc::K_LONG; }
+bool is_bytes_kind(int k) { return k == orc::K_STRING || k == orc::K_VARCHAR || k == orc::K_BINARY; }
+bool fits_int64(__int128 v) { return v >= (__int128)INT64_MIN && v <= (__int128)INT64_MAX; }
+
+double as_double(int64_t bits) {
+    double x;
+    memcpy(&x, &bits, 8);
+    return x;
+}
+
+// the ORC statistics of a task from its counts and k_pw_stats words
+orc::ColumnStats task_stats(const OeTask &t, const int64_t *cnt, const int64_t *st) {
+    orc::ColumnStats s;
+    s.values = (uint64_t)cnt[0];
+    s.has_null = cnt[0] < t.rows;
+    if (!s.values) return s;
+    const int k = t.kind;
+    s.sum = (__int128)(((unsigned __int128)(uint64_t)cnt[4] << 64) | (uint64_t)cnt[3]);
+    if (is_int_kind(k) || k == orc::K_DATE || k == orc::K_DECIMAL) {
+        s.has_minmax = true;
+        s.imin = st[0];
+        s.imax = st[1];
+        s.has_sum = k == orc::K_DECIMAL || (is_int_kind(k) && fits_int64(s.sum));
+    } else if (k == orc::K_FLOAT || k == orc::K_DOUBLE) {
+        s.has_minmax = true;
+        if (st[4]) { s.dmin = -INFINITY; s.dmax = NAN; }
+        else { s.dmin = as_double(zero_as(st[0], -0.0)); s.dmax = as_double(zero_as(st[1], 0.0)); }
+    } else if (k == orc::K_BOOLEAN) s.trues = (uint64_t)cnt[2];
+    else s.bytes = cnt[1];
+    return s;
+}
+
+// a column's file statistics: the merge of its stripes' (a NaN anywhere gives [-Infinity, NaN])
+void merge_stats(int kind, orc::ColumnStats &f, const orc::ColumnStats &s, bool first) {
+    if (first) { f = s; return; }
+    f.values += s.values;
+    f.has_null |= s.has_null;
+    f.trues += s.trues;
+    f.bytes += s.bytes;
+    f.sum += s.sum;
+    f.has_sum = kind == orc::K_DECIMAL || (is_int_kind(kind) && fits_int64(f.sum));
+    if (!s.has_minmax) return;
+    if (!f.has_minmax) { f.has_minmax = true; f.imin = s.imin; f.imax = s.imax; f.dmin = s.dmin; f.dmax = s.dmax; return; }
+    f.imin = std::min(f.imin, s.imin);
+    f.imax = std::max(f.imax, s.imax);
+    if (isnan(f.dmax) || isnan(s.dmax)) { f.dmin = -INFINITY; f.dmax = NAN; }
+    else { f.dmin = std::min(f.dmin, s.dmin); f.dmax = std::max(f.dmax, s.dmax); }
+}
+
+struct Stream {
+    int task, kind;
+    int64_t length = 0;           // raw bytes
+    size_t job0 = 0, job1 = 0;    // its run-length jobs
+    int64_t raw_off = 0;          // offset in the raw image
+    size_t chunk0 = 0, chunk1 = 0;
+    int64_t stored = 0;           // bytes in the file
+};
+
+pg_status encode_orc(uint64_t source, const char *const *names, int64_t row0, int64_t n_rows,
+                     const pg_orc_write_options *opt, uint64_t *out_file) {
+    const int codec = opt ? opt->compression : orc::C_NONE;
+    const int level = opt ? opt->zstd_level : 1;
+    const int64_t block = opt && opt->compression_block_size > 0 ? opt->compression_block_size : 256 << 10;
+    if (codec < 0 || codec > 6)
+        return fail(PG_ERR_INVALID, "orc encode: compression " + std::to_string(codec) + " is not an ORC CompressionKind");
+    if (codec != orc::C_NONE && codec != orc::C_ZSTD)
+        return fail(PG_ERR_UNSUPPORTED, "orc encode: compression " + std::to_string(codec) +
+                                            " is not written on the device (NONE and ZSTD are)");
+    if (codec == orc::C_ZSTD && (level == 0 || level > 1))
+        return fail(PG_ERR_UNSUPPORTED, "orc encode: zstd level " + std::to_string(level) +
+                                            " is not written on the device (level 1 and the negative fast levels are)");
+    if (opt && (opt->compression_block_size < 0 || opt->compression_block_size >= ((int64_t)1 << 23)))
+        return fail(PG_ERR_INVALID, "orc encode: compression block size " + std::to_string(opt->compression_block_size) +
+                                        " outside [0, 2^23) (a chunk header holds 23 bits of length)");
+    pg_status st = ensure_device();
+    if (st) return st;
+    BatchColumns batch;                                      // held until the encode below is done
+    if ((st = batch_columns(source, &batch))) return st;
+    const Schema *s = batch.schema.get();
+    const std::vector<DevColumn> &dcols = batch.cols;
+    for (int c = 0; c < s->n_cols() && batch.n_rows > 0; c++)
+        if (!dcols[c].data && !dcols[c].offsets)
+            return fail(PG_ERR_INVALID, "orc encode: the batch was produced under a read-type projection and has no "
+                                        "column " + std::to_string(c) + "; a data file needs every column");
+    if (n_rows < 0) n_rows = batch.n_rows - row0;
+    if (row0 < 0 || (row0 & 7) || row0 + n_rows > batch.n_rows)
+        return fail(PG_ERR_INVALID, "orc encode: row range outside the batch or not starting at a multiple of 8");
+    const int nc = s->n_cols();
+    std::vector<OutType> types;
+    if ((st = resolve_types(*s, opt ? opt->types : nullptr, types))) return st;
+
+    SectionTimer tm;
+    PG_CUDA(cudaEventCreate(&tm.e0));
+    PG_CUDA(cudaEventCreate(&tm.e1));
+    PG_CUDA(cudaEventRecord(tm.e0, 0));
+
+    // ---- tasks: stripe major, then column
+    int64_t stripe_rows = opt && opt->stripe_rows > 0 ? opt->stripe_rows : (int64_t)1 << 20;
+    stripe_rows = (stripe_rows + 7) & ~(int64_t)7;
+    const int64_t n_stripes = n_rows == 0 ? 0 : (n_rows + stripe_rows - 1) / stripe_rows;
+    std::vector<EncColumn> cols;
+    for (int c = 0; c < nc; c++) {
+        const pg_field f = s->field(c);
+        cols.push_back(EncColumn{dcols[c].data, dcols[c].offsets, dcols[c].validity, f.type, type_width(f.type), 1, 0});
+    }
+    std::vector<OeTask> tasks;
+    std::vector<StatJob> sjobs;
+    for (int64_t g = 0; g < n_stripes; g++) {
+        const int64_t g0 = row0 + g * stripe_rows, g1 = std::min(row0 + n_rows, g0 + stripe_rows);
+        for (int c = 0; c < nc; c++) {
+            tasks.push_back(OeTask{c, types[c].kind, (int32_t)types[c].max_length, (int32_t)types[c].scale, g0, g1 - g0,
+                                   -1, -1, -1, -1});
+            sjobs.push_back(StatJob{c, 0, g0, g1 - g0});
+        }
+    }
+    const size_t nt = tasks.size();
+    Scratch scratch(0);                                      // temporaries, released on every path out of this function
+    EncColumn *d_cols = (EncColumn *)scratch.take(sizeof(EncColumn) * nc);
+    OeTask *d_tasks = (OeTask *)scratch.take(sizeof(OeTask) * std::max<size_t>(nt, 1));
+    StatJob *d_sjobs = (StatJob *)scratch.take(sizeof(StatJob) * std::max<size_t>(nt, 1));
+    int64_t *d_counts = (int64_t *)scratch.take(sizeof(int64_t) * kCountWords * (nt + 1));
+    int64_t *d_stats = (int64_t *)scratch.take(sizeof(int64_t) * kStatWords * (nt + 1));
+    if (!d_cols || !d_tasks || !d_sjobs || !d_counts || !d_stats)
+        return fail(PG_ERR_CUDA, "orc encode: out of device memory for the task tables");
+    PG_CUDA(cudaMemcpy(d_cols, cols.data(), sizeof(EncColumn) * nc, cudaMemcpyHostToDevice));
+    int launches = 0;
+    std::vector<int64_t> counts(kCountWords * (nt + 1)), stats(kStatWords * (nt + 1));
+    if (nt) {
+        PG_CUDA(cudaMemcpy(d_tasks, tasks.data(), sizeof(OeTask) * nt, cudaMemcpyHostToDevice));
+        PG_CUDA(cudaMemcpy(d_sjobs, sjobs.data(), sizeof(StatJob) * nt, cudaMemcpyHostToDevice));
+        k_oe_count<<<(unsigned)nt, 256>>>(d_cols, d_tasks, d_counts);
+        launch_pw_stats(d_cols, d_sjobs, (int)nt, d_stats);
+        launches += 2;
+        SmallReads rd(0);
+        if ((st = rd.add(counts.data(), d_counts, sizeof(int64_t) * kCountWords * nt))) return st;
+        if ((st = rd.add(stats.data(), d_stats, sizeof(int64_t) * kStatWords * nt))) return st;
+        launches++;
+        if ((st = rd.finish())) return st;
+    }
+
+    // ---- statistics, scratch slots, streams and their run-length jobs
+    auto ef = std::make_unique<EncodedFile>();
+    std::vector<orc::ColumnStats> file_stats(nc + 1);
+    file_stats[0].values = (uint64_t)n_rows;
+    std::vector<orc::OutStripe> stripes(n_stripes);
+    std::vector<char> file_nan(nc, 0);
+    std::vector<ColStats> &cs = ef->stats;
+    cs.assign(nc, ColStats{INT64_MAX, INT64_MIN, 0, 0});
+    std::vector<Stream> streams;
+    std::vector<RleJob> jobs;
+    int64_t n_ints = 0, n_bytes = 0;
+    auto add_runs = [&](Stream &sm, int64_t src, int64_t n, int mode) {
+        const int per = mode == 2 ? orcdev::kByteGroup : orcdev::kRunValues;
+        sm.job0 = jobs.size();
+        for (int64_t i = 0; i < n; i += per) jobs.push_back(RleJob{src + i, 0, (int32_t)std::min<int64_t>(per, n - i), mode});
+        sm.job1 = jobs.size();
+    };
+    for (size_t i = 0; i < nt; i++) {
+        OeTask &t = tasks[i];
+        const int64_t *cnt = &counts[kCountWords * i], *sw = &stats[kStatWords * i];
+        if (cnt[5])
+            return fail(PG_ERR_UNSUPPORTED, "orc encode: column " + std::to_string(t.col) + " holds a value longer than its "
+                                            "VARCHAR(" + std::to_string(t.max_len) + ") (orc-core would truncate it)");
+        const int64_t g = (int64_t)(i / nc), nn = cnt[0];
+        orc::OutStripe &sp = stripes[g];
+        if (sp.stats.empty()) {
+            sp.stats.resize(nc + 1);
+            sp.stats[0].values = (uint64_t)t.rows;
+            sp.rows = (uint64_t)t.rows;
+        }
+        sp.stats[t.col + 1] = task_stats(t, cnt, sw);
+        merge_stats(t.kind, file_stats[t.col + 1], sp.stats[t.col + 1], g == 0);
+        // the accessor's statistics: those of the Parquet output
+        ColStats &f = cs[t.col];
+        f.null_count += t.rows - nn;
+        const bool fp = t.kind == orc::K_FLOAT || t.kind == orc::K_DOUBLE;
+        file_nan[t.col] |= sw[4] != 0;
+        if (cols[t.col].width > 0 && nn > 0 && !sw[4]) {
+            int64_t mn = sw[0], mx = sw[1];
+            if (fp) { mn = zero_as(mn, -0.0); mx = zero_as(mx, 0.0); }
+            if (!f.has_minmax) { f.min = mn; f.max = mx; f.has_minmax = 1; }
+            else if (fp) {
+                const double a = std::min(as_double(f.min), as_double(mn)), b = std::max(as_double(f.max), as_double(mx));
+                memcpy(&f.min, &a, 8); memcpy(&f.max, &b, 8);
+            } else { f.min = std::min(f.min, mn); f.max = std::max(f.max, mx); }
+        }
+        if (t.col == s->n_key + 1) ef->meta.delete_row_count += sw[3];
+
+        if (nn < t.rows) {
+            Stream sm{(int)i, orc::S_PRESENT};
+            t.present = n_bytes;
+            add_runs(sm, n_bytes, (t.rows + 7) / 8, 2);
+            n_bytes += (t.rows + 7) / 8;
+            streams.push_back(sm);
+        }
+        Stream data{(int)i, orc::S_DATA};
+        const int k = t.kind;
+        if (k == orc::K_BYTE) { t.bytes = n_bytes; add_runs(data, n_bytes, nn, 2); n_bytes += nn; }
+        else if (k == orc::K_BOOLEAN) {
+            t.bytes = n_bytes;
+            add_runs(data, n_bytes, (nn + 7) / 8, 2);
+            n_bytes += (nn + 7) / 8;
+        } else if (k == orc::K_SHORT || k == orc::K_INT || k == orc::K_LONG || k == orc::K_DATE) {
+            t.ints = n_ints;
+            add_runs(data, n_ints, nn, 1);
+            n_ints += nn;
+        } else if (k == orc::K_FLOAT) data.length = 4 * nn;
+        else if (k == orc::K_DOUBLE) data.length = 8 * nn;
+        else data.length = cnt[1];                          // string bytes, decimal varints
+        streams.push_back(data);
+        if (is_bytes_kind(k) || k == orc::K_DECIMAL) {
+            Stream second{(int)i, is_bytes_kind(k) ? orc::S_LENGTH : orc::S_SECONDARY};
+            t.ints = n_ints;
+            add_runs(second, n_ints, nn, is_bytes_kind(k) ? 0 : 1);
+            n_ints += nn;
+            streams.push_back(second);
+        }
+    }
+    for (int c = 0; c < nc; c++)
+        if (file_nan[c]) cs[c] = ColStats{INT64_MAX, INT64_MIN, cs[c].null_count, 0};
+    const ColStats &sq = cs[s->n_key];
+    ef->meta.min_sequence_number = sq.has_minmax ? sq.min : 0;
+    ef->meta.max_sequence_number = sq.has_minmax ? sq.max : 0;
+
+    // ---- compaction and run sizes
+    const size_t nj = jobs.size();
+    int64_t *d_ints = (int64_t *)scratch.take(sizeof(int64_t) * (size_t)n_ints + 64);
+    uint8_t *d_bytes = (uint8_t *)scratch.take((size_t)n_bytes + 64);
+    RleJob *d_jobs = (RleJob *)scratch.take(sizeof(RleJob) * std::max<size_t>(nj, 1));
+    int32_t *d_sizes = (int32_t *)scratch.take(sizeof(int32_t) * std::max<size_t>(nj, 1));
+    if (!d_ints || !d_bytes || !d_jobs || !d_sizes) return fail(PG_ERR_CUDA, "orc encode: out of device memory for the run scratch");
+    std::vector<int32_t> sizes(nj);
+    if (nt) {
+        PG_CUDA(cudaMemsetAsync(d_bytes, 0, (size_t)n_bytes + 64, 0));
+        PG_CUDA(cudaMemcpy(d_tasks, tasks.data(), sizeof(OeTask) * nt, cudaMemcpyHostToDevice));
+        k_oe_values<<<(unsigned)nt, 256>>>(d_cols, d_tasks, 0, d_ints, d_bytes, nullptr);
+        launches++;
+    }
+    if (nj) {
+        PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(RleJob) * nj, cudaMemcpyHostToDevice));
+        k_oe_rle_size<<<(unsigned)((nj + 127) / 128), 128>>>(d_jobs, (int)nj, d_ints, d_bytes, d_sizes);
+        launches++;
+        SmallReads rd(0);
+        if ((st = rd.add(sizes.data(), d_sizes, sizeof(int32_t) * nj))) return st;
+        launches++;
+        if ((st = rd.finish())) return st;
+    }
+    for (Stream &sm : streams)
+        for (size_t j = sm.job0; j < sm.job1; j++) sm.length += sizes[j];
+
+    // ---- the raw streams: contiguous for ZSTD (a scratch image), at their file offsets for NONE (the file image)
+    const bool zstd = codec == orc::C_ZSTD;
+    std::vector<uint8_t> magic = {'O', 'R', 'C'};
+    ef->host_parts.push_back({0, magic});
+    std::vector<int> encodings(nc + 1, orc::E_DIRECT);
+    for (int c = 0; c < nc; c++) {
+        const int k = types[c].kind;
+        if (k != orc::K_BYTE && k != orc::K_BOOLEAN && k != orc::K_FLOAT && k != orc::K_DOUBLE) encodings[c + 1] = orc::E_DIRECT_V2;
+    }
+    // lays out the stripes from the streams' stored sizes: offsets, stripe footers, the tail
+    auto layout = [&](std::vector<int64_t> &stream_off) -> pg_status {
+        int64_t pos = 3;
+        size_t si = 0;
+        stream_off.assign(streams.size(), 0);
+        for (int64_t g = 0; g < n_stripes; g++) {
+            orc::OutStripe &sp = stripes[g];
+            sp.offset = (uint64_t)pos;
+            std::vector<orc::OutStream> list;
+            for (; si < streams.size() && streams[si].task / nc == g; si++) {
+                stream_off[si] = pos;
+                pos += streams[si].stored;
+                list.push_back(orc::OutStream{streams[si].kind, (uint32_t)(tasks[streams[si].task].col + 1),
+                                              (uint64_t)streams[si].stored});
+            }
+            sp.data_length = (uint64_t)pos - sp.offset;
+            std::vector<uint8_t> foot;
+            try {
+                foot = orc::compress_section(orc::stripe_footer(list, encodings), codec, (uint64_t)block);
+            } catch (const std::exception &e) { return fail(PG_ERR_INVALID, std::string("orc encode: ") + e.what()); }
+            sp.footer_length = foot.size();
+            ef->host_parts.push_back({pos, std::move(foot)});
+            pos += (int64_t)sp.footer_length;
+        }
+        ef->data_end = pos;
+        std::vector<std::string> col_names(nc);
+        for (int c = 0; c < nc; c++) col_names[c] = names && names[c] ? names[c] : "c" + std::to_string(c);
+        try {
+            ef->host_parts.push_back({pos, orc::file_tail(types, col_names, stripes, file_stats, (uint64_t)n_rows,
+                                                          (uint64_t)pos, codec, (uint64_t)block)});
+        } catch (const std::exception &e) { return fail(PG_ERR_INVALID, std::string("orc encode: ") + e.what()); }
+        ef->file_bytes = pos + (int64_t)ef->host_parts.back().second.size();
+        return PG_OK;
+    };
+    std::vector<int64_t> stream_off;
+    int64_t raw_bytes = 0;
+    if (zstd) {
+        for (Stream &sm : streams) { sm.raw_off = raw_bytes; raw_bytes += sm.length; }
+    } else {
+        for (Stream &sm : streams) sm.stored = sm.length;
+        if ((st = layout(stream_off))) return st;
+        for (size_t i = 0; i < streams.size(); i++) streams[i].raw_off = stream_off[i];
+    }
+    for (Stream &sm : streams) {
+        int64_t at = sm.raw_off;
+        for (size_t j = sm.job0; j < sm.job1; j++) { jobs[j].dst = at; at += sizes[j]; }
+        const int k = tasks[sm.task].kind;
+        if (sm.kind == orc::S_DATA && (k == orc::K_FLOAT || k == orc::K_DOUBLE || k == orc::K_DECIMAL || is_bytes_kind(k)))
+            tasks[sm.task].direct = sm.raw_off;
+    }
+    uint8_t *d_raw = nullptr;
+    if (zstd) d_raw = (uint8_t *)scratch.take((size_t)raw_bytes + 64);
+    else {
+        PG_CUDA(cudaMalloc(&ef->d_file, (size_t)ef->file_bytes + 64));
+        PG_CUDA(cudaMemsetAsync(ef->d_file, 0, (size_t)ef->file_bytes + 64, 0));
+        d_raw = ef->d_file;
+    }
+    if (!d_raw) return fail(PG_ERR_CUDA, "orc encode: out of device memory for the stream image");
+    if (nj) {
+        PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(RleJob) * nj, cudaMemcpyHostToDevice));
+        k_oe_rle_write<<<(unsigned)((nj + 127) / 128), 128>>>(d_jobs, (int)nj, d_ints, d_bytes, d_raw);
+        launches++;
+    }
+    if (nt) {
+        PG_CUDA(cudaMemcpy(d_tasks, tasks.data(), sizeof(OeTask) * nt, cudaMemcpyHostToDevice));
+        k_oe_values<<<(unsigned)nt, 256>>>(d_cols, d_tasks, 1, d_ints, d_bytes, d_raw);
+        launches++;
+    }
+
+    // ---- ZSTD: chunks of at most `block` bytes, one frame each; sizes back; layout; the chunks placed
+    if (zstd) {
+        std::vector<ZsPage> chunks;
+        std::vector<ZsBlockJob> bjobs;
+        int64_t out = 0, seq = 0;
+        for (Stream &sm : streams) {
+            sm.chunk0 = chunks.size();
+            for (int64_t c0 = 0; c0 < sm.length; c0 += block) {
+                const int64_t cn = std::min<int64_t>(block, sm.length - c0);
+                ZsPage ch{cn, (int32_t)bjobs.size(), 0};
+                for (int64_t b0 = 0; b0 < cn; b0 += zs::kMaxBlock) {
+                    const int32_t n = (int32_t)std::min<int64_t>(zs::kMaxBlock, cn - b0);
+                    bjobs.push_back(ZsBlockJob{sm.raw_off + c0 + b0, out, seq, n, (int32_t)chunks.size()});
+                    out += n;
+                    seq += n / 4 + 1;
+                    ch.n_blocks++;
+                }
+                chunks.push_back(ch);
+            }
+            sm.chunk1 = chunks.size();
+        }
+        const size_t nch = chunks.size(), nb = bjobs.size();
+        std::vector<int64_t> frame(nch), stored(nch), chunk_off(nch);
+        ZsBlockJob *d_bjobs = (ZsBlockJob *)scratch.take(sizeof(ZsBlockJob) * std::max<size_t>(nb, 1));
+        ZsPage *d_chunks = (ZsPage *)scratch.take(sizeof(ZsPage) * std::max<size_t>(nch, 1));
+        int2 *d_res = (int2 *)scratch.take(sizeof(int2) * std::max<size_t>(nb, 1));
+        int32_t *d_boff = (int32_t *)scratch.take(sizeof(int32_t) * std::max<size_t>(nb, 1));
+        int64_t *d_frame = (int64_t *)scratch.take(sizeof(int64_t) * std::max<size_t>(nch, 1));
+        int64_t *d_stored = (int64_t *)scratch.take(sizeof(int64_t) * std::max<size_t>(nch, 1));
+        uint8_t *d_zout = (uint8_t *)scratch.take((size_t)out + 64);
+        uint8_t *d_lits = (uint8_t *)scratch.take((size_t)raw_bytes + 64);
+        void *d_seqs = scratch.take(zs_seq_bytes(seq) + 64);
+        if (!d_bjobs || !d_chunks || !d_res || !d_boff || !d_frame || !d_stored || !d_zout || !d_lits || !d_seqs)
+            return fail(PG_ERR_CUDA, "orc encode: out of device memory for the zstd chunks");
+        if (nb) {
+            PG_CUDA(cudaMemcpy(d_bjobs, bjobs.data(), sizeof(ZsBlockJob) * nb, cudaMemcpyHostToDevice));
+            PG_CUDA(cudaMemcpy(d_chunks, chunks.data(), sizeof(ZsPage) * nch, cudaMemcpyHostToDevice));
+            launch_zs_compress(d_bjobs, (int)nb, d_chunks, (int)nch, d_raw, d_zout, d_seqs, d_lits, d_res, d_boff, d_frame);
+            launches += 2;
+            SmallReads rd(0);
+            if ((st = rd.add(frame.data(), d_frame, sizeof(int64_t) * nch))) return st;
+            launches++;
+            if ((st = rd.finish())) return st;
+        }
+        for (Stream &sm : streams) {
+            sm.stored = 0;
+            for (size_t c = sm.chunk0; c < sm.chunk1; c++) {
+                stored[c] = frame[c] < chunks[c].raw ? frame[c] : chunks[c].raw;
+                sm.stored += 3 + stored[c];
+            }
+        }
+        if ((st = layout(stream_off))) return st;
+        for (size_t i = 0; i < streams.size(); i++) {
+            int64_t at = stream_off[i];
+            for (size_t c = streams[i].chunk0; c < streams[i].chunk1; c++) { chunk_off[c] = at; at += 3 + stored[c]; }
+        }
+        PG_CUDA(cudaMalloc(&ef->d_file, (size_t)ef->file_bytes + 64));
+        PG_CUDA(cudaMemsetAsync(ef->d_file, 0, (size_t)ef->file_bytes + 64, 0));
+        if (nb) {
+            PG_CUDA(cudaMemcpy(d_frame, chunk_off.data(), sizeof(int64_t) * nch, cudaMemcpyHostToDevice));
+            PG_CUDA(cudaMemcpy(d_stored, stored.data(), sizeof(int64_t) * nch, cudaMemcpyHostToDevice));
+            k_oe_zs_gather<<<(unsigned)nb, 256>>>(d_bjobs, d_chunks, d_res, d_boff, d_frame, d_stored, d_raw, d_zout, ef->d_file);
+            launches++;
+        }
+    }
+    PG_CUDA(cudaEventRecord(tm.e1, 0));
+    PG_CUDA(cudaEventSynchronize(tm.e1));
+    const float ms = tm.ms();
+    cudaError_t le = cudaGetLastError();
+    if (le != cudaSuccess) return fail(PG_ERR_CUDA, std::string("orc encode: ") + cudaGetErrorString(le));
+
+    ef->meta.n_rows = n_rows;
+    ef->meta.file_bytes = ef->file_bytes;
+    ef->meta.n_row_groups = (int32_t)n_stripes;
+    ef->meta.n_pages = (int32_t)streams.size();
+    ef->meta.ms_encode = ms;
+    ef->meta.launches = launches;
+    *out_file = g_enc.put(std::move(ef));
+    return PG_OK;
+}
+
+}  // namespace
+
+}  // namespace pg
+
+extern "C" pg_status pg_orc_encode(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
+                                   const pg_orc_write_options *options, uint64_t *out_file) {
+    if (!out_file) return pg::fail(PG_ERR_INVALID, "null argument");
+    return pg::encode_orc(source, column_names, row0, n_rows, options, out_file);
+}

@@ -1,11 +1,15 @@
 // orc_meta.cc — protobuf wire reader + ORC file tail / stripe footers (see orc_meta.h).
 #include "orc_meta.h"
 
+#include <string.h>
+
 #include <algorithm>
+#include <memory>
 #include <stdexcept>
 
 #include "inflate_device.cuh"
 #include "zstd_device.cuh"
+#include "zstd_encode_device.cuh"
 
 namespace orc {
 
@@ -267,6 +271,187 @@ Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::
         row0 += (int64_t)t.stripes[si].rows;
     }
     return pl;
+}
+
+// ---------------------------------------------------------------- writer
+
+void PbWriter::varint(uint64_t v) {
+    while (v >= 0x80) { b.push_back((uint8_t)(v | 0x80)); v >>= 7; }
+    b.push_back((uint8_t)v);
+}
+void PbWriter::f64(uint32_t field, double v) {
+    key(field, 1);
+    uint8_t x[8];
+    memcpy(x, &v, 8);
+    b.insert(b.end(), x, x + 8);
+}
+void PbWriter::bytes(uint32_t field, const void *p, size_t n) {
+    key(field, 2);
+    varint(n);
+    b.insert(b.end(), (const uint8_t *)p, (const uint8_t *)p + n);
+}
+
+std::string decimal_string(__int128 v, int scale) {
+    const bool neg = v < 0;
+    unsigned __int128 u = neg ? (unsigned __int128)0 - (unsigned __int128)v : (unsigned __int128)v;
+    std::string digits;
+    do { digits.insert(digits.begin(), (char)('0' + (int)(u % 10))); u /= 10; } while (u);
+    if (scale > 0) {
+        if ((int)digits.size() <= scale) digits.insert(digits.begin(), (size_t)(scale + 1 - digits.size()), '0');
+        digits.insert(digits.end() - scale, '.');
+    }
+    return neg ? "-" + digits : digits;
+}
+
+std::vector<uint8_t> column_statistics(const OutType &t, const ColumnStats &s) {
+    PbWriter w;
+    w.u64(1, s.values);
+    if (s.values > 0) {
+        PbWriter m;
+        switch (t.kind) {
+            case K_BYTE: case K_SHORT: case K_INT: case K_LONG:
+                if (s.has_minmax) { m.s64(1, s.imin); m.s64(2, s.imax); }
+                if (s.has_sum) m.s64(3, (int64_t)s.sum);
+                w.msg(2, m);
+                break;
+            case K_FLOAT: case K_DOUBLE:
+                if (s.has_minmax) { m.f64(1, s.dmin); m.f64(2, s.dmax); }
+                w.msg(3, m);
+                break;
+            case K_STRING: case K_VARCHAR:
+                m.s64(3, s.bytes);
+                w.msg(4, m);
+                break;
+            case K_BOOLEAN: {
+                PbWriter packed;
+                packed.varint(s.trues);
+                m.bytes(1, packed.b.data(), packed.b.size());
+                w.msg(5, m);
+                break;
+            }
+            case K_DECIMAL:
+                if (s.has_minmax) { m.str(1, decimal_string(s.imin, (int)t.scale)); m.str(2, decimal_string(s.imax, (int)t.scale)); }
+                if (s.has_sum) m.str(3, decimal_string(s.sum, (int)t.scale));
+                w.msg(6, m);
+                break;
+            case K_DATE:
+                if (s.has_minmax) { m.s64(1, s.imin); m.s64(2, s.imax); }
+                w.msg(7, m);
+                break;
+            case K_BINARY:
+                m.s64(1, s.bytes);
+                w.msg(8, m);
+                break;
+            default:
+                break;                                   // the root struct: the counts only
+        }
+    }
+    w.u64(10, s.has_null ? 1 : 0);
+    return std::move(w.b);
+}
+
+std::vector<uint8_t> stripe_footer(const std::vector<OutStream> &streams, const std::vector<int> &encodings) {
+    PbWriter w;
+    for (const OutStream &s : streams) {
+        PbWriter m;
+        m.u64(1, (uint64_t)s.kind);
+        m.u64(2, s.column);
+        m.u64(3, s.length);
+        w.msg(1, m);
+    }
+    for (int e : encodings) {
+        PbWriter m;
+        m.u64(1, (uint64_t)e);
+        w.msg(2, m);
+    }
+    return std::move(w.b);
+}
+
+std::vector<uint8_t> compress_section(const std::vector<uint8_t> &raw, int codec, uint64_t block_size) {
+    if (codec == C_NONE) return raw;
+    if (codec != C_ZSTD) throw std::runtime_error("orc: compression kind " + std::to_string(codec) + " is not written");
+    std::vector<int32_t> htab((size_t)1 << zs::kHashLog);
+    std::vector<zs::Seq> seqs(zs::kMaxBlock / 4 + 1);
+    std::vector<uint8_t> lits(zs::kMaxBlock), blk(zs::kMaxBlock), frame;
+    std::unique_ptr<zs::EncWork> W(new zs::EncWork());
+    std::vector<uint8_t> out;
+    for (size_t pos = 0; pos < raw.size(); pos += block_size) {
+        const size_t n = std::min<size_t>(block_size, raw.size() - pos);
+        frame.resize((size_t)zs::frame_bound((int64_t)n));
+        const int64_t f = zs::compress_frame(raw.data() + pos, (int64_t)n, frame.data(), (int64_t)frame.size(), htab.data(),
+                                             seqs.data(), lits.data(), blk.data(), *W);
+        const bool original = f < 0 || (uint64_t)f >= n;
+        const uint32_t len = original ? (uint32_t)n : (uint32_t)f;
+        const uint32_t h = len << 1 | (original ? 1u : 0u);
+        out.push_back((uint8_t)h); out.push_back((uint8_t)(h >> 8)); out.push_back((uint8_t)(h >> 16));
+        if (original) out.insert(out.end(), raw.begin() + pos, raw.begin() + pos + n);
+        else out.insert(out.end(), frame.begin(), frame.begin() + f);
+    }
+    return out;
+}
+
+std::vector<uint8_t> file_tail(const std::vector<OutType> &types, const std::vector<std::string> &names,
+                               const std::vector<OutStripe> &stripes, const std::vector<ColumnStats> &file_stats,
+                               uint64_t rows, uint64_t content_length, int codec, uint64_t block_size) {
+    std::vector<OutType> all(1);
+    all[0].kind = K_STRUCT;
+    all.insert(all.end(), types.begin(), types.end());
+    PbWriter meta;                                       // Metadata: per stripe, the statistics of every column
+    for (const OutStripe &s : stripes) {
+        PbWriter ss;
+        for (size_t c = 0; c < all.size(); c++) {
+            const std::vector<uint8_t> cs = column_statistics(all[c], s.stats[c]);
+            ss.bytes(1, cs.data(), cs.size());
+        }
+        meta.msg(1, ss);
+    }
+    PbWriter f;                                          // Footer
+    f.u64(1, 3);
+    f.u64(2, content_length);
+    for (const OutStripe &s : stripes) {
+        PbWriter m;
+        m.u64(1, s.offset);
+        m.u64(2, 0);
+        m.u64(3, s.data_length);
+        m.u64(4, s.footer_length);
+        m.u64(5, s.rows);
+        f.msg(3, m);
+    }
+    for (size_t c = 0; c < all.size(); c++) {
+        PbWriter m;
+        m.u64(1, (uint64_t)all[c].kind);
+        if (c == 0) {
+            PbWriter sub;
+            for (size_t k = 1; k < all.size(); k++) sub.varint(k);
+            m.bytes(2, sub.b.data(), sub.b.size());
+            for (const std::string &n : names) m.str(3, n);
+        }
+        if (all[c].kind == K_VARCHAR) m.u64(4, all[c].max_length);
+        if (all[c].kind == K_DECIMAL) { m.u64(5, all[c].precision); m.u64(6, all[c].scale); }
+        f.msg(4, m);
+    }
+    f.u64(6, rows);
+    for (size_t c = 0; c < all.size(); c++) {
+        const std::vector<uint8_t> cs = column_statistics(all[c], file_stats[c]);
+        f.bytes(7, cs.data(), cs.size());
+    }
+    f.u64(8, 0);                                         // rowIndexStride: no row indexes
+    const std::vector<uint8_t> meta_c = compress_section(meta.b, codec, block_size);
+    const std::vector<uint8_t> foot_c = compress_section(f.b, codec, block_size);
+    PbWriter ps;                                         // PostScript
+    ps.u64(1, foot_c.size());
+    ps.u64(2, (uint64_t)codec);
+    ps.u64(3, block_size);
+    const uint8_t version[2] = {0, 12};
+    ps.bytes(4, version, 2);
+    ps.u64(5, meta_c.size());
+    ps.u64(6, 9);                                        // writerVersion ORC_14
+    ps.str(8000, "ORC");
+    std::vector<uint8_t> out = meta_c;
+    out.insert(out.end(), foot_c.begin(), foot_c.end());
+    out.insert(out.end(), ps.b.begin(), ps.b.end());
+    out.push_back((uint8_t)ps.b.size());
+    return out;
 }
 
 }  // namespace orc

@@ -81,4 +81,59 @@ struct Plan {
 // file_col_of[c] = the file's column (0-based child of the root struct) for caller column c, or < 0 = skip
 Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::vector<int> &file_col_of);
 
+// ---- writer side: the stripe footers and the file tail (Metadata, Footer, PostScript, PostScript length) of a flat
+// file, written DIRECT / DIRECT_V2 without row indexes
+struct PbWriter {
+    std::vector<uint8_t> b;
+    void varint(uint64_t v);
+    void key(uint32_t field, int wire) { varint((uint64_t)field << 3 | (uint64_t)wire); }
+    void u64(uint32_t field, uint64_t v) { key(field, 0); varint(v); }
+    void s64(uint32_t field, int64_t v) { key(field, 0); varint(((uint64_t)v << 1) ^ (uint64_t)(v >> 63)); }
+    void f64(uint32_t field, double v);
+    void bytes(uint32_t field, const void *p, size_t n);
+    void str(uint32_t field, const std::string &s) { bytes(field, s.data(), s.size()); }
+    void msg(uint32_t field, const PbWriter &m) { bytes(field, m.b.data(), m.b.size()); }
+};
+
+struct OutType {
+    int kind = 0;
+    uint32_t precision = 0, scale = 0, max_length = 0;   // DECIMAL; VARCHAR
+};
+// one column of one stripe or of the file; the typed message written follows the column's kind
+struct ColumnStats {
+    uint64_t values = 0;          // non-null values
+    bool has_null = false;
+    bool has_minmax = false;      // integers, DATE, DECIMAL (unscaled), FLOAT / DOUBLE
+    int64_t imin = 0, imax = 0;
+    double dmin = 0, dmax = 0;
+    bool has_sum = false;         // integers: the exact sum fits int64; DECIMAL: always
+    __int128 sum = 0;
+    int64_t bytes = 0;            // STRING / VARCHAR / BINARY: total bytes of the values
+    uint64_t trues = 0;           // BOOLEAN
+};
+struct OutStream {
+    int kind = 0;
+    uint32_t column = 0;
+    uint64_t length = 0;
+};
+struct OutStripe {
+    uint64_t offset = 0, data_length = 0, footer_length = 0, rows = 0;
+    std::vector<ColumnStats> stats;   // [0] = the root struct
+};
+
+// an unscaled decimal as the text orc_proto's DecimalStatistics carries ("-123.45")
+std::string decimal_string(__int128 unscaled, int scale);
+// the serialized ColumnStatistics of a column of type t
+std::vector<uint8_t> column_statistics(const OutType &t, const ColumnStats &s);
+// a StripeFooter: the streams in file order, one encoding per column (root first)
+std::vector<uint8_t> stripe_footer(const std::vector<OutStream> &streams, const std::vector<int> &encodings);
+// a section stored under the file's compression: NONE = the bytes; ZSTD = chunks of at most block_size bytes, each one
+// zstd frame behind a 3-byte header, or the original bytes when the frame is not smaller
+std::vector<uint8_t> compress_section(const std::vector<uint8_t> &raw, int codec, uint64_t block_size);
+// Metadata, Footer, PostScript and its length byte.  types / names: the columns (the root struct is added);
+// file_stats[0] = the root; content_length: the bytes in front of the Metadata ("ORC" and the stripes)
+std::vector<uint8_t> file_tail(const std::vector<OutType> &types, const std::vector<std::string> &names,
+                               const std::vector<OutStripe> &stripes, const std::vector<ColumnStats> &file_stats,
+                               uint64_t rows, uint64_t content_length, int codec, uint64_t block_size);
+
 }  // namespace orc

@@ -21,22 +21,13 @@
 #include <string>
 
 #include "device_utils.cuh"
+#include "encoded_file.h"
 #include "parquet_meta.h"
 #include "zstd_encode_device.cuh"
 
 namespace pg {
 
 // ------------------------------------------------------------------ page jobs
-
-struct EncColumn {
-    const void *data;
-    const int32_t *offsets;
-    const uint8_t *validity;     // NULL = no nulls
-    int32_t type;                // pg_type
-    int32_t width;               // bytes in memory, 0 = var-len
-    int32_t optional;            // OPTIONAL in the file (definition levels are written)
-    int32_t pad;
-};
 
 struct EncJob {                   // one data page of one column
     int32_t col;
@@ -151,8 +142,6 @@ k_pw_encode(const EncColumn *cols, const EncJob *jobs, uint8_t *file) {
 // per column chunk (one CTA): min / max of the non-null values of a fixed-width numeric column, as int64 / double
 // bit patterns (FLOAT / DOUBLE: of the non-NaN values, whichever zero comes first; the host applies the zero rule),
 // whether a non-null value is NaN; also used for the sequence number range and the delete count (kind column)
-struct StatJob { int32_t col; int32_t pad; int64_t row0; int64_t n_rows; };
-constexpr int kStatWords = 5;     // per job: min, max, non-null rows, retracts, NaN seen
 __global__ void k_pw_stats(const EncColumn *cols, const StatJob *jobs, int64_t *out /* [job][kStatWords] */) {
     const StatJob j = jobs[blockIdx.x];
     const EncColumn c = cols[j.col];
@@ -237,18 +226,6 @@ __global__ void k_pw_patch(const PatchJob *jobs, int n, const uint8_t *bytes, ui
 // per-page frame sizes go back to the host (which lays out the file and writes the page headers), and a gather places
 // the frames at their file offsets.
 
-struct ZsBlockJob {
-    int64_t src;                  // offset of the block in the body image
-    int64_t out;                  // offset of its payload slot (n bytes)
-    int64_t seq;                  // first sequence slot (n / 4 + 1 of them)
-    int32_t n;                    // input bytes (<= 128 KiB)
-    int32_t page;
-};
-struct ZsPage {
-    int64_t raw;                  // body bytes
-    int32_t first_block, n_blocks;
-};
-
 constexpr size_t kZsSmem = (sizeof(int32_t) << zs::kHashLog) + sizeof(zs::EncWork);
 
 __global__ void __launch_bounds__(32)
@@ -293,29 +270,19 @@ __global__ void k_zs_gather(const ZsBlockJob *jobs, const ZsPage *pages, const i
 
 // ------------------------------------------------------------------ host orchestration
 
-struct ColStats { int64_t min = 0, max = 0, null_count = 0; int has_minmax = 0; };
+Table<EncodedFile> g_enc(6);
 
-// the bits of a FLOAT / DOUBLE bound (held as a double), a zero of either sign replaced by `zero`
-static int64_t zero_as(int64_t bits, double zero) {
-    double x;
-    memcpy(&x, &bits, 8);
-    if (x == 0) memcpy(&bits, &zero, 8);
-    return bits;
+void launch_pw_stats(const EncColumn *cols, const StatJob *jobs, int n_jobs, int64_t *out) {
+    if (n_jobs) k_pw_stats<<<(unsigned)n_jobs, 256>>>(cols, jobs, out);
 }
 
-using Part = std::pair<int64_t, std::vector<uint8_t>>;  // a host-built piece of the file: (offset, bytes)
+void launch_zs_compress(const ZsBlockJob *jobs, int n_blocks, const ZsPage *pages, int n_pages, const uint8_t *img,
+                        uint8_t *out, void *seqs, uint8_t *lits, int2 *res, int32_t *boff, int64_t *frame_bytes) {
+    k_zs_block<<<(unsigned)n_blocks, 32, kZsSmem>>>(jobs, img, out, (zs::Seq *)seqs, lits, res);
+    k_zs_page_sizes<<<(unsigned)((n_pages + 127) / 128), 128>>>(pages, n_pages, res, boff, frame_bytes);
+}
 
-struct EncodedFile {
-    unsigned char *d_file = nullptr;         // device image of the file (page bodies at their final offsets)
-    int64_t file_bytes = 0;
-    int64_t data_end = 0;                    // end of the page data, where the footer starts
-    std::vector<Part> host_parts;            // headers, level prefixes, footer
-    pg_file_meta meta{};
-    std::vector<ColStats> stats;             // whole-file, per column
-    bool image_complete = false;             // host_parts have been patched into d_file
-    ~EncodedFile() { if (d_file) cudaFree(d_file); }
-};
-static Table<EncodedFile> g_enc(6);
+size_t zs_seq_bytes(int64_t seq) { return sizeof(zs::Seq) * (size_t)seq; }
 
 static int parquet_type_of(int t) {
     switch (t) {
@@ -455,9 +422,7 @@ static std::vector<Part> place_bodies(Plan &pl, const std::vector<int64_t> &base
     return prefixes;
 }
 
-// Copies host-built parts into the device image `dst` with one k_pw_patch launch, none when there are no parts.  The
-// staging buffers come from `scratch`; `what` names them when the device is out of memory.
-static pg_status patch(Scratch &scratch, const std::vector<Part> &parts, uint8_t *dst, const char *what) {
+pg_status patch(Scratch &scratch, const std::vector<Part> &parts, uint8_t *dst, const char *what) {
     if (parts.empty()) return PG_OK;
     std::vector<PatchJob> jobs;
     std::vector<uint8_t> bytes;

@@ -233,7 +233,7 @@ struct SectionTimer {
 };
 
 // ---- handle tables: one per handle kind.  A handle carries its kind's tag in the top byte (1 schema, 2 merge spec,
-// 3 run, 4 merge; 5 Parquet reader, 6 encoded Parquet file, 7 upload), so a handle of one kind is never found by
+// 3 run, 4 merge; 5 Parquet reader, 6 encoded Parquet or ORC file, 7 upload), so a handle of one kind is never found by
 // another kind's entry points.
 // The table holds one reference to each object; get() hands out a lease that an entry point holds until it returns, and
 // objects hold leases on what they use, so freeing a handle never frees an object in use.  No object holds a lease on

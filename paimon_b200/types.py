@@ -100,6 +100,33 @@ def physical_type(logical: str) -> PhysicalType:
     return _LOGICAL[root]
 
 
+# ORC TypeKind numbers (orc_proto Type.Kind) of the Paimon type roots, as OrcTypeUtil.convertToOrcType maps them
+# (paimon-format/.../orc/OrcTypeUtil.java:50-120).  TIMESTAMP and CHAR are mapped too; the ORC encoder refuses them.
+_ORC_KIND = {
+    "BOOLEAN": 0, "TINYINT": 1, "SMALLINT": 2, "INT": 3, "TIME": 3, "BIGINT": 4, "FLOAT": 5, "DOUBLE": 6,
+    "STRING": 7, "BINARY": 8, "VARBINARY": 8, "BYTES": 8, "TIMESTAMP": 9, "DECIMAL": 14, "DATE": 15, "VARCHAR": 16,
+    "CHAR": 17,
+}
+VARCHAR_MAX_LENGTH = 2147483647            # VarCharType.MAX_LENGTH: STRING is VARCHAR of this length
+
+
+def orc_column_type(logical: str):
+    """(kind, precision, scale, max_length) of pg_orc_column_type for a Paimon SQL type name: DECIMAL keeps its
+    precision and scale, VARCHAR(n) its length (VARCHAR of the maximum length is an ORC string)."""
+    root = type_root(logical)
+    if root not in _ORC_KIND:
+        raise ValueError(f"unsupported type on the GPU merge path: {logical}")
+    kind = _ORC_KIND[root]
+    if root == "DECIMAL":
+        p, s = decimal_precision_scale(logical)
+        return kind, p, s, 0
+    if root == "VARCHAR":
+        args = _type_args(logical)
+        n = args[0] if args else 1                   # VARCHAR alone is VARCHAR(1) (VarCharType.java)
+        return (7, 0, 0, 0) if n == VARCHAR_MAX_LENGTH else (kind, 0, 0, n)
+    return kind, 0, 0, 0
+
+
 def numpy_dtype(t: PhysicalType):
     return _NP[PhysicalType(t)]
 

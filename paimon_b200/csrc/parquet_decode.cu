@@ -831,13 +831,17 @@ k_pq_walk_dicts(const PqPage *dicts, int n_dicts, const PqChunk *chunks, int32_t
 // chains per warp instead of one lane working while 31 idle (the warp-per-page version was issue-bound).  Pages of a column chunk are neighbours in the page table, so the
 // lanes of a warp walk streams of similar length.
 // Reading the length words straight from global memory makes every lane miss a 32-byte sector on nearly every value
-// (32 scattered sector fetches per warp step, one round trip each), so the warp works in ROUNDS: it
-// loads the next kWvWin bytes of all 32 streams into shared memory with coalesced 16-byte loads (32 KiB in flight per
-// warp), then every lane walks the values whose length word lies inside its window at shared-memory latency.  A round
-// costs about one round trip whatever its size, so the window is as large as the shared memory allows: 1 KiB windows
-// took the C3 walk from 15.3 to 12.1 ms beside the expansion (H100, DESIGN.md §5), 512 B ones did not help.  Rows of the
-// window buffer are XOR-swizzled per 16-byte chunk (lanes walk their rows at similar offsets: without it every access
-// is a 32-way bank conflict).
+// (32 scattered sector fetches per warp step, one round trip each), so each lane's stream comes into shared memory
+// through a RING of kWvRing chunks of kWvChunk bytes, loaded by the warp with coalesced 16-byte async copies (8 lanes
+// per chunk).  The warp advances in uniform steps: every lane walks the length words inside its landed chunks (at most
+// kWvCap values), then the warp refills the chunks the lanes have left and commits exactly one copy group, so every
+// lane's group count stays the same and `cp.async.wait_group kWvLead` at the top of a step means "the chunks requested
+// kWvLead + 1 steps ago have landed".  A lane never waits for a copy it has just issued: the round trip hides behind
+// kWvLead steps of walking.  A small ring leaves the SMs' shared memory to the expansion beside the walk (1 KiB per
+// lane held it back for about 4 ms of the C3 decode).
+// Chunk k of a lane holds stream bytes [a0 + kWvChunk k, a0 + kWvChunk (k + 1)), a0 = the 16-byte boundary at or below
+// the stream start, so the ring is plain modulo addressing.  Rows are XOR-swizzled per 16-byte unit (lanes walk their
+// rows at similar offsets: without it every access is a 32-way bank conflict).
 __device__ __forceinline__ void cp_async16(void *smem_dst, const void *gsrc) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(gsrc) : "memory");
 }
@@ -846,13 +850,47 @@ __device__ __forceinline__ void cp_async4(void *smem_dst, const void *gsrc) {
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N> __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory"); }
-constexpr int kWvWarps = 1, kWvWin = 1024;
-static_assert(kWvWin % 16 == 0 && kWvWarps * 32 * kWvWin <= 48 * 1024, "whole 16-byte chunks, static shared memory");
+constexpr int kWvWarps = 1;
+constexpr int kWvChunk = 128, kWvRing = 4, kWvLead = 1, kWvCap = 32;
+constexpr int kWvRow = kWvChunk * kWvRing;                      // ring bytes per lane
+static_assert(kWvCap == 32, "one lane's values of a step leave as one warp store");
+static_assert((kWvRow & (kWvRow - 1)) == 0 && kWvChunk == 8 * 16 && kWvRow / 16 >= 16, "power-of-two ring, 8 units per chunk");
+
+#ifdef PG_WALK_TIMING
+// Cycle split of the value walk for every 4th warp (of the first 1024) that walks any value: per step, issuing the
+// copies, waiting for them and walking; plus steps, values, the warp's start / end on the global timer (waves) and its
+// SM.  Build with EXTRA_DEFS=-DPG_WALK_TIMING; every decode then synchronises and prints the split.
+constexpr int kWtSlots = 256;
+__device__ long long g_walk_ts[kWtSlots][8];
+#define WT_DECL long long wt_t = 0, wt_acc[3] = {0, 0, 0}, wt_steps = 0, wt_g0 = 0; \
+    const int wt_slot = (blockIdx.x % 4 == 0 && blockIdx.x < 4 * kWtSlots) ? (int)(blockIdx.x / 4) : -1; \
+    if (wt_slot >= 0) { asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(wt_g0)); wt_t = clock64(); }
+#define WT_MARK(k) do { if (wt_slot >= 0) { const long long wt_n = clock64(); wt_acc[k] += wt_n - wt_t; wt_t = wt_n; \
+    if ((k) == 2) wt_steps++; } } while (0)
+#define WT_END(vals) do { if (wt_slot >= 0) { long long wt_v = (vals); \
+    for (int d = 16; d > 0; d >>= 1) wt_v += __shfl_xor_sync(0xffffffffu, wt_v, d); \
+    if ((threadIdx.x & 31) == 0 && wt_v > 0) { long long g1; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(g1)); \
+        unsigned smid; asm("mov.u32 %0, %%smid;" : "=r"(smid)); long long *o = g_walk_ts[wt_slot]; \
+        o[0] = wt_acc[0]; o[1] = wt_acc[1]; o[2] = wt_acc[2]; o[3] = wt_steps; o[4] = wt_v; o[5] = wt_g0; o[6] = g1; \
+        o[7] = smid; } } } while (0)
+#else
+#define WT_DECL
+#define WT_MARK(k) do {} while (0)
+#define WT_END(vals) do {} while (0)
+#endif
+
 __global__ void __launch_bounds__(kWvWarps * 32)
 k_pq_walk_values(PqPage *pages, int n_pages, const PqChunk *chunks, int32_t *vstart, int32_t *err) {
-    __shared__ __align__(16) uint8_t s_win[kWvWarps][32][kWvWin];
+    __shared__ __align__(16) uint8_t s_ring[kWvWarps][32][kWvRow];
+    // the step's copy requests, one per chunk: source, and (lane << 8 | slot << 4 | 16-byte units to load)
+    __shared__ const uint8_t *s_req_src[kWvWarps][32 * kWvRing];
+    __shared__ uint32_t s_req_dst[kWvWarps][32 * kWvRing];
+    // the step's value starts of every lane, written out by the warp one lane's run at a time (one lane's stores are
+    // one 128-byte run; storing straight from the walk would scatter every warp store over 32 lines)
+    __shared__ int32_t s_vs[kWvWarps][32][kWvCap + 1];
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int t = blockIdx.x * (kWvWarps * 32) + threadIdx.x;
+    WT_DECL
     bool done = true;
     PqPage pg;
     pg.nnz = 0;
@@ -861,59 +899,98 @@ k_pq_walk_values(PqPage *pages, int n_pages, const PqChunk *chunks, int32_t *vst
         done = pg.bad || pg.enc != ENC_PLAIN || chunks[pg.chunk].phys != pq::T_BYTE_ARRAY;
     }
     const bool mine = !done;
-    int32_t *vs = mine ? vstart + pg.vs_base : nullptr;
     const uint8_t *stream = mine ? pg.body + pg.values_off : nullptr;
-    const int64_t slen = mine ? pg.body_len - pg.values_off : 0;
+    const int32_t slen = mine ? pg.body_len - pg.values_off : 0;
     const int nnz = mine ? pg.nnz : 0;
-    int64_t q = 0, bias = mine ? pg.payload_base : 0;     // out(j) = payload_base + (offset of value j's length word) - 4 j
+    const uint8_t *a0 = (const uint8_t *)((uintptr_t)stream & ~(uintptr_t)15);
+    // Positions are 32-bit offsets from a0 (a page body's size is an int32): p = the next length word, pend = the
+    // stream end.  out(j) = payload_base + (offset of value j's length word in the stream) - 4 j = p_j + bias_j.
+    const uint32_t off0 = (uint32_t)(stream - a0);
+    uint32_t p = off0, pend = off0 + (uint32_t)max(slen, 0);
+    uint32_t bias = mine ? (uint32_t)pg.payload_base - off0 : 0;
+    int32_t *vs = mine ? vstart + pg.vs_base : nullptr;
     int j = 0;
-    bool bad = false;
-    if (nnz == 0) done = true;
-    uint8_t (*rows)[kWvWin] = s_win[warp];
-    while (!__all_sync(0xffffffffu, done)) {
-        // ---- load every live lane's window [wb, wb + kWvWin): wb = the 16-byte boundary at or below its position
-        const uint8_t *wb = done ? nullptr : (const uint8_t *)((uintptr_t)(stream + q) & ~(uintptr_t)15);
-        const uint8_t *wend = done ? nullptr : stream + slen;
-        // (kWvWin / 16 async 16-byte copies per lane, all in flight together: one round trip per round; chunks past the
-        // stream's end are not loaded — the walk never reads a length word it has not bounds-checked against the stream)
-        constexpr int kChunks = kWvWin / 16;                          // 16-byte chunks per window
-#pragma unroll 4
-        for (int i = 0; i < kChunks; i++) {
-            const int f = 32 * i + lane, w = f / kChunks, c = f % kChunks;
-            const uint8_t *wbw = (const uint8_t *)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)wb, w);
-            const uint8_t *wew = (const uint8_t *)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)wend, w);
-            if (wbw != nullptr && wbw + 16 * c < wew) cp_async16(&rows[w][((c ^ (w & 15)) << 4)], wbw + 16 * c);   // (<= 15 bytes past the page)
-        }
-        cp_async_commit();
-        cp_async_wait<0>();
+    bool bad = slen < 0;
+    if (nnz == 0 || bad) done = true;
+    const int n_chunks = done ? 0 : (int)((pend + kWvChunk - 1) / kWvChunk);
+    int next = 0;                                      // chunks [0, next) requested (or skipped)
+    int hist[kWvLead + 1];                             // next after each of the last kWvLead + 1 steps' requests
+#pragma unroll
+    for (int i = 0; i <= kWvLead; i++) hist[i] = 0;
+    uint8_t (*rows)[kWvRow] = s_ring[warp];
+    const uint8_t *row = rows[lane];
+    const int sw = lane & 15;
+    while (true) {
+        cp_async_wait<kWvLead>();
         __syncwarp();
-        // ---- walk the values whose length word lies inside the window
+        WT_MARK(1);
+        // ---- walk the length words inside the landed chunks [p / kWvChunk, hist[0])
+        const uint32_t lim = (uint32_t)hist[0] * kWvChunk;
+        const int j0 = j;
         if (!done) {
-            int rel = (int)((stream + q) - wb);
-            const uint8_t *row = rows[lane];
-            const int sw = lane & 15;
-            while (j < nnz && rel + 4 <= kWvWin) {
-                if (q + 4 > slen) { bad = true; break; }
-                // the length word: two aligned words of the (chunk-swizzled) row, funnel-shifted
-                const int wi = rel >> 2, wj = min(wi + 1, kWvWin / 4 - 1);
+            for (int c = 0; c < kWvCap; c++) {
+                if (p + 4 > pend) { bad = true; break; }
+                if (p + 4 > lim) break;
+                // the length word: two aligned words of the (unit-swizzled) ring row, funnel-shifted
+                const uint32_t wi = (p >> 2) & (kWvRow / 4 - 1), wj = (wi + 1) & (kWvRow / 4 - 1);
                 const uint32_t lo = *(const uint32_t *)(row + ((((wi >> 2) ^ sw) << 4) | ((wi & 3) << 2)));
                 const uint32_t hi = *(const uint32_t *)(row + ((((wj >> 2) ^ sw) << 4) | ((wj & 3) << 2)));
-                const uint32_t len = __funnelshift_r(lo, hi, (rel & 3) * 8);
-                if ((int64_t)len > slen - q - 4) { bad = true; break; }
-                vs[j] = (int32_t)(q + bias);
+                const uint32_t len = __funnelshift_r(lo, hi, (p & 3) * 8);
+                if (len > pend - p - 4) { bad = true; break; }
+                s_vs[warp][lane][c] = (int32_t)(p + bias);
                 bias -= 4;
-                j++;
-                q += 4 + (int64_t)len;
-                // (a long value ends the round: rel leaves the window)
-                rel = len > (uint32_t)kWvWin ? kWvWin : rel + 4 + (int)len;
+                p += 4 + len;
+                if (++j == nnz) break;
             }
-            if (bad || j >= nnz) done = true;
+            if (bad || j == nnz) done = true;
         }
         __syncwarp();
+        for (unsigned m = __ballot_sync(0xffffffffu, j > j0); m != 0; m &= m - 1) {
+            const int i = __ffs(m) - 1;
+            const int n = __shfl_sync(0xffffffffu, j - j0, i);
+            int32_t *dst = (int32_t *)__shfl_sync(0xffffffffu, (unsigned long long)(uintptr_t)(vs + j0), i);
+            if (lane < n) dst[lane] = s_vs[warp][i][lane];
+        }
+        WT_MARK(2);
+        if (__all_sync(0xffffffffu, done)) break;
+        // ---- refill: chunks from `next` on, while the ring slot is free (its chunk was walked past, or a value skipped
+        // it) and its previous occupant has landed (so two copies never target one slot)
+        const int cur = (int)(p / kWvChunk);
+        const int first = max(next, cur);
+        const int nreq = done ? 0 : max(0, min(min(cur, hist[0]) + kWvRing, n_chunks) - first);
+        next = first + nreq;
+        int incl = nreq;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, incl, d);
+            if (lane >= d) incl += y;
+        }
+        const int total = __shfl_sync(0xffffffffu, incl, 31);
+        for (int r = 0; r < nreq; r++) {
+            const int k = first + r;
+            const uint32_t units = min(8u, (pend - (uint32_t)k * kWvChunk + 15) / 16);   // (<= 15 bytes past the page)
+            s_req_src[warp][incl - nreq + r] = a0 + (size_t)k * kWvChunk;
+            s_req_dst[warp][incl - nreq + r] = (uint32_t)lane << 8 | (uint32_t)(k % kWvRing) << 4 | units;
+        }
+        __syncwarp();
+        for (int e = lane >> 3; e < total; e += 4) {
+            const uint32_t d = s_req_dst[warp][e], u = lane & 7;
+            if (u < (d & 15)) {
+                const int owner = (int)(d >> 8), unit = (int)(((d >> 4) & 15) * 8 + u);
+                cp_async16(&rows[owner][(unit ^ (owner & 15)) << 4], s_req_src[warp][e] + 16 * u);
+            }
+        }
+        cp_async_commit();
+#pragma unroll
+        for (int i = 0; i < kWvLead; i++) hist[i] = hist[i + 1];
+        hist[kWvLead] = next;
+        WT_MARK(0);
     }
+    cp_async_wait<0>();
+    WT_END(nnz);
     if (mine) {
-        if (bad || (nnz > 0 && q != slen) || (nnz == 0 && slen != 0)) { pq_err(err, KERR_BAD_PAGE); pages[t].bad = 1; return; }
-        vs[nnz] = (int32_t)(q + bias);
+        if (bad || (nnz > 0 && p != pend) || (nnz == 0 && slen != 0)) { pq_err(err, KERR_BAD_PAGE); pages[t].bad = 1; return; }
+        vs[nnz] = (int32_t)(p + bias);
     }
 }
 
@@ -1442,6 +1519,47 @@ static pg_status build_chunk_tables(const Schema *s, const std::vector<SectionFi
     return PG_OK;
 }
 
+#ifdef PG_WALK_TIMING
+// prints the sampled warps' split (synchronises: a timing build only) and clears the samples
+static void walk_timing_dump() {
+    static long long h[kWtSlots][8];
+    cudaDeviceSynchronize();
+    cudaMemcpyFromSymbol(h, g_walk_ts, sizeof(h));
+    double acc[3] = {0, 0, 0}, steps = 0, vals = 0, steps_max = 0;
+    long long g_lo = LLONG_MAX, g_hi = 0;
+    int n = 0;
+    for (int s = 0; s < kWtSlots; s++) {
+        if (h[s][4] == 0) continue;
+        n++;
+        for (int k = 0; k < 3; k++) acc[k] += (double)h[s][k];
+        steps += (double)h[s][3];
+        steps_max = std::max(steps_max, (double)h[s][3]);
+        vals += (double)h[s][4];
+        g_lo = std::min(g_lo, h[s][5]);
+        g_hi = std::max(g_hi, h[s][6]);
+    }
+    if (n == 0) return;
+    const double tot = acc[0] + acc[1] + acc[2];
+    fprintf(stderr, "[walk timing] %d warps: cycles per step issue %.0f wait %.0f walk %.0f (%.1f / %.1f / %.1f %%); "
+                    "steps per warp %.1f (max %.0f), values per lane-step %.2f, span %.3f ms\n",
+            n, acc[0] / steps, acc[1] / steps, acc[2] / steps, 100 * acc[0] / tot, 100 * acc[1] / tot, 100 * acc[2] / tot,
+            steps / n, steps_max, vals / (32.0 * steps), (g_hi - g_lo) * 1e-6);
+    // start times in tenths of the span: how the CTAs fall into waves
+    int hist[10] = {0};
+    double busy = 0;
+    for (int s = 0; s < kWtSlots; s++) {
+        if (h[s][4] == 0) continue;
+        hist[std::min(9, (int)(10.0 * (h[s][5] - g_lo) / (double)(g_hi - g_lo + 1)))]++;
+        busy += (double)(h[s][6] - h[s][5]);
+    }
+    fprintf(stderr, "[walk timing] warp start by tenth of the span:");
+    for (int i = 0; i < 10; i++) fprintf(stderr, " %d", hist[i]);
+    fprintf(stderr, "; mean warp lifetime %.3f ms\n", busy / n * 1e-6);
+    static long long z[kWtSlots][8];
+    cudaMemcpyToSymbol(g_walk_ts, z, sizeof(z));
+}
+#endif
+
 // The value walk and the expansion.  With var-len columns, the value walk (one lane per page: latency-bound at low
 // occupancy) and the PLAIN BYTE_ARRAY pages that need it run on a side stream beside the expansion of all other pages.
 static pg_status expand_pages(cudaStream_t sm, bool byte_arrays, PqPage *d_pages, int np, const PqPage *d_dicts,
@@ -1475,6 +1593,9 @@ static pg_status expand_pages(cudaStream_t sm, bool byte_arrays, PqPage *d_pages
     k_pq_expand<false><<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
                                                    d_dict_len);
     PG_CUDA(cudaStreamWaitEvent(sm, ev_join, 0));
+#ifdef PG_WALK_TIMING
+    walk_timing_dump();
+#endif
     *launches += 3;
     return PG_OK;
 }

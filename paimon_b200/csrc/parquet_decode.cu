@@ -97,15 +97,17 @@ struct PqPair {
     int32_t idx, pad;
 };
 
-__device__ __forceinline__ uint32_t pq_varint(const uint8_t *&p, const uint8_t *end) {
+// a run header of the RLE / bit-packed hybrid; `ok` is cleared when the stream ends inside it
+__device__ __forceinline__ uint32_t pq_varint(const uint8_t *&p, const uint8_t *end, bool &ok) {
     uint32_t v = 0;
     int shift = 0;
     while (p < end) {
         uint8_t b = *p++;
         v |= (uint32_t)(b & 0x7f) << shift;
-        if (!(b & 0x80)) break;
+        if (!(b & 0x80)) return v;
         shift += 7;
     }
+    ok = false;
     return v;
 }
 
@@ -250,6 +252,9 @@ __global__ void k_pq_walk(PqChunk *chunks, int n_chunks, PqPage *pages, PqPage *
                 break;
             }
             const int body_len = codec_on ? h.unc : h.comp;
+            // fixed-width entries are looked up at body + id * width: every entry the header claims must be in the body
+            // (BYTE_ARRAY entries are walked and bounded by k_pq_walk_dicts)
+            if ((int64_t)h.nv * ch.phys_width > (int64_t)body_len) { pq_err(err, KERR_BAD_PAGE); break; }
             if (FILL) {
                 PqPage d;
                 memset(&d, 0, sizeof(d));
@@ -549,24 +554,22 @@ __global__ void k_pq_delta(PqPage *pages, int n_pages, const PqChunk *chunks, in
 //
 // Definition levels of a flat OPTIONAL column (bit width 1): the RLE / bit-packed hybrid stream
 // (VectorizedRleValuesReader.java:928-1019) is turned straight into the run's Arrow validity bitmap at bit
-// row0 + i.  A bit-packed run IS a bitmap: every lane moves 32 bits of it.  Returns the number of set bits.
-__device__ int pq_def_to_bits(const uint8_t *p, const uint8_t *end, int count, uint32_t *bm, int64_t row0) {
+// row0 + i.  A bit-packed run IS a bitmap: every lane moves 32 bits of it.  Returns the number of set bits; `ok` is
+// cleared when the stream ends before `count` levels or inside a run (parquet-mr refuses such a page too).
+__device__ int pq_def_to_bits(const uint8_t *p, const uint8_t *end, int count, uint32_t *bm, int64_t row0, bool &ok) {
     const int lane = threadIdx.x & 31;
     int pos = 0, nnz = 0;
-    while (pos < count && p < end) {
-        const uint32_t h = pq_varint(p, end);
+    while (pos < count) {
+        if (p >= end) { ok = false; break; }
+        const uint32_t h = pq_varint(p, end, ok);
         const bool packed = h & 1;
-        int64_t span = packed ? (int64_t)(h >> 1) * 8 : (int64_t)(h >> 1);       // values the run stands for
+        const int64_t span = packed ? (int64_t)(h >> 1) * 8 : (int64_t)(h >> 1);   // values the run stands for
+        const int64_t run_bytes = packed ? (int64_t)(h >> 1) : 1;
+        if (!ok || run_bytes > end - p) { ok = false; break; }
         const uint8_t *src = p;
-        if (packed) {
-            int64_t groups = h >> 1;
-            if (groups > end - p) { groups = end - p; span = groups * 8; }
-            p += groups;
-        } else {
-            p += 1;
-        }
+        p += run_bytes;
         const int nv = (int)pq_min64(span, count - pos);
-        const bool ones = !packed && src < end && (src[0] & 1);
+        const bool ones = !packed && (src[0] & 1);
         if (nv > 0 && (packed || ones)) {
             const int64_t d0 = row0 + pos, d1 = d0 + nv;
             for (int64_t w = (d0 >> 5) + lane; w <= ((d1 - 1) >> 5); w += 32) {
@@ -596,9 +599,10 @@ __device__ int pq_def_to_bits(const uint8_t *p, const uint8_t *end, int count, u
     return nnz;
 }
 
-// Warp-cooperative RLE / bit-packed hybrid decode of `count` values of bit width bw: out(i, value).
+// Warp-cooperative RLE / bit-packed hybrid decode of `count` values of bit width bw: out(i, value).  Returns false
+// (and stops before the run) when the stream ends before `count` values or a run's bytes reach past `end`.
 template <typename Out>
-__device__ void pq_hybrid_decode(const uint8_t *p, const uint8_t *end, int bw, int count, Out out) {
+__device__ bool pq_hybrid_decode(const uint8_t *p, const uint8_t *end, int bw, int count, Out out) {
     const int lane = threadIdx.x & 31;
     const uint32_t mask = bw >= 32 ? 0xffffffffu : ((1u << bw) - 1);
     int pos = 0;
@@ -607,11 +611,14 @@ __device__ void pq_hybrid_decode(const uint8_t *p, const uint8_t *end, int bw, i
             for (int i = pos + lane; i < count; i += 32) out(i, 0u);
             break;
         }
-        if (p >= end) break;
-        const uint32_t h = pq_varint(p, end);
+        if (p >= end) return false;
+        bool ok = true;
+        const uint32_t h = pq_varint(p, end, ok);
+        if (!ok) return false;
         if (h & 1) {
             const int64_t groups = (int64_t)(h >> 1);
             const int64_t nvals = groups * 8;
+            if (groups * bw > end - p) return false;
             for (int64_t i = lane; i < nvals && pos + i < count; i += 32) {
                 const int64_t bit = i * bw;
                 const uint8_t *q = p + (bit >> 3);
@@ -621,19 +628,20 @@ __device__ void pq_hybrid_decode(const uint8_t *p, const uint8_t *end, int bw, i
                     if (q + b < end) w |= (uint64_t)q[b] << (8 * b);
                 out(pos + (int)i, (uint32_t)(w >> (bit & 7)) & mask);
             }
-            if (groups * bw > end - p) p = end; else p += groups * bw;
+            p += groups * bw;
             pos = (int)pq_min64((int64_t)pos + nvals, (int64_t)count);
         } else {
             const int run = (int)(h >> 1);
             uint32_t v = 0;
             const int nb = (bw + 7) / 8;
-            for (int b = 0; b < nb; b++)
-                if (p + b < end) v |= (uint32_t)p[b] << (8 * b);
+            if (nb > end - p) return false;
+            for (int b = 0; b < nb; b++) v |= (uint32_t)p[b] << (8 * b);
             p += nb;
             for (int i = lane; i < run && pos + i < count; i += 32) out(pos + i, v & mask);
             pos = (int)pq_min64((int64_t)pos + run, (int64_t)count);
         }
     }
+    return true;
 }
 
 // one warp per data page
@@ -663,7 +671,9 @@ __global__ void k_pq_levels(PqPage *pages, int n_pages, const PqPage *dicts, con
         if (!bad && (dlen < 0 || (int64_t)values_off + dlen > pg.body_len)) bad = true;
         if (!bad) {
             values_off += dlen;
-            nnz = pq_def_to_bits(dp, dp + dlen, nv, out.validity, pg.row0);
+            bool ok = true;
+            nnz = pq_def_to_bits(dp, dp + dlen, nv, out.validity, pg.row0, ok);
+            bad = !ok;
         }
     }
     else if (out.validity != nullptr) {
@@ -688,8 +698,9 @@ __global__ void k_pq_levels(PqPage *pages, int n_pages, const PqPage *dicts, con
             const bool ba = ch.phys == pq::T_BYTE_ARRAY;
             const int32_t *dl = dict_len + dj.entry_base;
             bool oob = false;
-            if (bw > 32) bad = true;
-            else pq_hybrid_decode(vp + 1, end, bw, nnz, [&](int i, uint32_t v) {
+            // (the ids the stream does not cover would be whatever the ids scratch held: a short stream is refused)
+            if (bw > 32 || (nnz > 0 && vp >= end)) bad = true;
+            else bad = !pq_hybrid_decode(vp + 1, end, bw, nnz, [&](int i, uint32_t v) {
                 if (v >= n_entries) { oob = true; v = 0; }
                 dst[i] = (int32_t)v;
                 if (ba && n_entries) payload += dl[v];
@@ -699,7 +710,7 @@ __global__ void k_pq_levels(PqPage *pages, int n_pages, const PqPage *dicts, con
             // RLE-encoded BOOLEAN values: <length:4> <hybrid stream of bit width 1>
             int32_t *dst = ids + pg.ids_base;
             if (vbytes < 4) bad = nnz > 0;
-            else pq_hybrid_decode(vp + 4, end, 1, nnz, [&](int i, uint32_t v) { dst[i] = (int32_t)v; });
+            else bad = !pq_hybrid_decode(vp + 4, end, 1, nnz, [&](int i, uint32_t v) { dst[i] = (int32_t)v; });
         } else if (ch.phys == pq::T_BYTE_ARRAY) {
             const int64_t pb = vbytes - 4 * (int64_t)nnz;
             if (pb < 0) bad = true;

@@ -282,8 +282,9 @@ pg_status pg_thread_stream(void **out_cuda_stream);
  * 113-148, reader/VectorizedParquetRecordReader.java:178-241) for KeyValue data files: the file bytes (read by the
  * Java FileIO) are parsed on the host for footer + page headers and decoded on the device straight into the
  * columnar run the merge consumes.  Decoded: flat schemas, BOOLEAN/INT32/INT64/FLOAT/DOUBLE/BYTE_ARRAY, PLAIN and
- * dictionary encodings, RLE booleans, DELTA_BINARY_PACKED integers, data pages V1/V2, uncompressed, Snappy-, zstd- and
- * gzip-compressed pages (decompressed on the device); anything else (lz4, brotli, byte-array DELTA encodings,
+ * dictionary encodings, RLE booleans, DELTA_BINARY_PACKED integers, data pages V1/V2, uncompressed, Snappy-, zstd-,
+ * gzip- and LZ4-compressed pages (codec 5, Hadoop block framing; decompressed on the device); anything else (LZ4_RAW
+ * = codec 7, brotli, lzo, byte-array DELTA encodings,
  * INT96 / FIXED_LEN_BYTE_ARRAY, nested columns) returns PG_ERR_UNSUPPORTED.  pg_parquet_open walks the page headers
  * on the host once so that such files are refused before any device work. */
 typedef struct {
@@ -350,7 +351,7 @@ pg_status pg_parquet_read_section(uint64_t schema, const pg_file_desc *files, in
  * OrcReaderFactory.java:98-163): every stripe of every file of a section, the files of a run concatenated.  Decoded:
  * flat schemas, BOOLEAN / TINYINT / SMALLINT / INT / BIGINT / FLOAT / DOUBLE / DATE / DECIMAL(p <= 18) / STRING-family /
  * BINARY, integer RLE v1 and v2, DIRECT and DICTIONARY string encodings, PRESENT streams, compression NONE / ZLIB /
- * ZSTD; columns are resolved by field name (missing nullable fields -> NULL, integer / float widening).  Timestamps,
+ * LZ4 / ZSTD; columns are resolved by field name (missing nullable fields -> NULL, integer / float widening).  Timestamps,
  * DECIMAL(p > 18), nested types and the other codecs return PG_ERR_UNSUPPORTED.  The file bytes must be host memory
  * (footers and compression-chunk headers are walked on the host); pg_section_info.n_chunks counts (stripe, column)
  * tasks and n_data_pages counts streams. */

@@ -9,7 +9,7 @@
 // One call decodes a whole SECTION like pg_parquet_read_section: the files of a sorted run are concatenated into one
 // device run.  Host: file tails (protobuf footers, inflated on the host) -> a plan of streams and (stripe, column)
 // tasks.  Device: k_orc_inflate (one warp per stream: compression chunks -> contiguous bytes with the shared
-// DEFLATE / zstd decoders), k_orc_task<0> (one thread per task: PRESENT -> validity, values / lengths), an offsets
+// DEFLATE / zstd / LZ4 decoders), k_orc_task<0> (one thread per task: PRESENT -> validity, values / lengths), an offsets
 // scan per var-len column, k_orc_task<1> (payload bytes).  The stream decoders are the host-pinned orc_device.cuh.
 #include <algorithm>
 #include <cstring>
@@ -17,6 +17,7 @@
 #include <stdexcept>
 
 #include "inflate_device.cuh"
+#include "lz4_device.cuh"
 #include "orc_device.cuh"
 #include "orc_meta.h"
 #include "scan_kernels.cuh"
@@ -74,6 +75,7 @@ k_orc_inflate(OrcStream *streams, int n_streams, uint8_t *lit_scratch, int32_t *
                 const int64_t cap = min(block_size, st.bound - out);
                 int64_t got;
                 if (codec == orc::C_ZLIB) got = inflate::inflate_raw(st.src + pos, len, st.dst + out, cap, *(inflate::Tables *)&ZT[w], nullptr);
+                else if (codec == orc::C_LZ4) got = lz4::decode_block(st.src + pos, len, st.dst + out, cap);
                 else got = zs::decode(st.src + pos, len, st.dst + out, cap, lit, ZT[w]);
                 __syncwarp();
                 if (got < 0) { bad = true; break; }
@@ -164,9 +166,10 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
             tails[f] = orc::parse_file(files[f].bytes, files[f].size);
             const orc::FileTail &t = tails[f];
             if (t.types.empty() || t.types[0].kind != orc::K_STRUCT) return fail(PG_ERR_UNSUPPORTED, "orc: the root type is not a struct");
-            if (t.compression != orc::C_NONE && t.compression != orc::C_ZLIB && t.compression != orc::C_ZSTD)
+            if (t.compression != orc::C_NONE && t.compression != orc::C_ZLIB && t.compression != orc::C_ZSTD &&
+                t.compression != orc::C_LZ4)
                 return fail(PG_ERR_UNSUPPORTED, "orc: compression kind " + std::to_string(t.compression) +
-                                                " is not decoded on device (NONE, ZLIB and ZSTD are)");
+                                                " is not decoded on device (NONE, ZLIB, LZ4 and ZSTD are)");
             if (t.compression != orc::C_NONE) any_compressed = true;
             if (t.compression == orc::C_ZSTD) any_zstd = true;
             if (t.block_size > (1u << 30)) return fail(PG_ERR_UNSUPPORTED, "orc: compression block size above 1 GiB");

@@ -8,6 +8,7 @@
 #include <stdexcept>
 
 #include "inflate_device.cuh"
+#include "lz4_device.cuh"
 #include "zstd_device.cuh"
 #include "zstd_encode_device.cuh"
 
@@ -64,8 +65,8 @@ struct Pb {
 // a metadata section stored as compression chunks: [3-byte header: length << 1 | isOriginal][bytes]...
 std::vector<uint8_t> inflate_section(const uint8_t *p, uint64_t n, int codec, uint64_t block_size) {
     if (codec == C_NONE) return std::vector<uint8_t>(p, p + n);
-    if (codec != C_ZLIB && codec != C_ZSTD)
-        throw std::runtime_error("orc: compression kind " + std::to_string(codec) + " is not decoded (NONE, ZLIB and ZSTD are)");
+    if (codec != C_ZLIB && codec != C_ZSTD && codec != C_LZ4)
+        throw std::runtime_error("orc: compression kind " + std::to_string(codec) + " is not decoded (NONE, ZLIB, LZ4 and ZSTD are)");
     std::vector<uint8_t> out;
     std::vector<uint8_t> buf(block_size + 64), lit(zs::kMaxBlock + 64);
     inflate::Tables it;
@@ -80,8 +81,9 @@ std::vector<uint8_t> inflate_section(const uint8_t *p, uint64_t n, int codec, ui
         if (n - pos < len) throw std::runtime_error("orc: truncated compression chunk");
         if (h & 1) out.insert(out.end(), p + pos, p + pos + len);
         else {
-            const int64_t got = codec == C_ZLIB ? inflate::inflate_raw(p + pos, len, buf.data(), (int64_t)block_size, it, nullptr)
-                                                : zs::decode(p + pos, len, buf.data(), (int64_t)block_size, lit.data(), *zt);
+            const int64_t got = codec == C_ZLIB  ? inflate::inflate_raw(p + pos, len, buf.data(), (int64_t)block_size, it, nullptr)
+                                : codec == C_LZ4 ? lz4::decode_block(p + pos, len, buf.data(), (int64_t)block_size)
+                                                 : zs::decode(p + pos, len, buf.data(), (int64_t)block_size, lit.data(), *zt);
             if (got < 0) throw std::runtime_error("orc: a metadata compression chunk does not inflate");
             out.insert(out.end(), buf.data(), buf.data() + got);
         }

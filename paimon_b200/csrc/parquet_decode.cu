@@ -17,7 +17,7 @@
 //   host    footers only (Thrift FileMetaData) -> a table of column chunks, ordered (run, column, file, row group)
 //   walk    one thread per column chunk parses the Thrift page headers ON THE DEVICE (count pass, scan, fill pass)
 //           -> one page table for the section
-//   inflate Snappy pages -> scratch images; DELTA_BINARY_PACKED pages -> PLAIN images
+//   inflate Snappy / LZ4 / zstd / GZIP pages -> scratch images; DELTA_BINARY_PACKED pages -> PLAIN images
 //   levels  one warp per page: definition levels -> the output validity bitmap (bit-packed runs are copied 32 bits
 //           at a time), dictionary ids -> scratch, per-page non-null counts and var-len payload sizes
 //   scan    per (run, var-len column): payload base of every page (files of a run continue each other's offsets)
@@ -34,6 +34,7 @@
 #include "device_utils.cuh"
 #include "parquet_meta.h"
 #include "inflate_device.cuh"
+#include "lz4_device.cuh"
 #include "scan_kernels.cuh"
 #include "zstd_device.cuh"
 
@@ -343,7 +344,7 @@ __global__ void __launch_bounds__(kScanThreads) k_pq_chunk_scan(PqChunk *chunks,
     }
 }
 
-// ------------------------------------------------------------------ Snappy page decompression
+// ------------------------------------------------------------------ Snappy / LZ4 page decompression
 //
 // parquet-mr hands compressed pages to snappy-java 1.1.10.8 (not under /root/reference); the format restated here is
 // the public Snappy format description: a varint uncompressed length, then literal and copy elements.  One warp per
@@ -351,12 +352,15 @@ __global__ void __launch_bounds__(kScanThreads) k_pq_chunk_scan(PqChunk *chunks,
 // lane-parallel.  A copy may overlap its own output (offset < length): byte i comes from out - offset +
 // (i mod offset), which always lies in front of the copy.  Data page V2: the level bytes in front of the values are
 // stored uncompressed and copied verbatim.
-__global__ void k_pq_snappy(const PqPage *pages, int n_pages, const PqPage *dicts, int n_dicts, const PqChunk *chunks,
-                            int32_t *err) {
+// Codec 5 (LZ4) pages are Hadoop-framed LZ4 blocks (lz4_device.cuh, the same warp-per-page shape); no length of a
+// chunk's output is stored, so one warp walks a page's blocks in order.
+__global__ void k_pq_snappy_lz4(const PqPage *pages, int n_pages, const PqPage *dicts, int n_dicts, const PqChunk *chunks,
+                                int32_t *err) {
     const int w = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
     if (w >= n_pages + n_dicts) return;
     const PqPage &pg = w < n_pages ? pages[w] : dicts[w - n_pages];
-    if (!pg.compressed || chunks[pg.chunk].codec != pq::C_SNAPPY) return;
+    const int codec = chunks[pg.chunk].codec;
+    if (!pg.compressed || (codec != pq::C_SNAPPY && codec != pq::C_LZ4)) return;
     const int prefix = pg.type == pq::P_DATA_V2 ? pg.def_len : 0;
     uint8_t *out0 = const_cast<uint8_t *>(pg.body);
     const uint8_t *in0 = pg.src;
@@ -365,6 +369,10 @@ __global__ void k_pq_snappy(const PqPage *pages, int n_pages, const PqPage *dict
     const uint8_t *src = in0 + prefix;
     uint8_t *dst = out0 + prefix;
     const int n_src = pg.src_len - prefix, n_dst = pg.body_len - prefix;
+    if (codec == pq::C_LZ4) {
+        if (lz4::decode_hadoop(src, n_src, dst, n_dst) != n_dst && lane == 0) pq_err(err, KERR_BAD_PAGE);
+        return;
+    }
     int pos = 0, out = 0;
     uint32_t ulen = 0;                                    // preamble: uncompressed length
     for (int sh = 0; pos < n_src && sh < 35; sh += 7) {
@@ -1391,10 +1399,11 @@ static pg_status map_file_schema(RunBuilder &b, const pq::FileMetaData &m, int r
     for (const pq::RowGroup &g : m.row_groups) {
         if ((int)g.columns.size() != nleaf) return fail(PG_ERR_FORMAT, "parquet: row group with a different column count");
         for (const pq::ColumnChunk &cc : g.columns)
-            if (cc.codec != pq::C_UNCOMPRESSED && cc.codec != pq::C_SNAPPY && cc.codec != pq::C_ZSTD && cc.codec != pq::C_GZIP)
+            if (cc.codec != pq::C_UNCOMPRESSED && cc.codec != pq::C_SNAPPY && cc.codec != pq::C_ZSTD && cc.codec != pq::C_GZIP &&
+                cc.codec != pq::C_LZ4)
                 return fail(PG_ERR_UNSUPPORTED, "parquet: compression codec " + std::to_string(cc.codec) +
-                                                " is not decoded on device (UNCOMPRESSED, SNAPPY, ZSTD and GZIP are); write with "
-                                                "'file.compression'='zstd' / 'snappy' / 'gzip' / 'none' or let the Java side decompress");
+                                                " is not decoded on device (UNCOMPRESSED, SNAPPY, ZSTD, GZIP and Hadoop-framed LZ4 = 5 are); write with "
+                                                "'file.compression'='zstd' / 'snappy' / 'gzip' / 'lz4' / 'none' or let the Java side decompress");
     }
     return PG_OK;
 }
@@ -1471,7 +1480,7 @@ static pg_status fetch_footers(const std::vector<SectionFile> &files, cudaStream
 struct ChunkTables {
     std::vector<PqChunk> chunks;
     std::vector<PqPair> pairs;
-    bool any_snappy = false, any_delta = false, any_zstd = false;
+    bool any_snappy = false, any_lz4 = false, any_delta = false, any_zstd = false;
     int64_t pair_rows = 0;
 };
 
@@ -1512,6 +1521,7 @@ static pg_status build_chunk_tables(const Schema *s, const std::vector<SectionFi
                     ch.cast = phys_cast(s->field(c).type, cc.type);
                     if (cc.type != m.schema[fc + 1].type) return fail(PG_ERR_FORMAT, "parquet: column chunk type differs from the schema");
                     if (cc.codec == pq::C_SNAPPY) t.any_snappy = true;
+                    if (cc.codec == pq::C_LZ4) t.any_lz4 = true;
                     if (cc.codec == pq::C_ZSTD || cc.codec == pq::C_GZIP) t.any_zstd = true;
                     for (int32_t e : cc.encodings) if (e == pq::E_DELTA_BINARY_PACKED) t.any_delta = true;
                     if (cc.num_values > 0) t.chunks.push_back(ch);
@@ -1734,9 +1744,9 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const st
     if (np > 0) {
         k_pq_walk<true><<<(n_chunks + 63) / 64, 64, 0, sm>>>(d_chunks, n_chunks, d_pages, d_dicts, d_sc, d_err);
         launches++;
-        if (ct.any_snappy) {
+        if (ct.any_snappy || ct.any_lz4) {
             const int64_t th = (int64_t)(np + nd) * 32;
-            k_pq_snappy<<<(unsigned)((th + 127) / 128), 128, 0, sm>>>(d_pages, np, d_dicts, nd, d_chunks, d_err);
+            k_pq_snappy_lz4<<<(unsigned)((th + 127) / 128), 128, 0, sm>>>(d_pages, np, d_dicts, nd, d_chunks, d_err);
             launches++;
         }
         if (ct.any_zstd && zs_ctas > 0) {

@@ -341,7 +341,14 @@ ORC_HD inline void decode_task_a(Task &t) {
             if (ok) {
                 v = read_vslong(d);
                 int64_t s = irle_next(sc);
-                for (; s < t.scale; s++) v *= 10;          // rescale to the type's scale (DecimalColumnVector semantics)
+                // a value's own scale is 0..38 and at most 18 away from the type's (any other is a corrupt stream):
+                // the rescale to the type's scale (DecimalColumnVector semantics) then takes at most 18 steps
+                if (s < 0 || s > 38 || s - t.scale > 18 || t.scale - s > 18) { bad = 1; break; }
+                for (; s < t.scale; s++) {
+                    if (v > INT64_MAX / 10 || v < INT64_MIN / 10) { bad = 1; break; }
+                    v *= 10;
+                }
+                if (bad) break;
                 for (; s > t.scale; s--) v /= 10;
             }
             store_val(t.out_data, t.out_width, t.row0 + i, (uint64_t)v);
@@ -351,13 +358,14 @@ ORC_HD inline void decode_task_a(Task &t) {
         if (dict) {
             irle_init(len, t.length, t.length_n, v2, 0);
             int64_t acc = 0;
-            for (int j = 0; j < t.dict_size; j++) {
+            for (int j = 0; j < t.dict_size && !bad; j++) {    // (stops where the LENGTH stream runs dry)
                 t.dict_off[j] = (int32_t)acc;
-                acc += irle_next(len);
+                const int64_t l = irle_next(len);
+                acc += l;
+                if (len.s.bad || l < 0 || acc > t.dict_data_n || acc > 0x7fffffffLL) bad = 1;
             }
-            t.dict_off[t.dict_size] = (int32_t)acc;
-            if (acc > t.dict_data_n || acc > 0x7fffffffLL) bad = 1;
-            bad |= len.s.bad;
+            if (t.dict_size < 0) bad = 1;
+            if (!bad) t.dict_off[t.dict_size] = (int32_t)acc;
             IntRle &ids = r;
             irle_init(ids, t.data, t.data_n, v2, 0);
             for (int64_t i = 0; i < t.rows && !bad; i++) {

@@ -150,7 +150,10 @@ StripeFooter read_stripe_footer(Pb pb) {
                 if (w2 != 0) { s.skip(w2); continue; }
                 const uint64_t v = s.varint();
                 if (f2 == 1) ce.kind = (int)v;
-                else if (f2 == 2) ce.dictionary_size = (uint32_t)v;
+                else if (f2 == 2) {
+                    if (v > 0xffffffffull) throw std::runtime_error("orc: dictionarySize outside uint32");
+                    ce.dictionary_size = (uint32_t)v;
+                }
             }
             sf.columns.push_back(ce);
         } else pb.skip(w);
@@ -265,6 +268,11 @@ Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::
                 pl.streams.push_back(ps);
             }
             if (task.enc == E_DICTIONARY || task.enc == E_DICTIONARY_V2) {
+                // a dictionary holds distinct values of the stripe's rows: a larger claim is a corrupt footer, refused
+                // before the offsets scratch is sized from it
+                if (task.dict_size > (uint64_t)task.rows)
+                    throw std::runtime_error("orc: stripe " + std::to_string(si) + " claims a dictionary of " +
+                                             std::to_string(task.dict_size) + " entries for " + std::to_string(task.rows) + " rows");
                 task.dict_off_base = pl.dict_entries;
                 pl.dict_entries += (uint64_t)task.dict_size + 1;
             }

@@ -446,7 +446,8 @@ ZS_HD inline int read_literals(const uint8_t *p, int len, uint8_t *lit_buf, Tabl
 #endif
     }
 #if defined(__CUDA_ARCH__)
-    rc = __any_sync(0xffffffffu, rc != 0) ? -1 : 0;        // (also makes lit_buf visible to the whole warp)
+    __syncwarp();                                           // lanes 0..3 wrote lit_buf: order it before every lane reads
+    rc = __any_sync(0xffffffffu, rc != 0) ? -1 : 0;        // (a vote alone implies no memory ordering)
 #endif
     if (rc) return -1;
     L.ptr = lit_buf; L.size = regen; L.rle = 0; L.value = 0;

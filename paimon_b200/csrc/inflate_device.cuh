@@ -10,7 +10,8 @@
 //
 // One decoder = one warp on the device, like zstd_device.cuh: every lane runs the same control flow, lane 0 builds
 // the code tables and writes literals, match copies are lane-parallel (byte i of an overlapping copy comes from
-// out - dist + (i mod dist)).  tests/test_inflate_cpu.py pins the host build against zlib.
+// out - dist + (i mod dist)).  tests/test_inflate_cpu.py pins the host build against zlib, and tests/test_codecs_cpu.py
+// fuzzes it under sanitizers: every stream it accepts, zlib accepts with the same bytes once the CRCs it skips are right.
 #pragma once
 
 #include <stdint.h>
@@ -83,8 +84,11 @@ IF_HD inline uint32_t getbits(Bits &b, int n) {           // n <= 32
     return v;
 }
 
-// canonical Huffman code from code lengths (RFC 1951 §3.2.2).  Returns 0, or -1 for an over-subscribed code.
-IF_HD inline int build(Huff &h, const uint8_t *lens, int n) {
+// canonical Huffman code from code lengths (RFC 1951 §3.2.2).  Returns 0, or -1 for an over-subscribed code and for
+// an incomplete code of a dynamic block.  zlib's rule: a code with no symbols is allowed (using it is an error), and a
+// literal/length or distance code may be a single code of 1 bit; the fixed distance code is incomplete by design.
+enum CodeKind { kFixed, kCodeLengths, kLitDist };
+IF_HD inline int build(Huff &h, const uint8_t *lens, int n, CodeKind kind) {
     for (int i = 0; i < 16; i++) h.count[i] = 0;
     for (int i = 0; i < n; i++) h.count[lens[i]]++;
     h.count[0] = 0;
@@ -97,6 +101,11 @@ IF_HD inline int build(Huff &h, const uint8_t *lens, int n) {
         h.first[l] = (uint16_t)code;
         h.index[l] = (uint16_t)idx;
         idx += h.count[l];
+    }
+    if (left > 0 && kind != kFixed) {
+        int max = 15;
+        while (max > 0 && !h.count[max]) max--;
+        if (max > 0 && (kind == kCodeLengths || max != 1)) return -1;
     }
     // symbols in (length, symbol) order
     uint16_t next[16];
@@ -177,9 +186,9 @@ IF_HD inline int64_t inflate_raw(const uint8_t *src, int64_t n, uint8_t *dst, in
                     for (int i = 144; i < 256; i++) T.lens[i] = 9;
                     for (int i = 256; i < 280; i++) T.lens[i] = 7;
                     for (int i = 280; i < 288; i++) T.lens[i] = 8;
-                    rc = build(T.lit, T.lens, 288);
+                    rc = build(T.lit, T.lens, 288, kFixed);
                     for (int i = 0; i < 30; i++) T.lens[i] = 5;
-                    rc |= build(T.dist, T.lens, 30);
+                    rc |= build(T.dist, T.lens, 30, kFixed);
                 }
                 rc = bcast0(rc);
             } else {
@@ -190,7 +199,7 @@ IF_HD inline int64_t inflate_raw(const uint8_t *src, int64_t n, uint8_t *dst, in
                 for (int i = 0; i < 19; i++) cl[i] = 0;
                 for (int i = 0; i < hclen; i++) cl[clc_order[i]] = (uint8_t)getbits(b, 3);
                 warp_sync();                              // (nobody still decodes with the previous block's tables)
-                if (lane_id() == 0) rc = build(T.lit, cl, 19);          // borrowed: T.lit is rebuilt below
+                if (lane_id() == 0) rc = build(T.lit, cl, 19, kCodeLengths);          // borrowed: T.lit is rebuilt below
                 rc = bcast0(rc);
                 if (rc) return -1;
                 // code lengths of the literal/length and distance alphabets, run-length coded
@@ -215,8 +224,8 @@ IF_HD inline int64_t inflate_raw(const uint8_t *src, int64_t n, uint8_t *dst, in
                     else {
                         uint8_t tmp[32];
                         for (int k = 0; k < hdist; k++) tmp[k] = T.lens[hlit + k];
-                        rc = build(T.lit, T.lens, hlit);
-                        rc |= build(T.dist, tmp, hdist);
+                        rc = build(T.lit, T.lens, hlit, kLitDist);
+                        rc |= build(T.dist, tmp, hdist, kLitDist);
                     }
                 }
                 rc = bcast0(rc);
@@ -264,6 +273,7 @@ IF_HD inline int64_t inflate_gzip(const uint8_t *src, int64_t n, uint8_t *dst, i
     while (pos < n) {                                     // concatenated members are legal
         if (n - pos < 18 || src[pos] != 0x1f || src[pos + 1] != 0x8b || src[pos + 2] != 8) return -1;
         const int flg = src[pos + 3];
+        if (flg & 0xE0) return -1;                        // reserved flags
         int64_t p = pos + 10;
         if (flg & 4) { if (p + 2 > n) return -1; p += 2 + (src[p] | (src[p + 1] << 8)); }
         if (flg & 8) { while (p < n && src[p]) p++; p++; }
@@ -274,16 +284,20 @@ IF_HD inline int64_t inflate_gzip(const uint8_t *src, int64_t n, uint8_t *dst, i
         const int64_t got = inflate_raw(src + p, n - p, dst + out, cap - out, T, &used);
         if (got < 0) return -1;
         out += got;
-        pos = p + used + 8;                               // CRC32 + ISIZE are not verified
+        pos = p + used + 8;                               // the header CRC16 and CRC32 are not verified; ISIZE is
         if (pos > n) return -1;
+        const uint32_t isize = src[pos - 4] | (src[pos - 3] << 8) | (src[pos - 2] << 16) | ((uint32_t)src[pos - 1] << 24);
+        if (isize != (uint32_t)got) return -1;
     }
     return out;
 }
 
-// a zlib stream (RFC 1950: 2-byte header, DEFLATE, Adler-32) -> dst
+// a zlib stream (RFC 1950: 2-byte header, DEFLATE, Adler-32) -> dst.  The Adler-32 must be there; it is not verified.
 IF_HD inline int64_t inflate_zlib(const uint8_t *src, int64_t n, uint8_t *dst, int64_t cap, Tables &T) {
-    if (n < 6 || (src[0] & 15) != 8 || ((src[0] << 8) | src[1]) % 31 != 0 || (src[1] & 32)) return -1;
-    return inflate_raw(src + 2, n - 2, dst, cap, T, nullptr);
+    if (n < 6 || (src[0] & 15) != 8 || (src[0] >> 4) > 7 || ((src[0] << 8) | src[1]) % 31 != 0 || (src[1] & 32)) return -1;
+    int64_t used = 0;
+    const int64_t got = inflate_raw(src + 2, n - 2, dst, cap, T, &used);
+    return got >= 0 && n - 2 - used >= 4 ? got : -1;
 }
 
 }  // namespace inflate

@@ -40,7 +40,9 @@ struct OrcTaskRef {            // stream table indexes of a task (-1 = absent)
 };
 
 constexpr int kOrcWarps = 4;
-__global__ void __launch_bounds__(kOrcWarps * 32)
+// the grid launches at most 4 CTAs per SM; the bound caps the registers (128) so that all 4 stay resident, which
+// the decoders alone would not (153 registers leave room for 3)
+__global__ void __launch_bounds__(kOrcWarps * 32, 4)
 k_orc_inflate(OrcStream *streams, int n_streams, uint8_t *lit_scratch, int32_t *counter, int32_t *err) {
     __shared__ zs::Tables ZT[kOrcWarps];               // (the DEFLATE tables are smaller and overlay them)
     static_assert(sizeof(inflate::Tables) <= sizeof(zs::Tables), "tables overlay");

@@ -35,6 +35,7 @@
 #include "parquet_meta.h"
 #include "inflate_device.cuh"
 #include "lz4_device.cuh"
+#include "snappy_device.cuh"
 #include "scan_kernels.cuh"
 #include "zstd_device.cuh"
 
@@ -346,12 +347,9 @@ __global__ void __launch_bounds__(kScanThreads) k_pq_chunk_scan(PqChunk *chunks,
 
 // ------------------------------------------------------------------ Snappy / LZ4 page decompression
 //
-// parquet-mr hands compressed pages to snappy-java 1.1.10.8 (not under /root/reference); the format restated here is
-// the public Snappy format description: a varint uncompressed length, then literal and copy elements.  One warp per
-// page: the element stream is parsed by all lanes in lock step, the bytes of a literal / copy are moved
-// lane-parallel.  A copy may overlap its own output (offset < length): byte i comes from out - offset +
-// (i mod offset), which always lies in front of the copy.  Data page V2: the level bytes in front of the values are
-// stored uncompressed and copied verbatim.
+// Codec 1 (SNAPPY) pages are one Snappy stream (snappy_device.cuh): one warp per page parses the element stream in
+// lock step and moves the bytes of a literal / copy lane-parallel.  Data page V2: the level bytes in front of the
+// values are stored uncompressed and copied verbatim.
 // Codec 5 (LZ4) pages are Hadoop-framed LZ4 blocks (lz4_device.cuh, the same warp-per-page shape); no length of a
 // chunk's output is stored, so one warp walks a page's blocks in order.
 __global__ void k_pq_snappy_lz4(const PqPage *pages, int n_pages, const PqPage *dicts, int n_dicts, const PqChunk *chunks,
@@ -373,56 +371,7 @@ __global__ void k_pq_snappy_lz4(const PqPage *pages, int n_pages, const PqPage *
         if (lz4::decode_hadoop(src, n_src, dst, n_dst) != n_dst && lane == 0) pq_err(err, KERR_BAD_PAGE);
         return;
     }
-    int pos = 0, out = 0;
-    uint32_t ulen = 0;                                    // preamble: uncompressed length
-    for (int sh = 0; pos < n_src && sh < 35; sh += 7) {
-        const uint8_t b = src[pos++];
-        ulen |= (uint32_t)(b & 0x7f) << sh;
-        if (!(b & 0x80)) break;
-    }
-    bool bad = (int)ulen != n_dst;
-    while (!bad && pos < n_src) {
-        const uint32_t tag = src[pos];
-        int len, offset = 0;
-        if ((tag & 3) == 0) {
-            len = (int)(tag >> 2) + 1;
-            pos += 1;
-            if (len > 60) {
-                const int extra = len - 60;
-                if (pos + extra > n_src) { bad = true; break; }
-                len = 0;
-                for (int b = 0; b < extra; b++) len |= (int)src[pos + b] << (8 * b);
-                len += 1;
-                pos += extra;
-            }
-            if (len < 0 || pos + len > n_src || out + len > n_dst) { bad = true; break; }
-            for (int i = lane; i < len; i += 32) dst[out + i] = src[pos + i];
-            pos += len;
-        } else {
-            if ((tag & 3) == 1) {
-                if (pos + 2 > n_src) { bad = true; break; }
-                len = 4 + (int)((tag >> 2) & 7);
-                offset = (int)((tag >> 5) << 8) | src[pos + 1];
-                pos += 2;
-            } else if ((tag & 3) == 2) {
-                if (pos + 3 > n_src) { bad = true; break; }
-                len = 1 + (int)(tag >> 2);
-                offset = src[pos + 1] | (src[pos + 2] << 8);
-                pos += 3;
-            } else {
-                if (pos + 5 > n_src) { bad = true; break; }
-                len = 1 + (int)(tag >> 2);
-                offset = (int)(src[pos + 1] | (src[pos + 2] << 8) | (src[pos + 3] << 16) | ((uint32_t)src[pos + 4] << 24));
-                pos += 5;
-            }
-            if (offset <= 0 || offset > out || out + len > n_dst) { bad = true; break; }
-            const uint8_t *from = dst + out - offset;
-            for (int i = lane; i < len; i += 32) dst[out + i] = from[i % offset];
-        }
-        out += len;
-        __syncwarp();                                    // later copies may read what other lanes just wrote
-    }
-    if ((bad || out != n_dst) && lane == 0) pq_err(err, KERR_BAD_PAGE);
+    if (snappy::decode(src, n_src, dst, n_dst) != n_dst && lane == 0) pq_err(err, KERR_BAD_PAGE);
 }
 
 // ------------------------------------------------------------------ Zstandard / GZIP page decompression

@@ -6,14 +6,14 @@
 // Zstandard format specification (RFC 8878): frame header, raw / RLE / compressed blocks, literals section (raw, RLE,
 // Huffman with 1 or 4 streams, treeless), Huffman tree descriptions (direct or FSE-compressed weights), sequences
 // section (predefined / RLE / FSE-compressed / repeat tables, three interleaved FSE states read from a backward
-// bit stream, repeat offsets) and sequence execution.  No dictionaries (Parquet pages never use them), checksums
-// are skipped, skippable frames are skipped.
+// bit stream, repeat offsets) and sequence execution.  No dictionaries (Parquet pages never use them), content
+// checksums are skipped, skippable frames are skipped; a frame that declares its content size must produce exactly it.
 //
 // One decoder instance = one page = one warp on the device: every lane runs the same control flow over the same
 // bytes (the stream is inherently sequential), byte moves are lane-parallel (literal copies, match copies — a match
 // may overlap its own output: byte i comes from out - offset + (i mod offset)) and the four Huffman literal streams
 // are decoded by four lanes.  The same source compiles for the host (tests/zstd_host_check.cc pins it against
-// pyarrow-compressed buffers without a GPU).
+// pyarrow-compressed buffers without a GPU; tests/test_codecs_cpu.py fuzzes it under sanitizers against libzstd).
 #pragma once
 
 #include <stdint.h>
@@ -595,6 +595,7 @@ ZS_HD inline int64_t decode(const uint8_t *src, int64_t n, uint8_t *dst, int64_t
         if ((magic & 0xFFFFFFF0u) == 0x184D2A50u) {         // skippable frame
             if (n - pos < 8) return -1;
             const uint32_t sz = src[pos + 4] | (src[pos + 5] << 8) | (src[pos + 6] << 16) | ((uint32_t)src[pos + 7] << 24);
+            if ((int64_t)sz > n - pos - 8) return -1;
             pos += 8 + (int64_t)sz;
             continue;
         }
@@ -608,8 +609,12 @@ ZS_HD inline int64_t decode(const uint8_t *src, int64_t n, uint8_t *dst, int64_t
         const int did_bytes = did_flag == 0 ? 0 : (did_flag == 1 ? 1 : (did_flag == 2 ? 2 : 4));
         for (int i = 0; i < did_bytes; i++) if (pos + i < n && src[pos + i]) return -1;   // dictionaries: not in Parquet pages
         pos += did_bytes;
-        pos += fcs_flag == 0 ? (single ? 1 : 0) : (fcs_flag == 1 ? 2 : (fcs_flag == 2 ? 4 : 8));
-        if (pos > n) return -1;
+        const int fcs_bytes = fcs_flag == 0 ? (single ? 1 : 0) : (fcs_flag == 1 ? 2 : (fcs_flag == 2 ? 4 : 8));
+        if (fcs_bytes > n - pos) return -1;
+        uint64_t fcs = 0;                                   // frame content size: the frame must produce exactly it
+        for (int i = 0; i < fcs_bytes; i++) fcs |= (uint64_t)src[pos + i] << (8 * i);
+        if (fcs_bytes == 2) fcs += 256;
+        pos += fcs_bytes;
         FrameState F;
         F.rep[0] = 1; F.rep[1] = 4; F.rep[2] = 8;
         warp_sync();
@@ -638,6 +643,7 @@ ZS_HD inline int64_t decode(const uint8_t *src, int64_t n, uint8_t *dst, int64_t
             } else return -1;
             if (last) break;
         }
+        if (fcs_bytes && (uint64_t)(out - frame_out) != fcs) return -1;
         if (checksum) pos += 4;
         if (pos > n) return -1;
     }

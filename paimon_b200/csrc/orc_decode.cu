@@ -16,8 +16,6 @@
 #include <memory>
 #include <stdexcept>
 
-#include "inflate_device.cuh"
-#include "lz4_device.cuh"
 #include "orc_device.cuh"
 #include "orc_meta.h"
 #include "scan_kernels.cuh"
@@ -45,7 +43,6 @@ constexpr int kOrcWarps = 4;
 __global__ void __launch_bounds__(kOrcWarps * 32, 4)
 k_orc_inflate(OrcStream *streams, int n_streams, uint8_t *lit_scratch, int32_t *counter, int32_t *err) {
     __shared__ zs::Tables ZT[kOrcWarps];               // (the DEFLATE tables are smaller and overlay them)
-    static_assert(sizeof(inflate::Tables) <= sizeof(zs::Tables), "tables overlay");
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint8_t *lit = lit_scratch + ((size_t)blockIdx.x * kOrcWarps + w) * (size_t)(zs::kMaxBlock + 64);
     while (true) {
@@ -54,41 +51,15 @@ k_orc_inflate(OrcStream *streams, int n_streams, uint8_t *lit_scratch, int32_t *
         j = __shfl_sync(0xffffffffu, j, 0);
         if (j >= n_streams) return;
         OrcStream st = streams[j];
-        const int codec = st.codec;
-        const int64_t block_size = st.block_size;
-        if (codec == orc::C_NONE) {
+        if (st.codec == orc::C_NONE) {
             if (lane == 0) { streams[j].bytes = st.src; streams[j].n = st.length; }
             continue;
         }
-        int64_t pos = 0, out = 0;
-        bool bad = false;
-        while (pos < st.length && !bad) {
-            if (st.length - pos < 3) { bad = true; break; }
-            const uint32_t h = st.src[pos] | (st.src[pos + 1] << 8) | (st.src[pos + 2] << 16);
-            const int64_t len = h >> 1;
-            pos += 3;
-            if (st.length - pos < len) { bad = true; break; }
-            if (h & 1) {
-                if (out + len > st.bound) { bad = true; break; }
-                for (int64_t i = lane; i < len; i += 32) st.dst[out + i] = st.src[pos + i];
-                __syncwarp();
-                out += len;
-            } else {
-                const int64_t cap = min(block_size, st.bound - out);
-                int64_t got;
-                if (codec == orc::C_ZLIB) got = inflate::inflate_raw(st.src + pos, len, st.dst + out, cap, *(inflate::Tables *)&ZT[w], nullptr);
-                else if (codec == orc::C_LZ4) got = lz4::decode_block(st.src + pos, len, st.dst + out, cap);
-                else got = zs::decode(st.src + pos, len, st.dst + out, cap, lit, ZT[w]);
-                __syncwarp();
-                if (got < 0) { bad = true; break; }
-                out += got;
-            }
-            pos += len;
-        }
+        const int64_t out = orcdev::inflate_chunks(st.src, st.length, st.codec, st.block_size, st.dst, st.bound, ZT[w], lit);
         if (lane == 0) {
-            if (bad) atomicCAS(err, KERR_NONE, KERR_BAD_PAGE);
+            if (out < 0) atomicCAS(err, KERR_NONE, KERR_BAD_PAGE);
             streams[j].bytes = st.dst;
-            streams[j].n = bad ? 0 : out;
+            streams[j].n = out < 0 ? 0 : out;
         }
     }
 }

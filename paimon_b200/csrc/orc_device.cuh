@@ -14,6 +14,10 @@
 
 #include <stdint.h>
 
+#include "inflate_device.cuh"
+#include "lz4_device.cuh"
+#include "zstd_device.cuh"
+
 #if defined(__CUDACC__)
 #define ORC_HD __host__ __device__
 #else
@@ -25,6 +29,68 @@ namespace orcdev {
 enum : int { T_BOOLEAN = 0, T_BYTE = 1, T_SHORT = 2, T_INT = 3, T_LONG = 4, T_FLOAT = 5, T_DOUBLE = 6, T_STRING = 7, T_BINARY = 8,
              T_TIMESTAMP = 9, T_DECIMAL = 14, T_DATE = 15, T_VARCHAR = 16, T_CHAR = 17 };
 enum : int { ENC_DIRECT = 0, ENC_DICTIONARY = 1, ENC_DIRECT_V2 = 2, ENC_DICTIONARY_V2 = 3 };
+enum : int { COMP_ZLIB = 1, COMP_LZ4 = 4, COMP_ZSTD = 5 };              // CompressionKind
+
+// ---- compression chunks.  A stream or metadata section of a compressed file is a sequence of [3-byte header:
+// length << 1 | isOriginal][length bytes]: an original chunk is stored as is, any other is one raw DEFLATE (ZLIB),
+// LZ4 or zstd block that inflates to at most the file's compression block size.
+
+// the bytes the chunks of p[0, n) inflate to at most (DEFLATE cannot expand more than 1032 : 1); -1 when a chunk header
+// or a chunk is cut off
+ORC_HD inline int64_t chunk_bound(const uint8_t *p, int64_t n, int codec, int64_t block) {
+    int64_t pos = 0, bound = 0;
+    while (pos < n) {
+        if (n - pos < 3) return -1;
+        const uint32_t h = p[pos] | (p[pos + 1] << 8) | (p[pos + 2] << 16);
+        const int64_t len = h >> 1;
+        pos += 3;
+        if (n - pos < len) return -1;
+        if (h & 1) bound += len;
+        else if (codec == COMP_ZLIB) bound += block < len * 1032 + 64 ? block : len * 1032 + 64;
+        else bound += block;
+        pos += len;
+    }
+    return bound;
+}
+
+// the chunks of p[0, n) -> dst[0, cap): the bytes produced, or -1 when a chunk is cut off, does not inflate or does not
+// fit.  On the device a whole warp calls it (the decoders are warp-cooperative; T and lit are the warp's); the DEFLATE
+// tables overlay T.
+ORC_HD inline int64_t inflate_chunks(const uint8_t *p, int64_t n, int codec, int64_t block, uint8_t *dst, int64_t cap,
+                                     zs::Tables &T, uint8_t *lit) {
+    static_assert(sizeof(inflate::Tables) <= sizeof(zs::Tables), "tables overlay");
+    int64_t pos = 0, out = 0;
+    while (pos < n) {
+        if (n - pos < 3) return -1;
+        const uint32_t h = p[pos] | (p[pos + 1] << 8) | (p[pos + 2] << 16);
+        const int64_t len = h >> 1;
+        pos += 3;
+        if (n - pos < len) return -1;
+        if (h & 1) {
+            if (out + len > cap) return -1;
+#if defined(__CUDA_ARCH__)
+            for (int64_t i = threadIdx.x & 31; i < len; i += 32) dst[out + i] = p[pos + i];
+            __syncwarp();
+#else
+            for (int64_t i = 0; i < len; i++) dst[out + i] = p[pos + i];
+#endif
+            out += len;
+        } else {
+            const int64_t lim = block < cap - out ? block : cap - out;
+            int64_t got;
+            if (codec == COMP_ZLIB) got = inflate::inflate_raw(p + pos, len, dst + out, lim, *(inflate::Tables *)&T, nullptr);
+            else if (codec == COMP_LZ4) got = lz4::decode_block(p + pos, len, dst + out, lim);
+            else got = zs::decode(p + pos, len, dst + out, lim, lit, T);
+#if defined(__CUDA_ARCH__)
+            __syncwarp();
+#endif
+            if (got < 0) return -1;
+            out += got;
+        }
+        pos += len;
+    }
+    return out;
+}
 
 struct Src {
     const uint8_t *p;

@@ -7,9 +7,7 @@
 #include <memory>
 #include <stdexcept>
 
-#include "inflate_device.cuh"
-#include "lz4_device.cuh"
-#include "zstd_device.cuh"
+#include "orc_device.cuh"
 #include "zstd_encode_device.cuh"
 
 namespace orc {
@@ -62,33 +60,19 @@ struct Pb {
     }
 };
 
-// a metadata section stored as compression chunks: [3-byte header: length << 1 | isOriginal][bytes]...
+// a metadata section stored as compression chunks
 std::vector<uint8_t> inflate_section(const uint8_t *p, uint64_t n, int codec, uint64_t block_size) {
     if (codec == C_NONE) return std::vector<uint8_t>(p, p + n);
     if (codec != C_ZLIB && codec != C_ZSTD && codec != C_LZ4)
         throw std::runtime_error("orc: compression kind " + std::to_string(codec) + " is not decoded (NONE, ZLIB, LZ4 and ZSTD are)");
-    std::vector<uint8_t> out;
-    std::vector<uint8_t> buf(block_size + 64), lit(zs::kMaxBlock + 64);
-    inflate::Tables it;
+    const int64_t bound = orcdev::chunk_bound(p, (int64_t)n, codec, (int64_t)block_size);
+    if (bound < 0) throw std::runtime_error("orc: truncated compression chunk");
+    std::vector<uint8_t> out((size_t)bound), lit(zs::kMaxBlock + 64);
     static thread_local zs::Tables *zt = nullptr;
     if (!zt) zt = new zs::Tables();
-    uint64_t pos = 0;
-    while (pos < n) {
-        if (n - pos < 3) throw std::runtime_error("orc: truncated compression chunk header");
-        const uint32_t h = p[pos] | (p[pos + 1] << 8) | (p[pos + 2] << 16);
-        const uint32_t len = h >> 1;
-        pos += 3;
-        if (n - pos < len) throw std::runtime_error("orc: truncated compression chunk");
-        if (h & 1) out.insert(out.end(), p + pos, p + pos + len);
-        else {
-            const int64_t got = codec == C_ZLIB  ? inflate::inflate_raw(p + pos, len, buf.data(), (int64_t)block_size, it, nullptr)
-                                : codec == C_LZ4 ? lz4::decode_block(p + pos, len, buf.data(), (int64_t)block_size)
-                                                 : zs::decode(p + pos, len, buf.data(), (int64_t)block_size, lit.data(), *zt);
-            if (got < 0) throw std::runtime_error("orc: a metadata compression chunk does not inflate");
-            out.insert(out.end(), buf.data(), buf.data() + got);
-        }
-        pos += len;
-    }
+    const int64_t got = orcdev::inflate_chunks(p, (int64_t)n, codec, (int64_t)block_size, out.data(), bound, *zt, lit.data());
+    if (got < 0) throw std::runtime_error("orc: a metadata compression chunk does not inflate");
+    out.resize((size_t)got);
     return out;
 }
 
@@ -246,21 +230,10 @@ Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::
                 ps.length = s.length;
                 if (t.compression == C_NONE) ps.out_bound = s.length;
                 else {
-                    // walk the chunk headers: an original chunk keeps its size, a compressed one inflates to at most
-                    // the block size (DEFLATE cannot expand more than 1032 : 1)
-                    uint64_t pos = 0, bound = 0;
-                    while (pos < s.length) {
-                        if (s.length - pos < 3) throw std::runtime_error("orc: truncated compression chunk header");
-                        const uint8_t *h = file + s.offset + pos;
-                        const uint32_t hv = h[0] | (h[1] << 8) | (h[2] << 16);
-                        const uint64_t len = hv >> 1;
-                        if (s.length - pos - 3 < len) throw std::runtime_error("orc: truncated compression chunk");
-                        if (hv & 1) bound += len;
-                        else if (t.compression == C_ZLIB) bound += std::min<uint64_t>(t.block_size, len * 1032 + 64);
-                        else bound += t.block_size;
-                        pos += 3 + len;
-                    }
-                    ps.out_bound = bound;
+                    const int64_t bound = orcdev::chunk_bound(file + s.offset, (int64_t)s.length, t.compression,
+                                                              (int64_t)t.block_size);
+                    if (bound < 0) throw std::runtime_error("orc: truncated compression chunk");
+                    ps.out_bound = (uint64_t)bound;
                 }
                 ps.out_off = pl.scratch_bytes;
                 pl.scratch_bytes += (ps.out_bound + 64 + 63) & ~(uint64_t)63;

@@ -229,34 +229,35 @@ __device__ __forceinline__ void pq_err(int32_t *err, int code) { atomicCAS(err, 
 __host__ __device__ __forceinline__ int64_t pq_al64(int64_t x) { return (x + 63) & ~(int64_t)63; }
 __host__ __device__ __forceinline__ int64_t pq_min64(int64_t a, int64_t b) { return a < b ? a : b; }
 
-// ------------------------------------------------------------------ page walk: one thread per column chunk
+// ------------------------------------------------------------------ page walk: one column chunk
 //
 // VectorizedColumnReader's page loop (:143-383) / ParquetFileReader.Chunk.readAllPages: header, body, next header.
-// FILL = false counts (pages, dictionary entries, scratch bytes); FILL = true writes the page table.
+// FILL = false counts (pages, dictionary entries, scratch bytes) into chunks[c]; FILL = true writes the page table.
+// Returns the first KERR_* the chunk breaks (KERR_NONE when it is well formed).  k_pq_walk runs it on the device, one
+// thread per chunk; pq_open runs the count pass on the host, so that pg_parquet_open refuses what the device would.
 template <bool FILL>
-__global__ void k_pq_walk(PqChunk *chunks, int n_chunks, PqPage *pages, PqPage *dicts, uint8_t *scratch, int32_t *err) {
-    const int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= n_chunks) return;
+__host__ __device__ inline int pq_walk_chunk(PqChunk *chunks, int c, PqPage *pages, PqPage *dicts, uint8_t *scratch) {
     const PqChunk ch = chunks[c];
     const uint8_t *p = ch.base, *end = ch.base + ch.avail;
     int64_t vals = 0, sc = 0, dict_entries = 0, page_bytes = 0;
     int n_pages = 0, n_dicts = 0;
+    int code = KERR_NONE;
     bool needs_ids = false;
     const bool codec_on = ch.codec != pq::C_UNCOMPRESSED;
     while (vals < ch.num_values) {
         PqHeader h;
-        if (p >= end || !pq_parse_header(p, end, h)) { pq_err(err, KERR_PQ_HEADER); break; }
+        if (p >= end || !pq_parse_header(p, end, h)) { code = KERR_PQ_HEADER; break; }
         const uint8_t *body = p + h.hdr;
-        if (h.comp < 0 || h.unc < 0 || h.nv < 0 || (int64_t)(end - body) < (int64_t)h.comp) { pq_err(err, KERR_PQ_HEADER); break; }
+        if (h.comp < 0 || h.unc < 0 || h.nv < 0 || (int64_t)(end - body) < (int64_t)h.comp) { code = KERR_PQ_HEADER; break; }
         if (h.type == pq::P_DICTIONARY) {
             if (n_dicts > 0 || n_pages > 0 || (h.enc != pq::E_PLAIN && h.enc != pq::E_PLAIN_DICTIONARY)) {
-                pq_err(err, KERR_PQ_ENCODING);
+                code = KERR_PQ_ENCODING;
                 break;
             }
             const int body_len = codec_on ? h.unc : h.comp;
             // fixed-width entries are looked up at body + id * width: every entry the header claims must be in the body
             // (BYTE_ARRAY entries are walked and bounded by k_pq_walk_dicts)
-            if ((int64_t)h.nv * ch.phys_width > (int64_t)body_len) { pq_err(err, KERR_BAD_PAGE); break; }
+            if ((int64_t)h.nv * ch.phys_width > (int64_t)body_len) { code = KERR_BAD_PAGE; break; }
             if (FILL) {
                 PqPage d;
                 memset(&d, 0, sizeof(d));
@@ -276,11 +277,11 @@ __global__ void k_pq_walk(PqChunk *chunks, int n_chunks, PqPage *pages, PqPage *
             else if (h.enc == pq::E_PLAIN_DICTIONARY || h.enc == pq::E_RLE_DICTIONARY) enc = ENC_DICT;
             else if (h.enc == pq::E_DELTA_BINARY_PACKED && (ch.phys == pq::T_INT32 || ch.phys == pq::T_INT64)) enc = ENC_DELTA_BP;
             else if (h.enc == pq::E_RLE && ch.phys == pq::T_BOOLEAN) enc = ENC_RLE_BOOL;
-            if (enc < 0 || (enc == ENC_DICT && ch.phys == pq::T_BOOLEAN)) { pq_err(err, KERR_PQ_ENCODING); break; }
-            if (enc == ENC_DICT && n_dicts == 0) { pq_err(err, KERR_PQ_NO_DICT); break; }
+            if (enc < 0 || (enc == ENC_DICT && ch.phys == pq::T_BOOLEAN)) { code = KERR_PQ_ENCODING; break; }
+            if (enc == ENC_DICT && n_dicts == 0) { code = KERR_PQ_NO_DICT; break; }
             const bool v2 = h.type == pq::P_DATA_V2;
             if ((v2 && h.rep_len != 0) || (!v2 && ch.max_def > 0 && h.def_enc != pq::E_RLE) || (v2 && h.def_len < 0)) {
-                pq_err(err, KERR_PQ_LEVELS);
+                code = KERR_PQ_LEVELS;
                 break;
             }
             const bool compressed = codec_on && (!v2 || h.is_compressed);
@@ -307,13 +308,22 @@ __global__ void k_pq_walk(PqChunk *chunks, int n_chunks, PqPage *pages, PqPage *
         }                                                // index pages are skipped
         p = body + h.comp;
     }
-    if (vals != ch.num_values) pq_err(err, KERR_PQ_ROWS);
+    if (code == KERR_NONE && vals != ch.num_values) code = KERR_PQ_ROWS;
     if (!FILL) {
         PqChunk &o = chunks[c];
         o.n_pages = n_pages; o.n_dicts = n_dicts; o.scratch_bytes = sc; o.dict_entries = dict_entries;
         o.ids_entries = needs_ids ? ch.num_values : 0;
         o.page_bytes = page_bytes;
     }
+    return code;
+}
+
+template <bool FILL>
+__global__ void k_pq_walk(PqChunk *chunks, int n_chunks, PqPage *pages, PqPage *dicts, uint8_t *scratch, int32_t *err) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n_chunks) return;
+    const int code = pq_walk_chunk<FILL>(chunks, c, pages, dicts, scratch);
+    if (code != KERR_NONE) pq_err(err, code);
 }
 
 // exclusive scans of the per-chunk counts -> bases; totals[0..5] = pages, dictionary pages, scratch bytes,
@@ -1786,8 +1796,8 @@ struct PqReader {
 
 static Table<PqReader> g_pq(5);
 
-// open = footer + schema check + a host walk of the page headers, so that files the device would refuse are refused
-// here, before any device work (and on a box without a GPU)
+// open = footer + schema check + the page walk's count pass on the host, so that files the device walk would refuse
+// are refused here, before any device work (and on a box without a GPU)
 static pg_status pq_open(uint64_t schema, const uint8_t *bytes, int64_t size, uint64_t *out) {
     std::shared_ptr<Schema> s = g_schemas.get(schema);
     if (!s || !bytes || !out) return fail(PG_ERR_INVALID, "bad schema handle or null argument");
@@ -1798,53 +1808,22 @@ static pg_status pq_open(uint64_t schema, const uint8_t *bytes, int64_t size, ui
     } catch (const std::exception &e) {
         return fail(PG_ERR_FORMAT, e.what());
     }
-    const pq::FileMetaData &m = rd->meta;
     Scratch scratch(nullptr);                          // (stays empty: the columns are resolved by position on the host)
     RunBuilder b(s, 1, scratch, "parquet");
-    pg_status st = map_file_schema(b, m, 0);
+    pg_status st = map_file_schema(b, rd->meta, 0);
     if (st) return st;
-    const int nc = s->n_cols();
-    rd->n_rows = m.num_rows;
-    int64_t row0 = 0;
-    for (const pq::RowGroup &g : m.row_groups) {
-        for (int c = 0; c < nc; c++) {
-            const pq::ColumnChunk &cc = g.columns[c];
-            const int max_def = m.schema[c + 1].repetition == pq::R_OPTIONAL ? 1 : 0;
-            int64_t pos = cc.start(), vals = 0;
-            bool have_dict = false;
-            while (vals < cc.num_values) {
-                if (pos < 4 || pos >= size) return fail(PG_ERR_FORMAT, "parquet: page offset out of range");
-                PqHeader h;
-                if (!pq_parse_header(bytes + pos, bytes + size, h)) return fail(PG_ERR_FORMAT, "parquet: malformed or truncated page header");
-                const int64_t body = pos + h.hdr;
-                if (h.comp < 0 || body + h.comp > size) return fail(PG_ERR_FORMAT, "parquet: truncated page");
-                if (h.type == pq::P_DICTIONARY) {
-                    if (h.enc != pq::E_PLAIN && h.enc != pq::E_PLAIN_DICTIONARY)
-                        return fail(PG_ERR_UNSUPPORTED, "parquet: dictionary page encoding");
-                    have_dict = true;
-                    rd->n_dict_pages++;
-                } else if (h.type == pq::P_DATA || h.type == pq::P_DATA_V2) {
-                    const bool is_dict = h.enc == pq::E_PLAIN_DICTIONARY || h.enc == pq::E_RLE_DICTIONARY;
-                    const bool is_delta = h.enc == pq::E_DELTA_BINARY_PACKED && (cc.type == pq::T_INT32 || cc.type == pq::T_INT64);
-                    const bool is_rle_bool = h.enc == pq::E_RLE && cc.type == pq::T_BOOLEAN;
-                    if (!is_dict && !is_delta && !is_rle_bool && h.enc != pq::E_PLAIN)
-                        return fail(PG_ERR_UNSUPPORTED, "parquet: value encoding " + std::to_string(h.enc) +
-                                                        " (PLAIN, dictionary, DELTA_BINARY_PACKED integers and RLE booleans "
-                                                        "are decoded on device)");
-                    if (is_dict && !have_dict) return fail(PG_ERR_FORMAT, "parquet: dictionary-encoded page without dictionary");
-                    if (h.type == pq::P_DATA_V2 && h.rep_len != 0) return fail(PG_ERR_UNSUPPORTED, "parquet: repetition levels");
-                    if (h.type == pq::P_DATA && max_def > 0 && h.def_enc != pq::E_RLE)
-                        return fail(PG_ERR_UNSUPPORTED, "parquet: BIT_PACKED definition levels");
-                    rd->n_data_pages++;
-                    vals += h.nv;
-                }                                        // index pages are skipped
-                pos = body + h.comp;
-            }
-            if (vals != g.num_rows) return fail(PG_ERR_FORMAT, "parquet: page row counts do not add up");
-        }
-        row0 += g.num_rows;
+    // the chunk table and the count pass of the section decode, over the host bytes
+    const std::vector<SectionFile> files{SectionFile{bytes, size, PG_MEM_HOST, 0, &rd->meta}};
+    ChunkTables ct;
+    st = build_chunk_tables(s.get(), files, {bytes}, {&rd->meta}, b, ct);
+    if (st) return st;
+    for (int c = 0; c < (int)ct.chunks.size(); c++) {
+        st = kernel_error_status(pq_walk_chunk<false>(ct.chunks.data(), c, nullptr, nullptr, nullptr));
+        if (st) return st;
+        rd->n_data_pages += ct.chunks[c].n_pages;
+        rd->n_dict_pages += ct.chunks[c].n_dicts;
     }
-    if (row0 != m.num_rows) return fail(PG_ERR_FORMAT, "parquet: row group row counts do not add up");
+    rd->n_rows = rd->meta.num_rows;
     rd->file.assign(bytes, bytes + size);
     *out = g_pq.put(std::move(rd));
     return PG_OK;

@@ -12,8 +12,9 @@
 // One decoder instance = one page = one warp on the device: every lane runs the same control flow over the same
 // bytes (the stream is inherently sequential), byte moves are lane-parallel (literal copies, match copies — a match
 // may overlap its own output: byte i comes from out - offset + (i mod offset)) and the four Huffman literal streams
-// are decoded by four lanes.  The same source compiles for the host (tests/zstd_host_check.cc pins it against
-// pyarrow-compressed buffers without a GPU; tests/test_codecs_cpu.py fuzzes it under sanitizers against libzstd).
+// are decoded by four lanes.  The same source compiles for the host (tests/native/codec_host_check.cc runs it under
+// sanitizers: tests/test_zstd_cpu.py pins it against pyarrow-compressed buffers, tests/test_codecs_cpu.py fuzzes it
+// against libzstd).
 #pragma once
 
 #include <stdint.h>

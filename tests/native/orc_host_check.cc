@@ -1,18 +1,17 @@
-// Host build of the ORC decode path: orc_meta.cc (metadata + plan), inflate_device.cuh / zstd_device.cuh (compression
-// chunks) and orc_device.cuh (stream decoders, task phases A and B) — the same sources the device path compiles —
-// driven serially on the host.  tests/test_orc_cpu.py pins the result against pyarrow.orc and the reference's golden
-// ORC files without a GPU.  Flat schemas; the caller names the output width of every column (0 = var-len).
+// Host build of the ORC decode path: orc_meta.cc (metadata + plan) and orc_device.cuh (compression chunks under ZLIB,
+// LZ4 and ZSTD, stream decoders, task phases A and B) — the same sources the device path compiles — driven serially on
+// the host.  tests/test_orc_cpu.py pins the result against pyarrow.orc and the reference's golden ORC files without a
+// GPU.  Flat schemas; the caller names the output width of every column (0 = var-len).
 #include <stdlib.h>
 #include <string.h>
 
+#include <memory>
 #include <stdexcept>
 #include <string>
 #include <vector>
 
-#include "inflate_device.cuh"
 #include "orc_device.cuh"
 #include "orc_meta.h"
-#include "zstd_device.cuh"
 
 namespace {
 
@@ -24,29 +23,6 @@ struct Result {
     std::string error;
     std::vector<int> kinds;
 };
-
-// a stream stored as compression chunks -> contiguous bytes
-int64_t inflate_stream(const uint8_t *p, uint64_t n, int codec, uint64_t block, uint8_t *dst, uint64_t cap) {
-    if (codec == orc::C_NONE) { memcpy(dst, p, n); return (int64_t)n; }
-    inflate::Tables it;
-    static zs::Tables zt;
-    std::vector<uint8_t> lit(zs::kMaxBlock + 64);
-    uint64_t pos = 0, out = 0;
-    while (pos < n) {
-        const uint32_t h = p[pos] | (p[pos + 1] << 8) | (p[pos + 2] << 16);
-        const uint32_t len = h >> 1;
-        pos += 3;
-        if (h & 1) { if (out + len > cap) return -1; memcpy(dst + out, p + pos, len); out += len; }
-        else {
-            const int64_t got = codec == orc::C_ZLIB ? inflate::inflate_raw(p + pos, len, dst + out, (int64_t)std::min<uint64_t>(block, cap - out), it, nullptr)
-                                                     : zs::decode(p + pos, len, dst + out, (int64_t)std::min<uint64_t>(block, cap - out), lit.data(), zt);
-            if (got < 0) return -1;
-            out += got;
-        }
-        pos += len;
-    }
-    return (int64_t)out;
-}
 
 }  // namespace
 
@@ -66,9 +42,15 @@ void *orc_host_decode(const unsigned char *file, long long size, int n_cols, con
         orc::Plan pl = orc::plan_file(t, file, size, cols);
         std::vector<uint8_t> scratch(pl.scratch_bytes + 64);
         std::vector<int64_t> slen(pl.streams.size());
+        std::unique_ptr<zs::Tables> zt(new zs::Tables());
+        std::vector<uint8_t> lit(zs::kMaxBlock + 64);
         for (size_t i = 0; i < pl.streams.size(); i++) {
             const orc::PlanStream &ps = pl.streams[i];
-            slen[i] = inflate_stream(file + ps.offset, ps.length, t.compression, t.block_size, scratch.data() + ps.out_off, ps.out_bound);
+            const uint8_t *src = file + ps.offset;
+            uint8_t *dst = scratch.data() + ps.out_off;
+            if (t.compression == orc::C_NONE) { memcpy(dst, src, ps.length); slen[i] = (int64_t)ps.length; }
+            else slen[i] = orcdev::inflate_chunks(src, (int64_t)ps.length, t.compression, (int64_t)t.block_size, dst,
+                                                  (int64_t)ps.out_bound, *zt, lit.data());
             if (slen[i] < 0) throw std::runtime_error("a stream does not inflate");
         }
         const int64_t n = (int64_t)t.rows;

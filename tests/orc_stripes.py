@@ -1113,6 +1113,7 @@ def malformed_cases():
         "chunk_past_stream": _chunk_past_stream,
         "chunk_not_inflating_zlib": _chunk_not_inflating(ZLIB),
         "chunk_not_inflating_zstd": _chunk_not_inflating(ZSTD),
+        "chunk_not_inflating_lz4": _chunk_not_inflating(LZ4),
         "decimal_scale_negative_huge": _decimal_scale(-(1 << 62)),
         "decimal_scale_negative": _decimal_scale(-1),
         "decimal_scale_39": _decimal_scale(39),

@@ -10,12 +10,11 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _NP = {1: np.int8, 2: np.int16, 4: np.int32, 8: np.int64}
 
 
-def build(tmp_dir: str, harness: str = "orc_host_check.cc"):
-    """harness: orc_host_check.cc (NONE, ZLIB, ZSTD chunks) or orc_lz4_host_check.cc (LZ4 chunks too)"""
-    so = os.path.join(tmp_dir, os.path.splitext(harness)[0] + ".so")
+def build(tmp_dir: str):
+    so = os.path.join(tmp_dir, "orc_host_check.so")
     csrc = os.path.join(ROOT, "paimon_b200", "csrc")
     subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-I" + csrc, "-o", so,
-                           os.path.join(ROOT, "tests", "native", harness), os.path.join(csrc, "orc_meta.cc")])
+                           os.path.join(ROOT, "tests", "native", "orc_host_check.cc"), os.path.join(csrc, "orc_meta.cc")])
     lib = C.CDLL(so)
     lib.orc_host_decode.restype = C.c_void_p
     lib.orc_host_decode.argtypes = [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p]

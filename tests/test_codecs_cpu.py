@@ -1,6 +1,6 @@
 """The Snappy, zstd and DEFLATE page decompressors (snappy_device.cuh, zstd_device.cuh, inflate_device.cuh) compiled for
 the HOST from the same sources the device kernels use, under AddressSanitizer and UBSan, with every buffer allocated
-at its exact size (tests/native/codec_host_check.cc).
+at its exact size (tests/native/codec_host_check.cc, run through codec_filter.py).
 
 - Snappy: hand-built streams (snappy_streams.py) at every literal-length and copy boundary, decoded equal to the
   writer and to libsnappy; one malformed stream per refusal rule.
@@ -11,43 +11,21 @@ at its exact size (tests/native/codec_host_check.cc).
 - The checks the decoders skip (gzip CRC32 and header CRC16, zlib Adler-32, zstd content checksum), compared with the
   reference with the check off, and the gzip ISIZE, which is checked."""
 import gzip
-import os
 import random
 import struct
-import subprocess
 import zlib
 
 import pytest
 
 import codec_corpora as K
+import codec_filter
 import snappy_streams as S
 from codec_corpora import GZIP, RAW_DEFLATE, SNAPPY, ZLIB, ZSTD, reference
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 @pytest.fixture(scope="module")
 def codec(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("codecs") / "codec_host_check")
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fsanitize=address,undefined", "-fno-sanitize-recover=all",
-                           "-I" + os.path.join(ROOT, "paimon_b200", "csrc"), "-o", exe,
-                           os.path.join(ROOT, "tests", "native", "codec_host_check.cc")])
-
-    def run(records):
-        """records: (mode, src bytes, cap) -> [(result, output bytes)]"""
-        inp = b"".join(struct.pack("<Bqq", m, cap, len(src)) + bytes(src) for m, src, cap in records)
-        env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0:abort_on_error=0", UBSAN_OPTIONS="print_stacktrace=1")
-        p = subprocess.run([exe], input=inp, capture_output=True, env=env)
-        assert p.returncode == 0, p.stderr.decode(errors="replace")[-3000:]
-        out, pos = [], 0
-        for _ in records:
-            (r,) = struct.unpack_from("<q", p.stdout, pos)
-            pos += 8
-            out.append((r, p.stdout[pos:pos + max(r, 0)]))
-            pos += max(r, 0)
-        assert pos == len(p.stdout)
-        return out
-    return run
+    return codec_filter.build(str(tmp_path_factory.mktemp("codecs")))
 
 
 # ------------------------------------------------------------------ Snappy

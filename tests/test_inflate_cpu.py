@@ -2,36 +2,24 @@
 source the device kernels use, pinned against zlib: stored, fixed and dynamic Huffman blocks, long and overlapping
 matches, every compression level, raw / zlib / gzip framing (ORC ZLIB chunks are raw DEFLATE, Parquet GZIP pages are
 gzip members)."""
-import ctypes as C
 import gzip
-import os
 import random
-import subprocess
 import zlib
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import codec_filter
+from codec_corpora import GZIP, RAW_DEFLATE, ZLIB
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("inflate") / "libif_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-I" + os.path.join(ROOT, "paimon_b200", "csrc"),
-                           "-o", so, os.path.join(ROOT, "tests", "native", "inflate_host_check.cc")])
-    lib = C.CDLL(so)
-    for fn in ("if_host_raw", "if_host_gzip", "if_host_zlib"):
-        getattr(lib, fn).restype = C.c_longlong
-        getattr(lib, fn).argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong]
-    return lib
+def codec(tmp_path_factory):
+    return codec_filter.build(str(tmp_path_factory.mktemp("inflate")))
 
 
-def run(fn, comp: bytes, n: int, cap=None):
-    src = np.frombuffer(comp, np.uint8)
-    dst = np.zeros(n + 64, np.uint8)
-    r = fn(src.ctypes.data, len(src), dst.ctypes.data, n if cap is None else cap)
-    return r, dst[:max(r, 0)].tobytes()
+def run(codec, mode, comp: bytes, n: int, cap=None):
+    return codec([(mode, comp, n if cap is None else cap)])[0]
 
 
 def corpus():
@@ -50,37 +38,37 @@ def corpus():
 
 
 @pytest.mark.parametrize("level", [0, 1, 6, 9])
-def test_decoder_matches_zlib(lib, level):
+def test_decoder_matches_zlib(codec, level):
     for name, data in corpus():
         co = zlib.compressobj(level, zlib.DEFLATED, -15)
         raw = co.compress(data) + co.flush()
-        r, out = run(lib.if_host_raw, raw, len(data))
+        r, out = run(codec, RAW_DEFLATE, raw, len(data))
         assert r == len(data) and out == data, f"raw {name} level {level}"
-        r, out = run(lib.if_host_zlib, zlib.compress(data, level), len(data))
+        r, out = run(codec, ZLIB, zlib.compress(data, level), len(data))
         assert r == len(data) and out == data, f"zlib {name} level {level}"
-        r, out = run(lib.if_host_gzip, gzip.compress(data, compresslevel=level), len(data))
+        r, out = run(codec, GZIP, gzip.compress(data, compresslevel=level), len(data))
         assert r == len(data) and out == data, f"gzip {name} level {level}"
 
 
-def test_fixed_huffman_blocks(lib):
+def test_fixed_huffman_blocks(codec):
     data = b"abcabcabc hello hello"
     co = zlib.compressobj(9, zlib.DEFLATED, -15, 9, zlib.Z_FIXED)
     raw = co.compress(data) + co.flush()
-    r, out = run(lib.if_host_raw, raw, len(data))
+    r, out = run(codec, RAW_DEFLATE, raw, len(data))
     assert r == len(data) and out == data
 
 
-def test_malformed_streams_are_rejected(lib):
+def test_malformed_streams_are_rejected(codec):
     data = b"hello hello hello hello " * 100
     co = zlib.compressobj(6, zlib.DEFLATED, -15)
     raw = bytearray(co.compress(data) + co.flush())
-    assert run(lib.if_host_raw, bytes(raw), len(data))[0] == len(data)
-    assert run(lib.if_host_raw, bytes(raw), len(data), cap=len(data) - 1)[0] == -1
-    assert run(lib.if_host_raw, bytes(raw[:-4]), len(data))[0] == -1
+    assert run(codec, RAW_DEFLATE, bytes(raw), len(data))[0] == len(data)
+    assert run(codec, RAW_DEFLATE, bytes(raw), len(data), cap=len(data) - 1)[0] == -1
+    assert run(codec, RAW_DEFLATE, bytes(raw[:-4]), len(data))[0] == -1
     rng = random.Random(2)
     for _ in range(300):
         bad = bytearray(raw)
         for _ in range(rng.randrange(1, 4)):
             bad[rng.randrange(len(bad))] = rng.randrange(256)
-        r, _ = run(lib.if_host_raw, bytes(bad), len(data))
+        r, _ = run(codec, RAW_DEFLATE, bytes(bad), len(data))
         assert r == -1 or 0 <= r <= len(data)

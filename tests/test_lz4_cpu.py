@@ -2,45 +2,24 @@
 under AddressSanitizer and UBSan, pinned against pyarrow's lz4_raw codec (liblz4's safe decoder): round trips of the
 zstd corpus and of the C3 / C5 page bodies, hand-built blocks at every length, offset and end-of-block boundary,
 byte-flip and truncation fuzz, and the Hadoop block / chunk framing of Parquet codec 5 pages."""
-import os
 import random
 import struct
-import subprocess
 
 import numpy as np
 import pyarrow as pa
 import pytest
 
+import codec_filter
 from lz4_parquet import HADOOP_LZ4_CHUNK, lz4_hadoop
 from test_zstd_cpu import corpus
 from zstd_pages import c3_pages, c5_pages
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-RAW, HADOOP = 0, 1
+RAW, HADOOP = codec_filter.LZ4_RAW, codec_filter.LZ4_HADOOP
 
 
 @pytest.fixture(scope="module")
 def lz4(tmp_path_factory):
-    exe = str(tmp_path_factory.mktemp("lz4") / "lz4_host_check")
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fsanitize=address,undefined", "-fno-sanitize-recover=all",
-                           "-I" + os.path.join(ROOT, "paimon_b200", "csrc"), "-o", exe,
-                           os.path.join(ROOT, "tests", "native", "lz4_host_check.cc")])
-
-    def run(records):
-        """records: (mode, src bytes, cap) -> [(result, output bytes)]"""
-        inp = b"".join(struct.pack("<Bqq", m, cap, len(src)) + bytes(src) for m, src, cap in records)
-        env = dict(os.environ, ASAN_OPTIONS="detect_leaks=0:abort_on_error=0", UBSAN_OPTIONS="print_stacktrace=1")
-        p = subprocess.run([exe], input=inp, capture_output=True, env=env)
-        assert p.returncode == 0, p.stderr.decode(errors="replace")[-3000:]
-        out, pos = [], 0
-        for _ in records:
-            (r,) = struct.unpack_from("<q", p.stdout, pos)
-            pos += 8
-            out.append((r, p.stdout[pos:pos + max(r, 0)]))
-            pos += max(r, 0)
-        assert pos == len(p.stdout)
-        return out
-    return run
+    return codec_filter.build(str(tmp_path_factory.mktemp("lz4")))
 
 
 def pyarrow_lz4(block: bytes, size: int):

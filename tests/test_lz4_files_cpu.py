@@ -1,13 +1,11 @@
-"""LZ4 files on the host, without a GPU: the ORC host build (tests/native/orc_lz4_host_check.cc over orc_meta.cc +
-lz4_device.cuh + orc_device.cuh, the sources the device path compiles) decodes pyarrow.orc files written with compression="lz4" (CompressionKind 4: one raw LZ4 block
-per compression chunk, the footers too) of every KeyValue type at several compression block sizes, equal to pyarrow;
-and pg_parquet_open accepts Parquet codec 5 (Hadoop-framed LZ4) files with pyarrow's counts, while codec 7 (LZ4_RAW)
-stays refused."""
+"""LZ4 files on the host, without a GPU: the ORC host build (tests/native/orc_host_check.cc over orc_meta.cc +
+orc_device.cuh, the sources the device path compiles) decodes pyarrow.orc files written with compression="lz4"
+(CompressionKind 4: one raw LZ4 block per compression chunk, the footers too) of every KeyValue type at several
+compression block sizes, equal to pyarrow; and pg_parquet_open accepts Parquet codec 5 (Hadoop-framed LZ4) files with
+pyarrow's counts, while codec 7 (LZ4_RAW) stays refused."""
 import ctypes as C
 import io
-import os
 import struct
-import subprocess
 
 import numpy as np
 import pyarrow.parquet as pq
@@ -26,26 +24,7 @@ from parquet_util import write_kv_parquet
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    """orc_util.build's library, from the harness that also decodes LZ4 chunks"""
-    so = str(tmp_path_factory.mktemp("orc_lz4") / "liborc_lz4_host.so")
-    csrc = os.path.join(orc_util.ROOT, "paimon_b200", "csrc")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-I" + csrc, "-o", so,
-                           os.path.join(orc_util.ROOT, "tests", "native", "orc_lz4_host_check.cc"),
-                           os.path.join(csrc, "orc_meta.cc")])
-    lib = C.CDLL(so)
-    lib.orc_host_decode.restype = C.c_void_p
-    lib.orc_host_decode.argtypes = [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p]
-    lib.orc_host_error.restype = C.c_char_p
-    lib.orc_host_rows.restype = C.c_longlong
-    lib.orc_host_rows.argtypes = [C.c_void_p]
-    lib.orc_host_data.restype = C.c_void_p
-    lib.orc_host_data.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_longlong)]
-    lib.orc_host_offsets.restype = C.c_void_p
-    lib.orc_host_offsets.argtypes = [C.c_void_p, C.c_int]
-    lib.orc_host_validity.restype = C.c_void_p
-    lib.orc_host_validity.argtypes = [C.c_void_p, C.c_int]
-    lib.orc_host_free.argtypes = [C.c_void_p]
-    return lib
+    return orc_util.build(str(tmp_path_factory.mktemp("orc_lz4")))
 
 
 @pytest.mark.parametrize("opts", [

@@ -16,13 +16,8 @@ MALFORMED = S.malformed_cases()
 
 
 @pytest.fixture(scope="module")
-def libs(tmp_path_factory):
-    d = str(tmp_path_factory.mktemp("orc_stripes"))
-    return {"plain": orc_util.build(d), "lz4": orc_util.build(d, "orc_lz4_host_check.cc")}
-
-
-def _lib(libs, codec):
-    return libs["lz4" if codec == S.LZ4 else "plain"]
+def lib(tmp_path_factory):
+    return orc_util.build(str(tmp_path_factory.mktemp("orc_stripes")))
 
 
 def _decode(lib, f: S.OrcFile, vtype: str):
@@ -33,11 +28,11 @@ def _decode(lib, f: S.OrcFile, vtype: str):
 
 
 @pytest.mark.parametrize("name", sorted(CASES))
-def test_host_decoder_matches_the_built_stripes(libs, name):
+def test_host_decoder_matches_the_built_stripes(lib, name):
     case = CASES[name]()
     got, key0 = [], 0
     for f in case.files:
-        cols, vals = _decode(_lib(libs, case.codec), f, case.vtype)
+        cols, vals = _decode(lib, f, case.vtype)
         assert cols[3][0].tolist() == list(range(key0, key0 + len(vals)))
         assert cols[1][1].all() and cols[3][1].all()
         got += vals
@@ -50,10 +45,10 @@ def test_host_decoder_matches_the_built_stripes(libs, name):
 
 
 @pytest.mark.parametrize("name", sorted(MALFORMED))
-def test_malformed_stream_is_refused(libs, name):
+def test_malformed_stream_is_refused(lib, name):
     f, vtype = MALFORMED[name]()
     with pytest.raises(RuntimeError):
-        _decode(libs["plain"], f, vtype)
+        _decode(lib, f, vtype)
 
 
 def test_builder_runs_match_the_specification_examples():

@@ -6,11 +6,15 @@ import numpy as np
 import pyarrow.parquet as pq
 import pytest
 
+import parquet_pages as P
 from paimon_b200 import _native as N
 from paimon_b200 import datagen
 from paimon_b200.sort_merge_reader import _SchemaHandle
+from paimon_b200.types import DataField, KeyValueSchema, RowType
 
 from parquet_util import write_kv_parquet
+
+PG_ERR_UNSUPPORTED, PG_ERR_FORMAT = 2, 6
 
 
 def _open(schema_handle, path):
@@ -89,6 +93,32 @@ def test_unsupported_files_are_refused(tmp_path):
     write_kv_parquet(run, p)
     st, _, _ = _open(sh2, p)
     assert st == 2                                                           # column count mismatch
+
+
+def _open_pages_file(data, vtype):
+    """pg_parquet_open's status on a parquet_pages.kv_file (the handles it made are freed)"""
+    lib = N.load()
+    sh = _schema_handle(KeyValueSchema.of(RowType((DataField("pk", "BIGINT", False), DataField("v", vtype, True))), ["pk"]))
+    buf = np.frombuffer(data, np.uint8)
+    h = C.c_uint64(0)
+    st = lib.pg_parquet_open(sh, buf.ctypes.data, len(buf), C.byref(h))
+    if st == 0:
+        assert lib.pg_parquet_free(h.value) == 0
+    assert lib.pg_schema_free(sh) == 0
+    return st
+
+
+def test_open_refuses_what_the_device_page_walk_refuses():
+    """pg_parquet_open runs the page walk of the device decoder on the host.  Of the malformed files, the one whose
+    dictionary page claims more entries than its body holds is refused there; the others break value streams, which
+    only the decode reads.  A dictionary page between two data pages is refused as an encoding the decoder lacks."""
+    statuses = {name: _open_pages_file(*make()) for name, make in P.malformed_cases().items()}
+    assert {k: v for k, v in statuses.items() if v != 0} == {"dict_page_overclaims": PG_ERR_FORMAT}
+    page = lambda vals: P.data_page_v1(len(vals), P.plain(P.INT64, vals), P.E_PLAIN, defs=P.levels([True] * len(vals)))
+    pages = [page(list(range(50))), P.dictionary_page(4, P.plain(P.INT64, [1, 2, 3, 4])), page(list(range(50, 100)))]
+    data = P.kv_file([100], [P.ValueColumn("v", P.INT64, True, [pages])])
+    assert _open_pages_file(data, "BIGINT") == PG_ERR_UNSUPPORTED
+    assert b"encoding" in N.load().pg_last_error()
 
 
 def test_decode_without_device_fails_loudly(tmp_path):

@@ -2,35 +2,25 @@
 the device kernel uses, pinned against libzstd (through pyarrow): every block type, Huffman literals (1 and 4 streams,
 FSE-compressed and direct weights, treeless), predefined / RLE / FSE / repeat sequence tables, repeat offsets, long
 and overlapping matches, multi-block frames, levels 1..19.  zstd-jni (the reference's codec) wraps the same libzstd."""
-import ctypes as C
-import os
 import random
-import subprocess
 
 import numpy as np
 import pyarrow as pa
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import codec_filter
+from codec_corpora import ZSTD
 
 
 @pytest.fixture(scope="module")
 def zs(tmp_path_factory):
-    so = str(tmp_path_factory.mktemp("zs") / "libzs_host.so")
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-I" + os.path.join(ROOT, "paimon_b200", "csrc"),
-                           "-o", so, os.path.join(ROOT, "tests", "native", "zstd_host_check.cc")])
-    lib = C.CDLL(so)
-    lib.zs_host_decode.restype = C.c_longlong
-    lib.zs_host_decode.argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong]
-    return lib
+    return codec_filter.build(str(tmp_path_factory.mktemp("zs")))
 
 
-def roundtrip(lib, data: bytes, level: int) -> bool:
+def roundtrip(codec, data: bytes, level: int) -> bool:
     comp = pa.Codec("zstd", compression_level=level).compress(data, asbytes=True)
-    src = np.frombuffer(comp, np.uint8)
-    dst = np.zeros(len(data) + 64, np.uint8)
-    r = lib.zs_host_decode(src.ctypes.data, len(src), dst.ctypes.data, len(data))
-    return r == len(data) and dst[: len(data)].tobytes() == data
+    [(r, out)] = codec([(ZSTD, comp, len(data))])
+    return r == len(data) and out == data
 
 
 def corpus():
@@ -61,11 +51,9 @@ def test_decoder_matches_libzstd(zs, level):
 def test_malformed_streams_are_rejected(zs):
     data = b"hello hello hello hello " * 100
     comp = bytearray(pa.Codec("zstd", compression_level=3).compress(data, asbytes=True))
-    dst = np.zeros(len(data) + 64, np.uint8)
 
     def run(buf, cap):
-        src = np.frombuffer(bytes(buf), np.uint8)
-        return zs.zs_host_decode(src.ctypes.data, len(src), dst.ctypes.data, cap)
+        return zs([(ZSTD, bytes(buf), cap)])[0][0]
     assert run(comp, len(data)) == len(data)
     assert run(comp, len(data) - 1) == -1                     # does not fit
     assert run(comp[:-3], len(data)) == -1                    # truncated

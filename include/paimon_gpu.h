@@ -352,9 +352,11 @@ pg_status pg_parquet_read_section(uint64_t schema, const pg_file_desc *files, in
  * flat schemas, BOOLEAN / TINYINT / SMALLINT / INT / BIGINT / FLOAT / DOUBLE / DATE / DECIMAL(p <= 18) / STRING-family /
  * BINARY, integer RLE v1 and v2, DIRECT and DICTIONARY string encodings, PRESENT streams, compression NONE / ZLIB /
  * LZ4 / ZSTD; columns are resolved by field name (missing nullable fields -> NULL, integer / float widening).  Timestamps,
- * DECIMAL(p > 18), nested types and the other codecs return PG_ERR_UNSUPPORTED.  The file bytes must be host memory
- * (footers and compression-chunk headers are walked on the host); pg_section_info.n_chunks counts (stripe, column)
- * tasks and n_data_pages counts streams. */
+ * DECIMAL(p > 18), nested types and the other codecs return PG_ERR_UNSUPPORTED.  The file bytes may be host or device
+ * memory, mixed in one section, like pg_parquet_read_section's: device bytes (an upload's descriptors,
+ * pg_parquet_file_device_image of a pg_orc_encode handle) are read in place, and only their tails come to the host, in
+ * at most three rounds of small reads per section; the compression chunks of every file are walked on the device.
+ * pg_section_info.n_chunks counts (stripe, column) tasks and n_data_pages counts streams. */
 pg_status pg_orc_read_section(uint64_t schema, const pg_file_desc *files, int32_t n_files, int32_t n_runs,
                               const char *const *column_names, const uint8_t *read_columns, uint64_t *out_runs,
                               pg_section_info *info);

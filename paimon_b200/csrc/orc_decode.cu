@@ -7,8 +7,11 @@
 // from the public ORC specification in orc_meta.cc / orc_device.cuh).
 //
 // One call decodes a whole SECTION like pg_parquet_read_section: the files of a sorted run are concatenated into one
-// device run.  Host: file tails (protobuf footers, inflated on the host) -> a plan of streams and (stripe, column)
-// tasks.  Device: k_orc_inflate (one warp per stream: compression chunks -> contiguous bytes with the shared
+// device run.  The file bytes may be host memory (copied to the device) or device memory (used in place).  Host: file
+// tails (protobuf footers, inflated on the host; those of device-resident files read back in at most three rounds of
+// small reads) -> a plan of streams and (stripe, column) tasks.  Device: k_orc_walk + k_orc_scan (one thread per
+// stream: the compression chunk headers -> the stream's bound of inflated bytes -> its place in the scratch; one
+// read-back of the total), k_orc_inflate (one warp per stream: compression chunks -> contiguous bytes with the shared
 // DEFLATE / zstd / LZ4 decoders), k_orc_task<0> (one thread per task: PRESENT -> validity, values / lengths), an offsets
 // scan per var-len column, k_orc_task<1> (payload bytes).  The stream decoders are the host-pinned orc_device.cuh.
 #include <algorithm>
@@ -25,8 +28,8 @@ namespace pg {
 
 struct OrcStream {
     const uint8_t *src;        // device: the stream as stored in the file
-    uint8_t *dst;              // scratch image (compressed files)
-    int64_t length, bound;
+    int64_t dst_off;           // compressed files: the inflated stream's place in the scratch (k_orc_scan)
+    int64_t length, bound;     // bound: of the inflated bytes (k_orc_walk)
     int32_t codec;             // orc::Compression of the stream's file (files of a section may differ)
     int32_t block_size;        // compression block size of that file
     const uint8_t *bytes;      // result: contiguous decoded bytes
@@ -37,11 +40,49 @@ struct OrcTaskRef {            // stream table indexes of a task (-1 = absent)
     int32_t s_present, s_data, s_length, s_dict, s_secondary;
 };
 
+// one thread per stream: the bound of the bytes its compression chunks inflate to, from the chunk headers (0 for the
+// streams of uncompressed files, which are read in place); a chunk cut off by the stream's end sets *err
+__global__ void k_orc_walk(OrcStream *streams, int n_streams, int32_t *err) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_streams) return;
+    const OrcStream &st = streams[i];
+    int64_t b = 0;
+    if (st.codec != orc::C_NONE) {
+        b = orcdev::chunk_bound(st.src, st.length, st.codec, st.block_size);
+        if (b < 0) { atomicCAS(err, KERR_NONE, KERR_BAD_PAGE); b = 0; }
+    }
+    streams[i].bound = b;
+}
+
+// one CTA: each compressed stream's scratch offset, 64-byte aligned with 64 bytes of slack behind it (the exclusive
+// scan of the bounds, in stream order); *total = the scratch bytes
+constexpr int kOrcScanThreads = 1024;
+__global__ void __launch_bounds__(kOrcScanThreads) k_orc_scan(OrcStream *streams, int n_streams, int64_t *total) {
+    __shared__ int64_t part[kOrcScanThreads];
+    const int per = (n_streams + kOrcScanThreads - 1) / kOrcScanThreads;
+    const int b = threadIdx.x * per, e = min(b + per, n_streams);
+    auto need = [&](int i) -> int64_t {
+        return streams[i].codec == orc::C_NONE ? 0 : (streams[i].bound + 64 + 63) & ~(int64_t)63;
+    };
+    int64_t s = 0;
+    for (int i = b; i < e; i++) s += need(i);
+    part[threadIdx.x] = s;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int64_t acc = 0;
+        for (int i = 0; i < kOrcScanThreads; i++) { const int64_t t = part[i]; part[i] = acc; acc += t; }
+        *total = acc;
+    }
+    __syncthreads();
+    s = part[threadIdx.x];
+    for (int i = b; i < e; i++) { streams[i].dst_off = s; s += need(i); }
+}
+
 constexpr int kOrcWarps = 4;
 // the grid launches at most 4 CTAs per SM; the bound caps the registers (128) so that all 4 stay resident, which
 // the decoders alone would not (153 registers leave room for 3)
 __global__ void __launch_bounds__(kOrcWarps * 32, 4)
-k_orc_inflate(OrcStream *streams, int n_streams, uint8_t *lit_scratch, int32_t *counter, int32_t *err) {
+k_orc_inflate(OrcStream *streams, int n_streams, uint8_t *scratch, uint8_t *lit_scratch, int32_t *counter, int32_t *err) {
     __shared__ zs::Tables ZT[kOrcWarps];               // (the DEFLATE tables are smaller and overlay them)
     const int w = threadIdx.x >> 5, lane = threadIdx.x & 31;
     uint8_t *lit = lit_scratch + ((size_t)blockIdx.x * kOrcWarps + w) * (size_t)(zs::kMaxBlock + 64);
@@ -55,10 +96,11 @@ k_orc_inflate(OrcStream *streams, int n_streams, uint8_t *lit_scratch, int32_t *
             if (lane == 0) { streams[j].bytes = st.src; streams[j].n = st.length; }
             continue;
         }
-        const int64_t out = orcdev::inflate_chunks(st.src, st.length, st.codec, st.block_size, st.dst, st.bound, ZT[w], lit);
+        uint8_t *dst = scratch + st.dst_off;
+        const int64_t out = orcdev::inflate_chunks(st.src, st.length, st.codec, st.block_size, dst, st.bound, ZT[w], lit);
         if (lane == 0) {
             if (out < 0) atomicCAS(err, KERR_NONE, KERR_BAD_PAGE);
-            streams[j].bytes = st.dst;
+            streams[j].bytes = dst;
             streams[j].n = out < 0 ? 0 : out;
         }
     }
@@ -113,6 +155,22 @@ static bool orc_type_ok(int pg_t, const orc::Type &ty) {
     }
 }
 
+// the tails of the section's device-resident files come back through small reads (readback.cu), so that they do not
+// wait behind another thread's large copies
+struct DeviceRanges : orc::RangeReader {
+    DeviceRanges(cudaStream_t sm, std::vector<const uint8_t *> bytes) : bytes(std::move(bytes)), rb(sm) {}
+    void read(int file, uint64_t off, uint64_t n, uint8_t *dst) override {
+        if (st == PG_OK) st = rb.add(dst, bytes[file] + off, (size_t)n);
+    }
+    void flush() override {
+        if (st == PG_OK) st = rb.finish();
+        if (st != PG_OK) throw std::runtime_error("orc: a read-back of the file tails failed");
+    }
+    std::vector<const uint8_t *> bytes;
+    SmallReads rb;
+    pg_status st = PG_OK;                              // a CUDA error (its message is set)
+};
+
 static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, const pg_file_desc *files, int nf, int n_runs,
                                     const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
                                     pg_section_info *info) {
@@ -126,17 +184,37 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
     PG_CUDA(cudaEventRecord(tm.e0, sm));
     { pg_status st = b.read_columns(read_cols, names); if (st) return st; }
 
-    // ---- file tails, column resolution, plans
+    // ---- file bytes on the device, file tails on the host, column resolution, plans
     std::vector<orc::FileTail> tails(nf);
     std::vector<orc::Plan> plans(nf);
     std::vector<const uint8_t *> d_file(nf, nullptr);
-    int64_t file_bytes = 0, page_bytes = 0;
+    int64_t file_bytes = 0, h2d = 0, page_bytes = 0;
     bool any_compressed = false, any_zstd = false;
+    // (a codec or type this decoder does not cover is a refusal, not a malformed file)
+    auto parse_error = [](const std::exception &e) {
+        const bool refusal = strstr(e.what(), "is not decoded") != nullptr || strstr(e.what(), "not supported") != nullptr;
+        return fail(refusal ? PG_ERR_UNSUPPORTED : PG_ERR_FORMAT, e.what());
+    };
+    {
+        std::vector<int> dev;                          // the device-resident files: their tails in one batch of reads
+        std::vector<uint64_t> sizes;
+        std::vector<const uint8_t *> bytes;
+        for (int f = 0; f < nf; f++)
+            if (files[f].mem == PG_MEM_DEVICE) { dev.push_back(f); sizes.push_back((uint64_t)files[f].size); bytes.push_back(files[f].bytes); }
+        if (!dev.empty()) {
+            DeviceRanges rd(sm, std::move(bytes));
+            try {
+                std::vector<orc::FileTail> t = orc::read_tails(rd, sizes);
+                for (size_t i = 0; i < dev.size(); i++) tails[dev[i]] = std::move(t[i]);
+            } catch (const std::exception &e) {
+                if (rd.st) return rd.st;
+                return parse_error(e);
+            }
+        }
+    }
     for (int f = 0; f < nf; f++) {
-        if (files[f].mem != PG_MEM_HOST)
-            return fail(PG_ERR_UNSUPPORTED, "orc: the file bytes must be host memory (the footers and chunk headers are walked on the host)");
         try {
-            tails[f] = orc::parse_file(files[f].bytes, files[f].size);
+            if (files[f].mem == PG_MEM_HOST) tails[f] = orc::parse_file(files[f].bytes, files[f].size);
             const orc::FileTail &t = tails[f];
             if (t.types.empty() || t.types[0].kind != orc::K_STRUCT) return fail(PG_ERR_UNSUPPORTED, "orc: the root type is not a struct");
             if (t.compression != orc::C_NONE && t.compression != orc::C_ZLIB && t.compression != orc::C_ZSTD &&
@@ -158,14 +236,16 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
                     return fail(PG_ERR_UNSUPPORTED, "orc: column " + std::to_string(c) + " has an ORC type the device decoder does "
                                                     "not map to the table type (timestamps, DECIMAL(p > 18), nested types: Java side)");
             }
-            plans[f] = orc::plan_file(t, files[f].bytes, files[f].size, file_col);
+            plans[f] = orc::plan_file(t, files[f].size, file_col);
         } catch (const std::exception &e) {
-            // (a codec or type this decoder does not cover is a refusal, not a malformed file)
-            const bool refusal = strstr(e.what(), "is not decoded") != nullptr || strstr(e.what(), "not supported") != nullptr;
-            return fail(refusal ? PG_ERR_UNSUPPORTED : PG_ERR_FORMAT, e.what());
+            return parse_error(e);
         }
         file_bytes += files[f].size;
-        { pg_status st = file_image(scratch, files[f].bytes, files[f].size, "orc", &d_file[f]); if (st) return st; }
+        if (files[f].mem == PG_MEM_DEVICE) d_file[f] = files[f].bytes;
+        else {
+            { pg_status st = file_image(scratch, files[f].bytes, files[f].size, "orc", &d_file[f]); if (st) return st; }
+            h2d += files[f].size;
+        }
     }
     { pg_status st = b.check_runs(); if (st) return st; }
 
@@ -184,23 +264,19 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
     std::vector<orcdev::Task> h_tasks;
     std::vector<OrcTaskRef> h_refs;
     std::vector<int32_t> h_task_out;
-    uint64_t sc_bytes = 0, dict_entries = 0;
-    for (int f = 0; f < nf; f++) { sc_bytes += plans[f].scratch_bytes; dict_entries += plans[f].dict_entries; }
-    uint8_t *d_sc = !any_compressed ? nullptr : (uint8_t *)scratch.take((size_t)sc_bytes + 256);
-    if (any_compressed && !d_sc) return oom("orc", "the stream scratch", (size_t)sc_bytes);
+    uint64_t dict_entries = 0;
+    for (int f = 0; f < nf; f++) dict_entries += plans[f].dict_entries;
     int32_t *d_dict_off = (int32_t *)scratch.take(4 * (size_t)(dict_entries + 1) + 256);
     if (!d_dict_off) return oom("orc", "the dictionary offsets", 4 * (size_t)(dict_entries + 1));
-    uint64_t sc_base = 0, dict_base = 0;
+    uint64_t dict_base = 0;
     for (int f = 0; f < nf; f++) {
         const int s0 = (int)h_streams.size();
         for (const orc::PlanStream &ps : plans[f].streams) {
             OrcStream st{};
             st.src = d_file[f] + ps.offset;
             st.length = (int64_t)ps.length;
-            st.bound = (int64_t)ps.out_bound;
             st.codec = tails[f].compression;
             st.block_size = (int32_t)tails[f].block_size;
-            st.dst = d_sc ? d_sc + sc_base + ps.out_off : nullptr;
             h_streams.push_back(st);
             page_bytes += (int64_t)ps.length;
         }
@@ -222,7 +298,6 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
             h_refs.push_back(OrcTaskRef{idx(p.s_present), idx(p.s_data), idx(p.s_length), idx(p.s_dict), idx(p.s_secondary)});
             h_task_out.push_back(r * nc + p.col);
         }
-        sc_base += plans[f].scratch_bytes;
         dict_base += plans[f].dict_entries;
     }
     const int n_streams = (int)h_streams.size(), n_tasks = (int)h_tasks.size();
@@ -245,16 +320,39 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
     uint8_t *d_lit = tb + tb_s + tb_t + tb_r + tb_o + tb_p;
     int32_t *d_err = (int32_t *)(d_lit + tb_lit);
     int32_t *d_counter = d_err + 4;
+    int64_t *d_sc_total = (int64_t *)(d_err + 8);
     PG_CUDA(cudaMemsetAsync(d_err, 0, 64, sm));
     int launches = 0;
-    if (n_streams) PG_CUDA(cudaMemcpyAsync(d_streams, h_streams.data(), sizeof(OrcStream) * n_streams, cudaMemcpyHostToDevice, sm));
+    // (tables go through small_h2d: a kernel reads them out of mapped host memory, so they do not queue behind an
+    // asynchronous upload of the next section on the copy engine)
+    if (n_streams) { pg_status ts = small_h2d(d_streams, h_streams.data(), sizeof(OrcStream) * n_streams, sm); if (ts) return ts; }
     if (n_tasks) {
-        PG_CUDA(cudaMemcpyAsync(d_tasks, h_tasks.data(), sizeof(orcdev::Task) * n_tasks, cudaMemcpyHostToDevice, sm));
-        PG_CUDA(cudaMemcpyAsync(d_refs, h_refs.data(), sizeof(OrcTaskRef) * n_tasks, cudaMemcpyHostToDevice, sm));
-        PG_CUDA(cudaMemcpyAsync(d_task_out, h_task_out.data(), 4 * (size_t)n_tasks, cudaMemcpyHostToDevice, sm));
+        pg_status ts = small_h2d(d_tasks, h_tasks.data(), sizeof(orcdev::Task) * n_tasks, sm);
+        if (!ts) ts = small_h2d(d_refs, h_refs.data(), sizeof(OrcTaskRef) * n_tasks, sm);
+        if (!ts) ts = small_h2d(d_task_out, h_task_out.data(), 4 * (size_t)n_tasks, sm);
+        if (ts) return ts;
+    }
+    // ---- compressed sections: the chunk walk sizes the stream scratch (one read-back)
+    uint8_t *d_sc = nullptr;
+    if (any_compressed && n_streams) {
+        k_orc_walk<<<(n_streams + 127) / 128, 128, 0, sm>>>(d_streams, n_streams, d_err);
+        k_orc_scan<<<1, kOrcScanThreads, 0, sm>>>(d_streams, n_streams, d_sc_total);
+        launches += 2;
+        int32_t herr = 0;
+        int64_t sc_bytes = 0;
+        {
+            SmallReads rb(sm);
+            pg_status rs = rb.add(&herr, d_err, 4);
+            if (!rs) rs = rb.add(&sc_bytes, d_sc_total, 8);
+            if (!rs) rs = rb.finish();
+            if (rs) return rs;
+        }
+        if (herr != KERR_NONE) return fail(PG_ERR_FORMAT, "orc: truncated compression chunk");
+        d_sc = (uint8_t *)scratch.take((size_t)sc_bytes + 256);
+        if (!d_sc) return oom("orc", "the stream scratch", (size_t)sc_bytes);
     }
     if (n_streams) {
-        k_orc_inflate<<<inflate_ctas, kOrcWarps * 32, 0, sm>>>(d_streams, n_streams, d_lit, d_counter, d_err);
+        k_orc_inflate<<<inflate_ctas, kOrcWarps * 32, 0, sm>>>(d_streams, n_streams, d_sc, d_lit, d_counter, d_err);
         launches++;
     }
     if (n_tasks) {
@@ -268,16 +366,16 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
         const int64_t max_n = *std::max_element(b.run_rows.begin(), b.run_rows.end());
         int64_t *d_sums = (int64_t *)scratch.take(8 * (size_t)(max_n / 4096 + 4));
         if (!d_sums) return oom("orc", "the offsets scan", 8 * (size_t)(max_n / 4096 + 4));
+        SmallReads rb(sm);                                 // the read-back: exact payload sizes
         for (size_t i = 0; i < b.out.size(); i++) {
             const OutColumn &o = b.out[i];
             if (!o.offsets) continue;
             const int64_t n = b.run_rows[i / nc];
             launch_offsets_scan(o.offsets, n, d_sums, d_err, sm);
             launches += n > 0 ? 3 : 0;
-            PG_CUDA(cudaMemcpyAsync(&totals[i], o.offsets + n, 4, cudaMemcpyDeviceToHost, sm));
+            { pg_status rs = rb.add(&totals[i], o.offsets + n, 4); if (rs) return rs; }
         }
-        PG_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, sm));
-        PG_CUDA(cudaStreamSynchronize(sm));               // the read-back: exact payload sizes
+        { pg_status rs = rb.add(&herr, d_err, 4); if (!rs) rs = rb.finish(); if (rs) return rs; }
         if (herr != KERR_NONE)
             return fail(herr == KERR_OFFSET_OVERFLOW ? PG_ERR_INTERNAL : PG_ERR_FORMAT,
                         herr == KERR_OFFSET_OVERFLOW ? "orc: a var-len column exceeds 2 GiB of payload"
@@ -285,20 +383,23 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
         { pg_status st = b.alloc_payload(std::vector<int64_t>(totals.begin(), totals.end())); if (st) return st; }
         std::vector<uint8_t *> h_payload(b.out.size());   // (k_orc_set_payload reads the var-len entries only)
         for (size_t i = 0; i < b.out.size(); i++) h_payload[i] = (uint8_t *)b.out[i].data;
-        PG_CUDA(cudaMemcpyAsync(d_payload, h_payload.data(), sizeof(void *) * h_payload.size(), cudaMemcpyHostToDevice, sm));
+        { pg_status ts = small_h2d(d_payload, h_payload.data(), sizeof(void *) * h_payload.size(), sm); if (ts) return ts; }
         if (n_tasks) {
             k_orc_set_payload<<<(n_tasks + 127) / 128, 128, 0, sm>>>(d_tasks, n_tasks, d_task_out, d_payload);
             k_orc_task<1><<<(n_tasks + 31) / 32, 32, 0, sm>>>(d_tasks, d_refs, d_streams, n_tasks, d_err);
             launches += 2;
         }
-        PG_CUDA(cudaStreamSynchronize(sm));               // (h_payload is a local)
     }
     PG_CUDA(cudaEventRecord(tm.e1, sm));
-    PG_CUDA(cudaMemcpyAsync(&herr, d_err, 4, cudaMemcpyDeviceToHost, sm));
-    PG_CUDA(cudaStreamSynchronize(sm));
+    {
+        SmallReads rb(sm);
+        pg_status rs = rb.add(&herr, d_err, 4);
+        if (!rs) rs = rb.finish();
+        if (rs) return rs;
+    }
     PG_CUDA(cudaGetLastError());
     if (herr != KERR_NONE) return fail(PG_ERR_FORMAT, "orc: a stream does not decode (malformed file or unsupported encoding)");
-    b.finish(out_runs, file_bytes, info);
+    b.finish(out_runs, h2d, info);
     if (info) {
         info->file_bytes = file_bytes;
         info->page_bytes = page_bytes;

@@ -145,16 +145,19 @@ StripeFooter read_stripe_footer(Pb pb) {
     return sf;
 }
 
+void check_magic(const uint8_t *head, uint64_t size) {
+    if (size < 4 || head[0] != 'O' || head[1] != 'R' || head[2] != 'C') throw std::runtime_error("orc: missing ORC magic");
+}
+
 }  // namespace
 
-FileTail parse_file(const uint8_t *file, int64_t size) {
-    if (size < 4 || file[0] != 'O' || file[1] != 'R' || file[2] != 'C') throw std::runtime_error("orc: missing ORC magic");
-    const uint64_t ps_len = file[size - 1];
-    if ((int64_t)ps_len + 1 > size) throw std::runtime_error("orc: bad postscript length");
-    FileTail t;
+uint64_t parse_tail(const uint8_t *tail, uint64_t n, uint64_t size, FileTail &t) {
+    const uint64_t ps_len = tail[n - 1];
+    if (ps_len + 1 > size) throw std::runtime_error("orc: bad postscript length");
+    t = FileTail();
     uint64_t footer_len = 0;
     {
-        Pb pb(file + size - 1 - ps_len, (size_t)ps_len);
+        Pb pb(tail + n - 1 - ps_len, (size_t)ps_len);
         uint32_t f;
         int w;
         while (pb.next(f, w)) {
@@ -165,8 +168,10 @@ FileTail parse_file(const uint8_t *file, int64_t size) {
             else pb.skip(w);
         }
     }
-    if (footer_len + ps_len + 1 > (uint64_t)size) throw std::runtime_error("orc: bad footer length");
-    const std::vector<uint8_t> footer = inflate_section(file + size - 1 - ps_len - footer_len, footer_len, t.compression, t.block_size);
+    if (footer_len > size - ps_len - 1) throw std::runtime_error("orc: bad footer length");
+    const uint64_t need = footer_len + ps_len + 1;
+    if (need > n) return need;
+    const std::vector<uint8_t> footer = inflate_section(tail + n - need, footer_len, t.compression, t.block_size);
     {
         Pb pb(footer.data(), footer.size());
         uint32_t f;
@@ -178,23 +183,97 @@ FileTail parse_file(const uint8_t *file, int64_t size) {
             else pb.skip(w);
         }
     }
-    for (const StripeInfo &si : t.stripes) {
-        const uint64_t fo = si.offset + si.index_length + si.data_length;
-        if (fo + si.footer_length > (uint64_t)size) throw std::runtime_error("orc: stripe footer outside the file");
-        const std::vector<uint8_t> raw = inflate_section(file + fo, si.footer_length, t.compression, t.block_size);
-        StripeFooter sf = read_stripe_footer(Pb(raw.data(), raw.size()));
-        uint64_t off = si.offset;
-        for (StreamInfo &s : sf.streams) {
-            s.offset = off;
-            off += s.length;
-        }
-        if (off > fo) throw std::runtime_error("orc: stream lengths exceed the stripe");
-        t.stripe_footers.push_back(std::move(sf));
+    t.stripe_footers.resize(t.stripes.size());
+    return 0;
+}
+
+uint64_t stripe_footer_offset(const FileTail &t, size_t i, uint64_t size) {
+    const StripeInfo &si = t.stripes[i];
+    uint64_t end = si.offset;                            // (each step is checked: corrupt lengths must not wrap)
+    for (const uint64_t len : {si.index_length, si.data_length, si.footer_length}) {
+        if (end > size || len > size - end) throw std::runtime_error("orc: stripe footer outside the file");
+        end += len;
     }
+    return end - si.footer_length;
+}
+
+void parse_stripe_footer(FileTail &t, size_t i, const uint8_t *stored) {
+    const StripeInfo &si = t.stripes[i];
+    const std::vector<uint8_t> raw = inflate_section(stored, si.footer_length, t.compression, t.block_size);
+    StripeFooter sf = read_stripe_footer(Pb(raw.data(), raw.size()));
+    const uint64_t fo = si.offset + si.index_length + si.data_length;      // (stripe_footer_offset checked the sum)
+    uint64_t off = si.offset;
+    for (StreamInfo &s : sf.streams) {
+        if (s.length > fo - off) throw std::runtime_error("orc: stream lengths exceed the stripe");
+        s.offset = off;
+        off += s.length;
+    }
+    t.stripe_footers[i] = std::move(sf);
+}
+
+FileTail parse_file(const uint8_t *file, int64_t size) {
+    check_magic(file, (uint64_t)size);
+    FileTail t;
+    parse_tail(file, (uint64_t)size, (uint64_t)size, t);
+    for (size_t i = 0; i < t.stripes.size(); i++) parse_stripe_footer(t, i, file + stripe_footer_offset(t, i, (uint64_t)size));
     return t;
 }
 
-Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::vector<int> &file_col_of) {
+std::vector<FileTail> read_tails(RangeReader &rd, const std::vector<uint64_t> &sizes) {
+    const size_t nf = sizes.size();
+    std::vector<FileTail> t(nf);
+    std::vector<std::vector<uint8_t>> tail(nf);
+    std::vector<uint8_t> head(4 * nf);
+    // round 1: the magic and the last min(size, 16 KiB) bytes of every file
+    for (size_t f = 0; f < nf; f++) {
+        if (sizes[f] < 4) throw std::runtime_error("orc: missing ORC magic");
+        tail[f].resize((size_t)std::min(sizes[f], kTailRead));
+        rd.read((int)f, 0, 3, &head[4 * f]);
+        rd.read((int)f, sizes[f] - tail[f].size(), tail[f].size(), tail[f].data());
+    }
+    rd.flush();
+    // round 2: the rest of each Footer that begins in front of its file's tail
+    std::vector<uint64_t> need(nf, 0);
+    std::vector<std::vector<uint8_t>> full(nf);
+    bool more = false;
+    for (size_t f = 0; f < nf; f++) {
+        check_magic(&head[4 * f], sizes[f]);
+        need[f] = parse_tail(tail[f].data(), tail[f].size(), sizes[f], t[f]);
+        if (!need[f]) continue;
+        const uint64_t have = tail[f].size();
+        full[f].resize((size_t)need[f]);
+        memcpy(full[f].data() + (need[f] - have), tail[f].data(), (size_t)have);
+        rd.read((int)f, sizes[f] - need[f], need[f] - have, full[f].data());
+        more = true;
+    }
+    if (more) rd.flush();
+    for (size_t f = 0; f < nf; f++) {
+        if (need[f] && parse_tail(full[f].data(), need[f], sizes[f], t[f]) != 0)
+            throw std::runtime_error("orc: the footer does not fit the length its postscript gives");
+        full[f] = std::vector<uint8_t>();
+    }
+    // round 3: every stripe footer of every file
+    std::vector<std::vector<std::vector<uint8_t>>> stored(nf);
+    bool any = false;
+    for (size_t f = 0; f < nf; f++) {
+        stored[f].resize(t[f].stripes.size());
+        uint64_t total = 0;                              // (the stripe footers of a file are disjoint parts of it: this
+        for (size_t i = 0; i < t[f].stripes.size(); i++) {   // bounds the host memory a corrupt Footer can claim)
+            const uint64_t off = stripe_footer_offset(t[f], i, sizes[f]);
+            total += t[f].stripes[i].footer_length;
+            if (total > sizes[f]) throw std::runtime_error("orc: the stripe footers are larger than the file");
+            stored[f][i].resize((size_t)t[f].stripes[i].footer_length);
+            rd.read((int)f, off, stored[f][i].size(), stored[f][i].data());
+            any = true;
+        }
+    }
+    if (any) rd.flush();
+    for (size_t f = 0; f < nf; f++)
+        for (size_t i = 0; i < t[f].stripes.size(); i++) parse_stripe_footer(t[f], i, stored[f][i].data());
+    return t;
+}
+
+Plan plan_file(const FileTail &t, int64_t size, const std::vector<int> &file_col_of) {
     Plan pl;
     if (t.types.empty() || t.types[0].kind != K_STRUCT) throw std::runtime_error("orc: the root type is not a struct");
     int64_t row0 = 0;
@@ -228,15 +307,6 @@ Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::
                 PlanStream ps;
                 ps.offset = s.offset;
                 ps.length = s.length;
-                if (t.compression == C_NONE) ps.out_bound = s.length;
-                else {
-                    const int64_t bound = orcdev::chunk_bound(file + s.offset, (int64_t)s.length, t.compression,
-                                                              (int64_t)t.block_size);
-                    if (bound < 0) throw std::runtime_error("orc: truncated compression chunk");
-                    ps.out_bound = (uint64_t)bound;
-                }
-                ps.out_off = pl.scratch_bytes;
-                pl.scratch_bytes += (ps.out_bound + 64 + 63) & ~(uint64_t)63;
                 *slot = (int)pl.streams.size();
                 pl.streams.push_back(ps);
             }
@@ -252,6 +322,21 @@ Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::
             pl.tasks.push_back(task);
         }
         row0 += (int64_t)t.stripes[si].rows;
+    }
+    return pl;
+}
+
+Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::vector<int> &file_col_of) {
+    Plan pl = plan_file(t, size, file_col_of);
+    for (PlanStream &ps : pl.streams) {
+        if (t.compression == C_NONE) ps.out_bound = ps.length;
+        else {
+            const int64_t bound = orcdev::chunk_bound(file + ps.offset, (int64_t)ps.length, t.compression, (int64_t)t.block_size);
+            if (bound < 0) throw std::runtime_error("orc: truncated compression chunk");
+            ps.out_bound = (uint64_t)bound;
+        }
+        ps.out_off = pl.scratch_bytes;
+        pl.scratch_bytes += (ps.out_bound + 64 + 63) & ~(uint64_t)63;
     }
     return pl;
 }

@@ -53,14 +53,41 @@ struct FileTail {
     std::vector<StripeFooter> stripe_footers;
 };
 
-// Throws std::runtime_error on malformed / unsupported input (only NONE, ZLIB and ZSTD metadata is inflated).
+// ---- the file tail.  Every parse below throws std::runtime_error on malformed / unsupported input (NONE, ZLIB, LZ4 and
+// ZSTD metadata is inflated).  A file in host memory is parsed whole by parse_file; the files of a section in device
+// memory come to the host a few byte ranges at a time through read_tails.  Both go through the same steps:
+// parse_tail, then stripe_footer_offset + parse_stripe_footer per stripe.
+
+// The PostScript and Footer of a file of `size` bytes from its last n bytes (tail = the file's bytes [size - n, size),
+// n >= min(size, 256) so that the PostScript is inside): 0 when both are parsed into t (which is reset first), else the
+// number of last bytes the Footer needs (> n).  The PostScript and Footer lengths are checked against the file.
+uint64_t parse_tail(const uint8_t *tail, uint64_t n, uint64_t size, FileTail &t);
+// where stripe i's footer starts; offset + index + data + footer length are checked against the file
+uint64_t stripe_footer_offset(const FileTail &t, size_t i, uint64_t size);
+// stripe i's footer from its stored bytes (t.stripes[i].footer_length of them): stored as t.stripe_footers[i], with
+// the absolute offsets of its streams
+void parse_stripe_footer(FileTail &t, size_t i, const uint8_t *stored);
+
 FileTail parse_file(const uint8_t *file, int64_t size);
+
+// Byte ranges of the files of a section: read() queues the copy of [off, off + n) of file `file` into dst, flush()
+// delivers every queued range (one round trip).
+struct RangeReader {
+    virtual ~RangeReader() = default;
+    virtual void read(int file, uint64_t off, uint64_t n, uint8_t *dst) = 0;
+    virtual void flush() = 0;
+};
+constexpr uint64_t kTailRead = 16384;
+// The tails of files of sizes[f] bytes read through rd in at most three rounds, however many files there are: the
+// last min(size, 16 KiB) bytes and the magic of every file; the rest of the Footers that did not fit; the stripe
+// footers of every file.  No range is queued before it is checked against its file.
+std::vector<FileTail> read_tails(RangeReader &rd, const std::vector<uint64_t> &sizes);
 
 // ---- decode plan of one file: which streams to inflate, and one task per (stripe, wanted column)
 struct PlanStream {
     uint64_t offset = 0, length = 0;     // in the file
-    uint64_t out_bound = 0;              // upper bound of the inflated bytes
-    uint64_t out_off = 0;                // position in the file's stream scratch (64-byte aligned)
+    uint64_t out_bound = 0;              // host layout only: upper bound of the inflated bytes
+    uint64_t out_off = 0;                // host layout only: position in the file's stream scratch (64-byte aligned)
 };
 struct PlanTask {
     int stripe = 0;
@@ -75,10 +102,16 @@ struct PlanTask {
 struct Plan {
     std::vector<PlanStream> streams;
     std::vector<PlanTask> tasks;
-    uint64_t scratch_bytes = 0;          // inflated streams
+    uint64_t scratch_bytes = 0;          // host layout only: inflated streams
     uint64_t dict_entries = 0;           // dictionary-offset scratch entries
 };
-// file_col_of[c] = the file's column (0-based child of the root struct) for caller column c, or < 0 = skip
+// file_col_of[c] = the file's column (0-based child of the root struct) for caller column c, or < 0 = skip.  The
+// streams are checked against the file's size; their compression chunks are not read (the device decoder walks them
+// with k_orc_walk and lays out its scratch with k_orc_scan).
+Plan plan_file(const FileTail &t, int64_t size, const std::vector<int> &file_col_of);
+// The same plan with the stream scratch laid out on the host, from the file's bytes in host memory: each stream's
+// out_bound from its chunk headers (orcdev::chunk_bound, the function k_orc_walk calls), out_off, scratch_bytes.  For
+// host builds of the decode path.
 Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::vector<int> &file_col_of);
 
 // ---- writer side: the stripe footers and the file tail (Metadata, Footer, PostScript, PostScript length) of a flat

@@ -112,7 +112,8 @@ class ParquetFileRecordReader(FileRecordReader):
 
 def read_section(schema: KeyValueSchema, files, n_runs: int, device: int = 0, check_names: bool = True,
                  read_value_fields=None, file_format: str = "parquet"):
-    """Decode every data file of a section with ONE batch of device launches (pg_parquet_read_section) and return
+    """Decode every data file of a section with ONE batch of device launches (pg_parquet_read_section, or
+    pg_orc_read_section for file_format="orc") and return
     (one SortedRunReader per run, PgSectionInfo).  `files` = [(buffer, run index)], in key order inside a run; a
     buffer is bytes / a numpy uint8 array (host memory) or a (device pointer, size) tuple (bytes already in HBM).
     The files of a run are concatenated on the device, as MergeTreeReaders.readerForRun's ConcatRecordReader does

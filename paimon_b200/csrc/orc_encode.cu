@@ -9,16 +9,19 @@
 //
 // Pipeline (the launch count does not depend on the number of columns; a task = one column of one stripe):
 //   1. k_oe_count + k_pw_stats per task: non-null values, payload bytes, exact sums, true count, VARCHAR lengths; min /
-//      max / NaN / retracts.  One read-back.
+//      max / NaN / retracts.  One read-back.  The ORC statistics come from both (task_stats, merge_stats); the file
+//      statistics of pg_parquet_file_column_stats and pg_file_meta from the k_pw_stats words (FileStats).
 //   2. k_oe_values (phase 0): the non-null values that are run-length coded are compacted into scratch (int64 values,
 //      string lengths, decimal scales; BYTE values, BOOLEAN bits; PRESENT bytes).
 //   3. k_oe_rle_size: one thread per integer RLE v2 run (kRunValues values) or byte-RLE group (kByteGroup bytes).  One
 //      read-back; the host lays out the streams.
 //   4. k_oe_rle_write and k_oe_values (phase 1): the runs, and the streams that are the values themselves (FLOAT /
 //      DOUBLE, string bytes, DECIMAL varints) straight from the batch, at their positions in the image.
-//   5. ZSTD: every stream cut into chunks of at most the block size, every chunk one frame of k_zs_block blocks; one
-//      read-back of the frame sizes; k_oe_zs_gather places each chunk, compressed or original, behind its header.
-// The stripe footers and the file tail are written on the host (orc_meta.cc) and patched in like Parquet's footer.
+//   5. ZSTD: every stream cut into chunks of at most the block size, every chunk one zstd frame (ZstdFrames); one
+//      read-back of the frame sizes; the host keeps the original bytes of a chunk whose frame is not smaller, lays
+//      out the stripes, and the gather places each chunk, compressed or original, behind its 3-byte header.
+// The chunk headers, the stripe footers and the file tail are written on the host (orc_meta.cc) as host parts, like
+// Parquet's page headers and footer.
 #include <math.h>
 
 #include <algorithm>
@@ -29,7 +32,6 @@
 #include "encoded_file.h"
 #include "orc_encode_device.cuh"
 #include "orc_meta.h"
-#include "zstd_encode_device.cuh"
 
 namespace pg {
 
@@ -205,38 +207,6 @@ __global__ void k_oe_rle_write(const RleJob *jobs, int n, const int64_t *ints, c
     }
 }
 
-// One CTA per zstd block: places its compression chunk at chunk_off (3-byte header, then the frame, or the original
-// bytes when the frame is not smaller: stored == raw)
-__global__ void k_oe_zs_gather(const ZsBlockJob *jobs, const ZsPage *chunks, const int2 *res, const int32_t *boff,
-                               const int64_t *chunk_off, const int64_t *stored, const uint8_t *img, const uint8_t *zout,
-                               uint8_t *file) {
-    const ZsBlockJob j = jobs[blockIdx.x];
-    const ZsPage ch = chunks[j.page];
-    const int64_t len = stored[j.page];
-    const bool original = len == ch.raw;
-    uint8_t *hdr = file + chunk_off[j.page];
-    const bool first = (int)blockIdx.x == ch.first_block;
-    if (threadIdx.x == 0 && first) {
-        const uint32_t h = (uint32_t)len << 1 | (original ? 1u : 0u);
-        hdr[0] = (uint8_t)h; hdr[1] = (uint8_t)(h >> 8); hdr[2] = (uint8_t)(h >> 16);
-    }
-    if (original) {
-        uint8_t *dst = hdr + 3 + (j.src - jobs[ch.first_block].src);
-        for (int i = threadIdx.x; i < j.n; i += blockDim.x) dst[i] = img[j.src + i];
-        return;
-    }
-    const int2 r = res[blockIdx.x];
-    uint8_t *frame = hdr + 3;
-    uint8_t *dst = frame + boff[blockIdx.x];
-    if (threadIdx.x == 0) {
-        if (first) zs::write_frame_header(frame, (uint64_t)ch.raw);
-        zs::write_block_header(dst, (int)blockIdx.x == ch.first_block + ch.n_blocks - 1, r.x,
-                               r.x == 2 ? (uint32_t)r.y : (uint32_t)j.n);
-    }
-    const uint8_t *pay = r.x == 0 ? img + j.src : zout + j.out;
-    for (int i = threadIdx.x; i < r.y; i += blockDim.x) dst[3 + i] = pay[i];
-}
-
 // ------------------------------------------------------------------ host side
 
 int default_kind(int t) {
@@ -369,27 +339,17 @@ pg_status encode_orc(uint64_t source, const char *const *names, int64_t row0, in
     if (opt && (opt->compression_block_size < 0 || opt->compression_block_size >= ((int64_t)1 << 23)))
         return fail(PG_ERR_INVALID, "orc encode: compression block size " + std::to_string(opt->compression_block_size) +
                                         " outside [0, 2^23) (a chunk header holds 23 bits of length)");
-    pg_status st = ensure_device();
-    if (st) return st;
     BatchColumns batch;                                      // held until the encode below is done
-    if ((st = batch_columns(source, &batch))) return st;
+    pg_status st = encode_source(source, "orc encode", row0, &n_rows, &batch);
+    if (st) return st;
     const Schema *s = batch.schema.get();
     const std::vector<DevColumn> &dcols = batch.cols;
-    for (int c = 0; c < s->n_cols() && batch.n_rows > 0; c++)
-        if (!dcols[c].data && !dcols[c].offsets)
-            return fail(PG_ERR_INVALID, "orc encode: the batch was produced under a read-type projection and has no "
-                                        "column " + std::to_string(c) + "; a data file needs every column");
-    if (n_rows < 0) n_rows = batch.n_rows - row0;
-    if (row0 < 0 || (row0 & 7) || row0 + n_rows > batch.n_rows)
-        return fail(PG_ERR_INVALID, "orc encode: row range outside the batch or not starting at a multiple of 8");
     const int nc = s->n_cols();
     std::vector<OutType> types;
     if ((st = resolve_types(*s, opt ? opt->types : nullptr, types))) return st;
 
     SectionTimer tm;
-    PG_CUDA(cudaEventCreate(&tm.e0));
-    PG_CUDA(cudaEventCreate(&tm.e1));
-    PG_CUDA(cudaEventRecord(tm.e0, 0));
+    if ((st = start_encode(tm))) return st;
 
     // ---- tasks: stripe major, then column
     int64_t stripe_rows = opt && opt->stripe_rows > 0 ? opt->stripe_rows : (int64_t)1 << 20;
@@ -440,9 +400,7 @@ pg_status encode_orc(uint64_t source, const char *const *names, int64_t row0, in
     std::vector<orc::ColumnStats> file_stats(nc + 1);
     file_stats[0].values = (uint64_t)n_rows;
     std::vector<orc::OutStripe> stripes(n_stripes);
-    std::vector<char> file_nan(nc, 0);
-    std::vector<ColStats> &cs = ef->stats;
-    cs.assign(nc, ColStats{INT64_MAX, INT64_MIN, 0, 0});
+    FileStats fs(*s);                                         // the accessor's statistics: those of the Parquet output
     std::vector<Stream> streams;
     std::vector<RleJob> jobs;
     int64_t n_ints = 0, n_bytes = 0;
@@ -467,21 +425,7 @@ pg_status encode_orc(uint64_t source, const char *const *names, int64_t row0, in
         }
         sp.stats[t.col + 1] = task_stats(t, cnt, sw);
         merge_stats(t.kind, file_stats[t.col + 1], sp.stats[t.col + 1], g == 0);
-        // the accessor's statistics: those of the Parquet output
-        ColStats &f = cs[t.col];
-        f.null_count += t.rows - nn;
-        const bool fp = t.kind == orc::K_FLOAT || t.kind == orc::K_DOUBLE;
-        file_nan[t.col] |= sw[4] != 0;
-        if (cols[t.col].width > 0 && nn > 0 && !sw[4]) {
-            int64_t mn = sw[0], mx = sw[1];
-            if (fp) { mn = zero_as(mn, -0.0); mx = zero_as(mx, 0.0); }
-            if (!f.has_minmax) { f.min = mn; f.max = mx; f.has_minmax = 1; }
-            else if (fp) {
-                const double a = std::min(as_double(f.min), as_double(mn)), b = std::max(as_double(f.max), as_double(mx));
-                memcpy(&f.min, &a, 8); memcpy(&f.max, &b, 8);
-            } else { f.min = std::min(f.min, mn); f.max = std::max(f.max, mx); }
-        }
-        if (t.col == s->n_key + 1) ef->meta.delete_row_count += sw[3];
+        fs.add(t.col, cols[t.col], sw, t.rows);
 
         if (nn < t.rows) {
             Stream sm{(int)i, orc::S_PRESENT};
@@ -513,11 +457,7 @@ pg_status encode_orc(uint64_t source, const char *const *names, int64_t row0, in
             streams.push_back(second);
         }
     }
-    for (int c = 0; c < nc; c++)
-        if (file_nan[c]) cs[c] = ColStats{INT64_MAX, INT64_MIN, cs[c].null_count, 0};
-    const ColStats &sq = cs[s->n_key];
-    ef->meta.min_sequence_number = sq.has_minmax ? sq.min : 0;
-    ef->meta.max_sequence_number = sq.has_minmax ? sq.max : 0;
+    fs.finish(*ef);
 
     // ---- compaction and run sizes
     const size_t nj = jobs.size();
@@ -607,8 +547,7 @@ pg_status encode_orc(uint64_t source, const char *const *names, int64_t row0, in
     uint8_t *d_raw = nullptr;
     if (zstd) d_raw = (uint8_t *)scratch.take((size_t)raw_bytes + 64);
     else {
-        PG_CUDA(cudaMalloc(&ef->d_file, (size_t)ef->file_bytes + 64));
-        PG_CUDA(cudaMemsetAsync(ef->d_file, 0, (size_t)ef->file_bytes + 64, 0));
+        if ((st = ef->alloc_image())) return st;
         d_raw = ef->d_file;
     }
     if (!d_raw) return fail(PG_ERR_CUDA, "orc encode: out of device memory for the stream image");
@@ -623,85 +562,45 @@ pg_status encode_orc(uint64_t source, const char *const *names, int64_t row0, in
         launches++;
     }
 
-    // ---- ZSTD: chunks of at most `block` bytes, one frame each; sizes back; layout; the chunks placed
+    // ---- ZSTD: chunks of at most `block` bytes, one frame each; sizes back; layout; the chunk headers among the host
+    // parts, each chunk behind its header, compressed or original
     if (zstd) {
-        std::vector<ZsPage> chunks;
-        std::vector<ZsBlockJob> bjobs;
-        int64_t out = 0, seq = 0;
+        std::vector<ZstdFrames::Body> chunks;
         for (Stream &sm : streams) {
             sm.chunk0 = chunks.size();
-            for (int64_t c0 = 0; c0 < sm.length; c0 += block) {
-                const int64_t cn = std::min<int64_t>(block, sm.length - c0);
-                ZsPage ch{cn, (int32_t)bjobs.size(), 0};
-                for (int64_t b0 = 0; b0 < cn; b0 += zs::kMaxBlock) {
-                    const int32_t n = (int32_t)std::min<int64_t>(zs::kMaxBlock, cn - b0);
-                    bjobs.push_back(ZsBlockJob{sm.raw_off + c0 + b0, out, seq, n, (int32_t)chunks.size()});
-                    out += n;
-                    seq += n / 4 + 1;
-                    ch.n_blocks++;
-                }
-                chunks.push_back(ch);
-            }
+            for (int64_t c0 = 0; c0 < sm.length; c0 += block)
+                chunks.push_back({sm.raw_off + c0, std::min<int64_t>(block, sm.length - c0)});
             sm.chunk1 = chunks.size();
         }
-        const size_t nch = chunks.size(), nb = bjobs.size();
-        std::vector<int64_t> frame(nch), stored(nch), chunk_off(nch);
-        ZsBlockJob *d_bjobs = (ZsBlockJob *)scratch.take(sizeof(ZsBlockJob) * std::max<size_t>(nb, 1));
-        ZsPage *d_chunks = (ZsPage *)scratch.take(sizeof(ZsPage) * std::max<size_t>(nch, 1));
-        int2 *d_res = (int2 *)scratch.take(sizeof(int2) * std::max<size_t>(nb, 1));
-        int32_t *d_boff = (int32_t *)scratch.take(sizeof(int32_t) * std::max<size_t>(nb, 1));
-        int64_t *d_frame = (int64_t *)scratch.take(sizeof(int64_t) * std::max<size_t>(nch, 1));
-        int64_t *d_stored = (int64_t *)scratch.take(sizeof(int64_t) * std::max<size_t>(nch, 1));
-        uint8_t *d_zout = (uint8_t *)scratch.take((size_t)out + 64);
-        uint8_t *d_lits = (uint8_t *)scratch.take((size_t)raw_bytes + 64);
-        void *d_seqs = scratch.take(zs_seq_bytes(seq) + 64);
-        if (!d_bjobs || !d_chunks || !d_res || !d_boff || !d_frame || !d_stored || !d_zout || !d_lits || !d_seqs)
-            return fail(PG_ERR_CUDA, "orc encode: out of device memory for the zstd chunks");
-        if (nb) {
-            PG_CUDA(cudaMemcpy(d_bjobs, bjobs.data(), sizeof(ZsBlockJob) * nb, cudaMemcpyHostToDevice));
-            PG_CUDA(cudaMemcpy(d_chunks, chunks.data(), sizeof(ZsPage) * nch, cudaMemcpyHostToDevice));
-            launch_zs_compress(d_bjobs, (int)nb, d_chunks, (int)nch, d_raw, d_zout, d_seqs, d_lits, d_res, d_boff, d_frame);
-            launches += 2;
-            SmallReads rd(0);
-            if ((st = rd.add(frame.data(), d_frame, sizeof(int64_t) * nch))) return st;
-            launches++;
-            if ((st = rd.finish())) return st;
-        }
+        ZstdFrames frames("orc encode");
+        std::vector<int64_t> stored, chunk_off(chunks.size());  // the frame sizes, then the bytes of each chunk's body
+        if ((st = frames.compress(scratch, d_raw, chunks, &stored, &launches))) return st;
+        std::vector<uint8_t> original(chunks.size());           // the frame is not smaller: the bytes as they are
         for (Stream &sm : streams) {
             sm.stored = 0;
             for (size_t c = sm.chunk0; c < sm.chunk1; c++) {
-                stored[c] = frame[c] < chunks[c].raw ? frame[c] : chunks[c].raw;
+                original[c] = stored[c] >= chunks[c].bytes;
+                if (original[c]) stored[c] = chunks[c].bytes;
                 sm.stored += 3 + stored[c];
             }
         }
         if ((st = layout(stream_off))) return st;
         for (size_t i = 0; i < streams.size(); i++) {
             int64_t at = stream_off[i];
-            for (size_t c = streams[i].chunk0; c < streams[i].chunk1; c++) { chunk_off[c] = at; at += 3 + stored[c]; }
+            for (size_t c = streams[i].chunk0; c < streams[i].chunk1; c++) {
+                const uint32_t h = (uint32_t)stored[c] << 1 | original[c];
+                ef->host_parts.push_back({at, {(uint8_t)h, (uint8_t)(h >> 8), (uint8_t)(h >> 16)}});
+                chunk_off[c] = at + 3;
+                at += 3 + stored[c];
+            }
         }
-        PG_CUDA(cudaMalloc(&ef->d_file, (size_t)ef->file_bytes + 64));
-        PG_CUDA(cudaMemsetAsync(ef->d_file, 0, (size_t)ef->file_bytes + 64, 0));
-        if (nb) {
-            PG_CUDA(cudaMemcpy(d_frame, chunk_off.data(), sizeof(int64_t) * nch, cudaMemcpyHostToDevice));
-            PG_CUDA(cudaMemcpy(d_stored, stored.data(), sizeof(int64_t) * nch, cudaMemcpyHostToDevice));
-            k_oe_zs_gather<<<(unsigned)nb, 256>>>(d_bjobs, d_chunks, d_res, d_boff, d_frame, d_stored, d_raw, d_zout, ef->d_file);
-            launches++;
-        }
+        if ((st = ef->alloc_image())) return st;
+        if ((st = frames.gather(chunk_off, original, ef->d_file, &launches))) return st;
     }
-    PG_CUDA(cudaEventRecord(tm.e1, 0));
-    PG_CUDA(cudaEventSynchronize(tm.e1));
-    const float ms = tm.ms();
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(PG_ERR_CUDA, std::string("orc encode: ") + cudaGetErrorString(le));
-
     ef->meta.n_rows = n_rows;
-    ef->meta.file_bytes = ef->file_bytes;
     ef->meta.n_row_groups = (int32_t)n_stripes;
     ef->meta.n_pages = (int32_t)streams.size();
-    ef->meta.ms_encode = ms;
-    ef->meta.launches = launches;
-    *out_file = g_enc.put(std::move(ef));
-    return PG_OK;
+    return finish_encode(tm, std::move(ef), launches, "orc encode", out_file);
 }
 
 }  // namespace

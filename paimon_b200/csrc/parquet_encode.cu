@@ -23,7 +23,6 @@
 #include "device_utils.cuh"
 #include "encoded_file.h"
 #include "parquet_meta.h"
-#include "zstd_encode_device.cuh"
 
 namespace pg {
 
@@ -139,151 +138,6 @@ k_pw_encode(const EncColumn *cols, const EncJob *jobs, uint8_t *file) {
     }
 }
 
-// per column chunk (one CTA): min / max of the non-null values of a fixed-width numeric column, as int64 / double
-// bit patterns (FLOAT / DOUBLE: of the non-NaN values, whichever zero comes first; the host applies the zero rule),
-// whether a non-null value is NaN; also used for the sequence number range and the delete count (kind column)
-__global__ void k_pw_stats(const EncColumn *cols, const StatJob *jobs, int64_t *out /* [job][kStatWords] */) {
-    const StatJob j = jobs[blockIdx.x];
-    const EncColumn c = cols[j.col];
-    const bool fp = c.type == PG_FLOAT || c.type == PG_DOUBLE;
-    int64_t imin = INT64_MAX, imax = INT64_MIN;
-    double dmin = INFINITY, dmax = -INFINITY;
-    long long nn = 0, retr = 0;
-    bool nan_seen = false;
-    for (int64_t i = threadIdx.x; i < j.n_rows; i += blockDim.x) {
-        const int64_t row = j.row0 + i;
-        if (c.validity && !valid_bit(c.validity, row)) continue;
-        nn++;
-        if (c.width == 0) continue;
-        if (fp) {
-            double x = c.type == PG_FLOAT ? (double)((const float *)c.data)[row] : ((const double *)c.data)[row];
-            if (x != x) { nan_seen = true; continue; }
-            dmin = fmin(dmin, x); dmax = fmax(dmax, x);
-        } else {
-            int64_t x = sext(load_fixed(c.data, c.width, row), c.width);
-            if (c.type == PG_BOOL) x = x != 0;
-            imin = min(imin, x); imax = max(imax, x);
-            if (c.type == PG_INT8 && (x == 1 || x == 3)) retr++;        // RowKind retracts, used for _VALUE_KIND
-        }
-    }
-    __shared__ long long s_i[2], s_n[2];
-    __shared__ double s_d[2];
-    __shared__ int s_nan;
-    if (threadIdx.x == 0) { s_i[0] = INT64_MAX; s_i[1] = INT64_MIN; s_d[0] = INFINITY; s_d[1] = -INFINITY; s_n[0] = s_n[1] = 0; s_nan = 0; }
-    __syncthreads();
-    if (fp) {
-        // doubles: order-preserving via atomicMin/Max on the transformed bit pattern is overkill here: serialise
-        // per warp leader through a CAS loop on the shared doubles
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) {
-            dmin = fmin(dmin, __shfl_xor_sync(0xffffffffu, dmin, d));
-            dmax = fmax(dmax, __shfl_xor_sync(0xffffffffu, dmax, d));
-        }
-        if ((threadIdx.x & 31) == 0) {
-            unsigned long long *pmin = (unsigned long long *)&s_d[0], *pmax = (unsigned long long *)&s_d[1];
-            unsigned long long old = *pmin;
-            while (dmin < __longlong_as_double((long long)old)) {
-                unsigned long long prev = atomicCAS(pmin, old, (unsigned long long)__double_as_longlong(dmin));
-                if (prev == old) break;
-                old = prev;
-            }
-            old = *pmax;
-            while (dmax > __longlong_as_double((long long)old)) {
-                unsigned long long prev = atomicCAS(pmax, old, (unsigned long long)__double_as_longlong(dmax));
-                if (prev == old) break;
-                old = prev;
-            }
-        }
-        if (nan_seen) s_nan = 1;
-    } else {
-        atomicMin(&s_i[0], (long long)imin);
-        atomicMax(&s_i[1], (long long)imax);
-    }
-    atomicAdd((unsigned long long *)&s_n[0], (unsigned long long)nn);
-    atomicAdd((unsigned long long *)&s_n[1], (unsigned long long)retr);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        int64_t *o = out + kStatWords * (int64_t)blockIdx.x;
-        if (fp) { o[0] = __double_as_longlong(s_d[0]); o[1] = __double_as_longlong(s_d[1]); }
-        else { o[0] = s_i[0]; o[1] = s_i[1]; }
-        o[2] = s_n[0];
-        o[3] = s_n[1];
-        o[4] = s_nan;
-    }
-}
-
-// host-built pieces of the file (page headers, level prefixes, footer) -> their places in the device image
-struct PatchJob { int64_t dst; int32_t src, len; };
-__global__ void k_pw_patch(const PatchJob *jobs, int n, const uint8_t *bytes, uint8_t *file) {
-    const int j = (int)(((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
-    if (j >= n) return;
-    const PatchJob pj = jobs[j];
-    for (int i = lane; i < pj.len; i += 32) file[pj.dst + i] = bytes[pj.src + i];
-}
-
-// ------------------------------------------------------------------ zstd page compression
-// The page bodies are written into a scratch image, every 128 KiB block of every body is compressed by one warp, the
-// per-page frame sizes go back to the host (which lays out the file and writes the page headers), and a gather places
-// the frames at their file offsets.
-
-constexpr size_t kZsSmem = (sizeof(int32_t) << zs::kHashLog) + sizeof(zs::EncWork);
-
-__global__ void __launch_bounds__(32)
-k_zs_block(const ZsBlockJob *jobs, const uint8_t *img, uint8_t *out, zs::Seq *seqs, uint8_t *lits, int2 *res) {
-    extern __shared__ __align__(16) uint8_t zs_smem[];
-    int32_t *htab = (int32_t *)zs_smem;
-    zs::EncWork &W = *(zs::EncWork *)(zs_smem + (sizeof(int32_t) << zs::kHashLog));
-    const ZsBlockJob j = jobs[blockIdx.x];
-    const zs::BlockOut r = zs::compress_block(img + j.src, j.n, out + j.out, htab, seqs + j.seq, lits + j.src, W);
-    if (threadIdx.x == 0) res[blockIdx.x] = make_int2(r.type, r.size);
-}
-
-// per page: where each block's header goes inside the frame, and the frame size
-__global__ void k_zs_page_sizes(const ZsPage *pages, int n_pages, const int2 *res, int32_t *boff, int64_t *frame_bytes) {
-    const int p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= n_pages) return;
-    const ZsPage pg = pages[p];
-    int64_t off = zs::frame_header_size((uint64_t)pg.raw);
-    for (int b = 0; b < pg.n_blocks; b++) {
-        boff[pg.first_block + b] = (int32_t)off;
-        off += 3 + res[pg.first_block + b].y;
-    }
-    frame_bytes[p] = off;
-}
-
-// one CTA per block: frame header (first block of a page), block header, payload at the frame's file offset
-__global__ void k_zs_gather(const ZsBlockJob *jobs, const ZsPage *pages, const int2 *res, const int32_t *boff,
-                            const int64_t *frame_off, const uint8_t *img, const uint8_t *out, uint8_t *file) {
-    const ZsBlockJob j = jobs[blockIdx.x];
-    const ZsPage pg = pages[j.page];
-    const int2 r = res[blockIdx.x];
-    uint8_t *frame = file + frame_off[j.page];
-    uint8_t *dst = frame + boff[blockIdx.x];
-    if (threadIdx.x == 0) {
-        if ((int)blockIdx.x == pg.first_block) zs::write_frame_header(frame, (uint64_t)pg.raw);
-        zs::write_block_header(dst, (int)blockIdx.x == pg.first_block + pg.n_blocks - 1, r.x,
-                               r.x == 2 ? (uint32_t)r.y : (uint32_t)j.n);
-    }
-    const uint8_t *pay = r.x == 0 ? img + j.src : out + j.out;
-    for (int i = threadIdx.x; i < r.y; i += blockDim.x) dst[3 + i] = pay[i];
-}
-
-// ------------------------------------------------------------------ host orchestration
-
-Table<EncodedFile> g_enc(6);
-
-void launch_pw_stats(const EncColumn *cols, const StatJob *jobs, int n_jobs, int64_t *out) {
-    if (n_jobs) k_pw_stats<<<(unsigned)n_jobs, 256>>>(cols, jobs, out);
-}
-
-void launch_zs_compress(const ZsBlockJob *jobs, int n_blocks, const ZsPage *pages, int n_pages, const uint8_t *img,
-                        uint8_t *out, void *seqs, uint8_t *lits, int2 *res, int32_t *boff, int64_t *frame_bytes) {
-    k_zs_block<<<(unsigned)n_blocks, 32, kZsSmem>>>(jobs, img, out, (zs::Seq *)seqs, lits, res);
-    k_zs_page_sizes<<<(unsigned)((n_pages + 127) / 128), 128>>>(pages, n_pages, res, boff, frame_bytes);
-}
-
-size_t zs_seq_bytes(int64_t seq) { return sizeof(zs::Seq) * (size_t)seq; }
-
 static int parquet_type_of(int t) {
     switch (t) {
         case PG_BOOL: return pq::T_BOOLEAN;
@@ -345,41 +199,13 @@ static Plan make_plan(const Schema &s, const std::vector<DevColumn> &dcols, int6
     return pl;
 }
 
-// The device's counts -> each page's level prefix and body size, each chunk's statistics, the file's statistics of
-// each column, and the count of retract rows in column `kind_col`.  counts: per page, non-null rows and payload
-// bytes (k_pw_count); stats: per chunk, kStatWords (k_pw_stats).
-static pg_status fold_counts(Plan &pl, const int64_t *counts, const int64_t *stats, int kind_col,
-                             std::vector<ColStats> &file, int64_t &deletes) {
-    const int nc = (int)pl.cols.size();
-    file.assign(nc, ColStats{INT64_MAX, INT64_MIN, 0, 0});
-    std::vector<char> file_nan(nc, 0);                       // per column: a chunk holds a NaN
+// The device's counts -> each page's level prefix and body size, each chunk's statistics (folded into the file's by
+// `fs`).  counts: per page, non-null rows and payload bytes (k_pw_count); stats: per chunk, kStatWords (k_pw_stats).
+static pg_status fold_counts(Plan &pl, const int64_t *counts, const int64_t *stats, FileStats &fs) {
     for (size_t k = 0; k < pl.chunks.size(); k++) {
-        const int c = pl.sjobs[k].col;
-        const EncColumn &ec = pl.cols[c];
-        const int64_t *cs = &stats[kStatWords * k];
-        const bool fp = ec.type == PG_FLOAT || ec.type == PG_DOUBLE, nan = cs[4] != 0;
+        const EncColumn &ec = pl.cols[pl.sjobs[k].col];
         Chunk &ch = pl.chunks[k];
-        ch.st.null_count = pl.sjobs[k].n_rows - cs[2];
-        ch.st.has_minmax = ec.width > 0 && cs[2] > 0 && !nan;   // a chunk with a NaN has no min / max
-        ch.st.min = cs[0];
-        ch.st.max = cs[1];
-        // parquet.thrift, Statistics: a zero min of a floating point column is written as -0.0, a zero max as +0.0,
-        // so that min <= v <= max holds for both zeros in the order readers compare with (Double.compare: -0.0 <
-        // +0.0).  The file-level merge below keeps the rule: the zero min it can take is -0.0, the zero max +0.0.
-        if (fp && ch.st.has_minmax) { ch.st.min = zero_as(ch.st.min, -0.0); ch.st.max = zero_as(ch.st.max, 0.0); }
-        file_nan[c] |= nan;
-        ColStats &fs = file[c];
-        fs.null_count += ch.st.null_count;
-        if (ch.st.has_minmax) {
-            if (!fs.has_minmax) { fs.min = ch.st.min; fs.max = ch.st.max; fs.has_minmax = 1; }
-            else if (fp) {
-                double a, b, x, y;
-                memcpy(&a, &fs.min, 8); memcpy(&b, &fs.max, 8); memcpy(&x, &ch.st.min, 8); memcpy(&y, &ch.st.max, 8);
-                a = std::min(a, x); b = std::max(b, y);
-                memcpy(&fs.min, &a, 8); memcpy(&fs.max, &b, 8);
-            } else { fs.min = std::min(fs.min, ch.st.min); fs.max = std::max(fs.max, ch.st.max); }
-        }
-        if (c == kind_col) deletes += cs[3];
+        ch.st = fs.add(pl.sjobs[k].col, ec, &stats[kStatWords * k], pl.sjobs[k].n_rows);
         for (size_t p = ch.page0; p < ch.page1; p++) {
             Page &pg = pl.pages[p];
             const int64_t nn = counts[2 * p], vb = counts[2 * p + 1];
@@ -400,10 +226,6 @@ static pg_status fold_counts(Plan &pl, const int64_t *counts, const int64_t *sta
             if (pg.body > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet encode: page larger than 2 GiB");
         }
     }
-    // A file with a NaN in a FLOAT / DOUBLE column has no min / max for that column, though its other chunks have
-    // some: NaN sorts above every value (Double.compare), so a max taken around it would prune rows `x > max` matches.
-    for (int c = 0; c < nc; c++)
-        if (file_nan[c]) file[c] = ColStats{INT64_MAX, INT64_MIN, file[c].null_count, 0};
     return PG_OK;
 }
 
@@ -420,24 +242,6 @@ static std::vector<Part> place_bodies(Plan &pl, const std::vector<int64_t> &base
         pl.jobs[p].val_off = base[p] + pg.def_bytes;
     }
     return prefixes;
-}
-
-pg_status patch(Scratch &scratch, const std::vector<Part> &parts, uint8_t *dst, const char *what) {
-    if (parts.empty()) return PG_OK;
-    std::vector<PatchJob> jobs;
-    std::vector<uint8_t> bytes;
-    for (const Part &p : parts) {
-        if (bytes.size() + p.second.size() > 0x7fffffffull) return fail(PG_ERR_UNSUPPORTED, "parquet encode: too many header bytes");
-        jobs.push_back(PatchJob{p.first, (int32_t)bytes.size(), (int32_t)p.second.size()});
-        bytes.insert(bytes.end(), p.second.begin(), p.second.end());
-    }
-    PatchJob *d_jobs = (PatchJob *)scratch.take(sizeof(PatchJob) * jobs.size() + 16);
-    uint8_t *d_bytes = (uint8_t *)scratch.take(bytes.size() + 16);
-    if (!d_jobs || !d_bytes) return fail(PG_ERR_CUDA, std::string("parquet encode: out of device memory for ") + what);
-    PG_CUDA(cudaMemcpy(d_jobs, jobs.data(), sizeof(PatchJob) * jobs.size(), cudaMemcpyHostToDevice));
-    PG_CUDA(cudaMemcpy(d_bytes, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
-    k_pw_patch<<<(unsigned)((jobs.size() * 32 + 127) / 128), 128>>>(d_jobs, (int)jobs.size(), d_bytes, dst);
-    return PG_OK;
 }
 
 // PageHeader of a data page V1: PLAIN values, RLE levels
@@ -545,28 +349,16 @@ static std::vector<uint8_t> footer(const Plan &pl, const char *const *names, int
 
 static pg_status encode(uint64_t source, const char *const *names, int64_t row0, int64_t n_rows,
                         const pg_parquet_write_options *opt, int codec, uint64_t *out_file) {
-    pg_status st = ensure_device();
-    if (st) return st;
     BatchColumns batch;                                      // held until the encode below is done
-    st = batch_columns(source, &batch);
+    pg_status st = encode_source(source, "parquet encode", row0, &n_rows, &batch);
     if (st) return st;
     const Schema *s = batch.schema.get();
-    const std::vector<DevColumn> &dcols = batch.cols;
-    for (int c = 0; c < s->n_cols() && batch.n_rows > 0; c++)
-        if (!dcols[c].data && !dcols[c].offsets)
-            return fail(PG_ERR_INVALID, "parquet encode: the batch was produced under a read-type projection and has no "
-                                        "column " + std::to_string(c) + "; a data file needs every column");
-    if (n_rows < 0) n_rows = batch.n_rows - row0;
-    if (row0 < 0 || (row0 & 7) || row0 + n_rows > batch.n_rows)
-        return fail(PG_ERR_INVALID, "parquet encode: row range outside the batch or not starting at a multiple of 8");
     const int nc = s->n_cols();
 
     SectionTimer tm;
-    PG_CUDA(cudaEventCreate(&tm.e0));
-    PG_CUDA(cudaEventCreate(&tm.e1));
-    PG_CUDA(cudaEventRecord(tm.e0, 0));
+    if ((st = start_encode(tm))) return st;
 
-    Plan pl = make_plan(*s, dcols, row0, n_rows, opt);
+    Plan pl = make_plan(*s, batch.cols, row0, n_rows, opt);
     const size_t nj = pl.jobs.size(), nsj = pl.sjobs.size();
     std::vector<int64_t> counts(2 * nj + 2), stats(kStatWords * (nsj + 1));
     Scratch scratch(0);                                      // temporaries, released on every path out of this function
@@ -583,73 +375,38 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         PG_CUDA(cudaMemcpy(d_jobs, pl.jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
         PG_CUDA(cudaMemcpy(d_sjobs, pl.sjobs.data(), sizeof(StatJob) * nsj, cudaMemcpyHostToDevice));
         k_pw_count<<<(unsigned)nj, 256>>>(d_cols, d_jobs, d_counts);
-        k_pw_stats<<<(unsigned)nsj, 256>>>(d_cols, d_sjobs, d_stats);
+        launch_pw_stats(d_cols, d_sjobs, (int)nsj, d_stats);
         launches += 2;
         PG_CUDA(cudaMemcpy(counts.data(), d_counts, sizeof(int64_t) * 2 * nj, cudaMemcpyDeviceToHost));
         PG_CUDA(cudaMemcpy(stats.data(), d_stats, sizeof(int64_t) * kStatWords * nsj, cudaMemcpyDeviceToHost));
     }
     auto ef = std::make_unique<EncodedFile>();
-    if ((st = fold_counts(pl, counts.data(), stats.data(), s->n_key + 1, ef->stats, ef->meta.delete_row_count)))
-        return st;
+    FileStats fs(*s);
+    if ((st = fold_counts(pl, counts.data(), stats.data(), fs))) return st;
+    fs.finish(*ef);
 
     // ---- zstd: bodies into a scratch image, one frame per body; the frame sizes come back before the layout
     const bool zstd = codec == pq::C_ZSTD;
-    size_t nb = 0;
-    uint8_t *d_img = nullptr, *d_zout = nullptr;
-    ZsBlockJob *d_bjobs = nullptr;
-    ZsPage *d_zpages = nullptr;
-    int2 *d_res = nullptr;
-    int32_t *d_boff = nullptr;
-    int64_t *d_frame = nullptr;
+    ZstdFrames frames("parquet encode");
     if (zstd && nj) {
-        std::vector<ZsBlockJob> bjobs;
-        std::vector<ZsPage> zpages(nj);
-        std::vector<int64_t> img_off(nj);
-        int64_t img = 0, out = 0, seq = 0;
+        std::vector<ZstdFrames::Body> bodies;
+        std::vector<int64_t> img_off(nj), frame_bytes;
+        int64_t img = 0;
         for (size_t p = 0; p < nj; p++) {
-            const int64_t body = pl.pages[p].body;
             img_off[p] = img;
-            zpages[p] = ZsPage{body, (int32_t)bjobs.size(), 0};
-            for (int64_t b0 = 0; b0 == 0 || b0 < body; b0 += zs::kMaxBlock) {
-                const int32_t n = (int32_t)std::min<int64_t>(zs::kMaxBlock, body - b0);
-                bjobs.push_back(ZsBlockJob{img + b0, out, seq, n, (int32_t)p});
-                out += n;
-                seq += n / 4 + 1;
-                zpages[p].n_blocks++;
-            }
-            img += body;
+            bodies.push_back({img, pl.pages[p].body});
+            img += pl.pages[p].body;
         }
         const std::vector<Part> prefixes = place_bodies(pl, img_off);
-        nb = bjobs.size();
-        d_img = (uint8_t *)scratch.take((size_t)img + 64);
-        d_zout = (uint8_t *)scratch.take((size_t)out + 64);
-        uint8_t *d_lits = (uint8_t *)scratch.take((size_t)img + 64);
-        zs::Seq *d_seqs = (zs::Seq *)scratch.take(sizeof(zs::Seq) * (size_t)seq);
-        d_bjobs = (ZsBlockJob *)scratch.take(sizeof(ZsBlockJob) * nb);
-        d_zpages = (ZsPage *)scratch.take(sizeof(ZsPage) * nj);
-        d_res = (int2 *)scratch.take(sizeof(int2) * nb);
-        d_boff = (int32_t *)scratch.take(sizeof(int32_t) * nb);
-        d_frame = (int64_t *)scratch.take(sizeof(int64_t) * nj);
-        if (!d_img || !d_zout || !d_lits || !d_seqs || !d_bjobs || !d_zpages || !d_res || !d_boff || !d_frame)
-            return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the zstd page images");
+        uint8_t *d_img = (uint8_t *)scratch.take((size_t)img + 64);
+        if (!d_img) return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the zstd page images");
         PG_CUDA(cudaMemsetAsync(d_img, 0, (size_t)img + 64, 0));
         PG_CUDA(cudaMemcpy(d_jobs, pl.jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
-        PG_CUDA(cudaMemcpy(d_bjobs, bjobs.data(), sizeof(ZsBlockJob) * nb, cudaMemcpyHostToDevice));
-        PG_CUDA(cudaMemcpy(d_zpages, zpages.data(), sizeof(ZsPage) * nj, cudaMemcpyHostToDevice));
         k_pw_encode<<<(unsigned)nj, 256>>>(d_cols, d_jobs, d_img);
         launches++;
         if ((st = patch(scratch, prefixes, d_img, "the zstd page images"))) return st;
         if (!prefixes.empty()) launches++;
-        k_zs_block<<<(unsigned)nb, 32, kZsSmem>>>(d_bjobs, d_img, d_zout, d_seqs, d_lits, d_res);
-        k_zs_page_sizes<<<(unsigned)((nj + 127) / 128), 128>>>(d_zpages, (int)nj, d_res, d_boff, d_frame);
-        launches += 2;
-        std::vector<int64_t> frame_bytes(nj);
-        SmallReads rd(0);
-        if ((st = rd.add(frame_bytes.data(), d_frame, sizeof(int64_t) * nj))) return st;
-        launches++;
-        if ((st = rd.finish())) return st;
-        cudaError_t le = cudaGetLastError();
-        if (le != cudaSuccess) return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(le));
+        if ((st = frames.compress(scratch, d_img, bodies, &frame_bytes, &launches))) return st;
         for (size_t p = 0; p < nj; p++) pl.pages[p].stored = frame_bytes[p];
     }
 
@@ -675,36 +432,19 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     ef->file_bytes = pos + (int64_t)ef->host_parts.back().second.size();
 
     // ---- page bodies on the device: the zstd frames gathered, or the bodies written in place behind their prefixes
-    PG_CUDA(cudaMalloc(&ef->d_file, (size_t)ef->file_bytes + 64));
-    PG_CUDA(cudaMemsetAsync(ef->d_file, 0, (size_t)ef->file_bytes + 64, 0));
+    if ((st = ef->alloc_image())) return st;
     if (nj && zstd) {
-        // (the frame sizes have been read: their buffer takes the frame offsets)
-        PG_CUDA(cudaMemcpy(d_frame, body_off.data(), sizeof(int64_t) * nj, cudaMemcpyHostToDevice));
-        k_zs_gather<<<(unsigned)nb, 256>>>(d_bjobs, d_zpages, d_res, d_boff, d_frame, d_img, d_zout, ef->d_file);
-        launches++;
+        if ((st = frames.gather(body_off, {}, ef->d_file, &launches))) return st;
     } else if (nj) {
         for (Part &prefix : place_bodies(pl, body_off)) ef->host_parts.push_back(std::move(prefix));
         PG_CUDA(cudaMemcpy(d_jobs, pl.jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
         k_pw_encode<<<(unsigned)nj, 256>>>(d_cols, d_jobs, ef->d_file);
         launches++;
     }
-    PG_CUDA(cudaEventRecord(tm.e1, 0));
-    PG_CUDA(cudaEventSynchronize(tm.e1));
-    const float ms = tm.ms();
-    cudaError_t le = cudaGetLastError();
-    if (le != cudaSuccess) return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(le));
-
     ef->meta.n_rows = n_rows;
-    ef->meta.file_bytes = ef->file_bytes;
     ef->meta.n_row_groups = (int32_t)pl.n_groups;
     ef->meta.n_pages = (int)nj;
-    ef->meta.ms_encode = ms;
-    ef->meta.launches = launches;
-    const ColStats &sq = ef->stats[s->n_key];
-    ef->meta.min_sequence_number = sq.has_minmax ? sq.min : 0;
-    ef->meta.max_sequence_number = sq.has_minmax ? sq.max : 0;
-    *out_file = g_enc.put(std::move(ef));
-    return PG_OK;
+    return finish_encode(tm, std::move(ef), launches, "parquet encode", out_file);
 }
 
 }  // namespace pg
@@ -732,58 +472,6 @@ pg_status pg_parquet_encode_compressed(uint64_t source, const char *const *colum
         return fail(PG_ERR_UNSUPPORTED, "parquet encode: file.compression.zstd-level " + std::to_string(level) +
                                             " is not written on the device (level 1 and the negative fast levels are)");
     return encode(source, column_names, row0, n_rows, options, codec, out_file);
-}
-
-pg_status pg_parquet_file_meta(uint64_t file, pg_file_meta *out) {
-    std::shared_ptr<EncodedFile> ef = g_enc.get(file);
-    if (!ef || !out) return fail(PG_ERR_INVALID, "unknown encoded file handle");
-    *out = ef->meta;
-    return PG_OK;
-}
-
-pg_status pg_parquet_file_column_stats(uint64_t file, int32_t column, int64_t *null_count, int32_t *has_min_max,
-                                       void *min8, void *max8) {
-    std::shared_ptr<EncodedFile> ef = g_enc.get(file);
-    if (!ef) return fail(PG_ERR_INVALID, "unknown encoded file handle");
-    if (column < 0 || column >= (int32_t)ef->stats.size()) return fail(PG_ERR_INVALID, "column out of range");
-    const ColStats &cs = ef->stats[column];
-    if (null_count) *null_count = cs.null_count;
-    if (has_min_max) *has_min_max = cs.has_minmax;
-    if (min8) memcpy(min8, &cs.min, 8);
-    if (max8) memcpy(max8, &cs.max, 8);
-    return PG_OK;
-}
-
-pg_status pg_parquet_file_fetch(uint64_t file, void *host_buffer, int64_t capacity) {
-    std::shared_ptr<EncodedFile> ef = g_enc.get(file);
-    if (!ef || !host_buffer) return fail(PG_ERR_INVALID, "unknown encoded file handle");
-    if (capacity < ef->file_bytes) return fail(PG_ERR_INVALID, "buffer smaller than the file");
-    pg_status st = ensure_device();
-    if (st) return st;
-    PG_CUDA(cudaMemcpy(host_buffer, ef->d_file, (size_t)ef->data_end, cudaMemcpyDeviceToHost));
-    for (const auto &p : ef->host_parts) memcpy((uint8_t *)host_buffer + p.first, p.second.data(), p.second.size());
-    return PG_OK;
-}
-
-pg_status pg_parquet_file_device_image(uint64_t file, const uint8_t **device_bytes, int64_t *size) {
-    std::shared_ptr<EncodedFile> ef = g_enc.get(file);
-    if (!ef || !device_bytes || !size) return fail(PG_ERR_INVALID, "unknown encoded file handle");
-    pg_status st = ensure_device();
-    if (st) return st;
-    if (!ef->image_complete) {
-        Scratch scratch(0);
-        if ((st = patch(scratch, ef->host_parts, ef->d_file, "the header patch"))) return st;
-        cudaError_t e = cudaDeviceSynchronize();
-        if (e != cudaSuccess) return fail(PG_ERR_CUDA, std::string("parquet encode: ") + cudaGetErrorString(e));
-        ef->image_complete = true;
-    }
-    *device_bytes = ef->d_file;
-    *size = ef->file_bytes;
-    return PG_OK;
-}
-
-pg_status pg_parquet_file_free(uint64_t file) {
-    return g_enc.take(file) ? PG_OK : fail(PG_ERR_INVALID, "unknown encoded file handle");
 }
 
 }  // extern "C"

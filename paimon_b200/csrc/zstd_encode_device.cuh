@@ -1,8 +1,8 @@
 // zstd_encode_device.cuh — Zstandard frame encoder for Parquet page bodies, written once for host and device.
 //
 // Paimon compresses every data file it writes with zstd level 1 unless told otherwise (CoreOptions.java:318-330,
-// 'file.compression' / 'file.compression.zstd-level'), so the compaction output encoder (parquet_encode.cu) writes one
-// zstd frame per page body.  The format is the public Zstandard specification (RFC 8878), the same one the decoder in
+// 'file.compression' / 'file.compression.zstd-level'), so the compaction output encoders write one zstd frame per
+// Parquet page body or ORC compression chunk (ZstdFrames, encoded_file.cu).  The format is the public Zstandard specification (RFC 8878), the same one the decoder in
 // zstd_device.cuh restates; the code tables (ll_code_info / ml_code_info) and the predefined distributions are that
 // header's.
 //
@@ -644,7 +644,7 @@ ZS_HD inline void write_block_header(uint8_t *d, int last, int type, uint32_t si
 ZS_HD inline int64_t frame_bound(int64_t n) { return frame_header_size((uint64_t)n) + n + 3 * (n / kMaxBlock + 1); }
 
 // A whole frame, block after block (the host build; the device runs the blocks as separate warps and places them with
-// a gather, parquet_encode.cu).  `htab` 2^kHashLog entries, `seqs` kMaxBlock / 4 + 1, `lits` and `out_blk` kMaxBlock
+// a gather, encoded_file.cu).  `htab` 2^kHashLog entries, `seqs` kMaxBlock / 4 + 1, `lits` and `out_blk` kMaxBlock
 // bytes.  Returns the frame size, or -1 when it does not fit `cap`.
 ZS_HD inline int64_t compress_frame(const uint8_t *src, int64_t n, uint8_t *dst, int64_t cap, int32_t *htab, Seq *seqs,
                                     uint8_t *lits, uint8_t *out_blk, EncWork &W) {

@@ -202,6 +202,60 @@ def test_accessors_and_nan_statistics(tmp_path):
     assert written.n_pages > 0 and written.meta.file_size == os.path.getsize(path)
 
 
+def _chunks(blob, block):
+    """(original, length, offset) of every compression chunk between the magic and the PostScript: the streams, the
+    stripe footers, the Metadata and the Footer, back to back"""
+    end = len(blob) - 1 - blob[-1]
+    pos, out = 3, []
+    while pos < end:
+        h = blob[pos] | blob[pos + 1] << 8 | blob[pos + 2] << 16
+        length = h >> 1
+        assert 0 < length <= block and pos + 3 + length <= end, (pos, length)
+        out.append((h & 1, length, pos + 3))
+        pos += 3 + length
+    assert pos == end
+    return out
+
+
+def _zstd_blocks(frame):
+    """the number of blocks of one zstd frame (RFC 8878), which has to fill `frame` exactly"""
+    assert frame[:4] == b"\x28\xb5\x2f\xfd"
+    fhd = frame[4]
+    single = fhd >> 5 & 1
+    pos = 5 + (1 - single) + (0, 1, 2, 4)[fhd & 3] + (single, 2, 4, 8)[fhd >> 6]
+    n = 0
+    while True:
+        h = frame[pos] | frame[pos + 1] << 8 | frame[pos + 2] << 16
+        pos += 3 + (1 if (h >> 1 & 3) == 1 else h >> 3)             # an RLE block holds one byte
+        n += 1
+        if h & 1:
+            break
+    assert pos + 4 * (fhd >> 2 & 1) == len(frame)
+    return n
+
+
+def test_zstd_chunks_stored_original_and_compressed(tmp_path):
+    """ORC ZSTD chunks as the device gathers them.  Under a 4096-byte block, random bytes are stored as original
+    chunks and a repeated string as compressed ones.  Under the default 256 KiB block, the 400 KB stream of the
+    repeated string has a chunk whose frame holds two zstd blocks, and the random one an original chunk longer than a
+    block.  Every chunk header is walked; the files read back through pyarrow.orc and the device decoder."""
+    vt = RowType((DataField("pk", "INT", False), DataField("rnd", "BYTES", False), DataField("rep", "STRING", False)))
+    schema = KeyValueSchema.of(vt, ["pk"])
+    rng = random.Random(11)
+    n = 8000
+    batch = KeyValueBatch.from_rows(schema, [(k, k + 1, 0, k, rng.randbytes(50), "paimon-orc" * 5) for k in range(n)])
+    for block in (4096, 0):
+        path = str(tmp_path / f"block{block}.orc")
+        written = encode(schema, batch, path, compression="zstd", compression_block_size=block)
+        check_file(schema, batch, path, written, 0)
+        chunks = _chunks(open(path, "rb").read(), block or 256 << 10)
+        assert any(orig for orig, _, _ in chunks) and any(not orig for orig, _, _ in chunks), block
+        if not block:
+            blob = open(path, "rb").read()
+            assert any(not orig and _zstd_blocks(blob[at:at + ln]) >= 2 for orig, ln, at in chunks)
+            assert any(orig and ln > 128 << 10 for orig, ln, _ in chunks)
+
+
 def test_refusals():
     schema = all_types_schema()
     batch = KeyValueBatch.from_rows(schema, random_rows(random.Random(5), 100, 0.2))

@@ -61,7 +61,7 @@ enum {
     PG_ERR_UNSUPPORTED = 2,     /* spec refused at plan time (no CPU fallback) */
     PG_ERR_CUDA = 3,
     PG_ERR_MERGE_FUNCTION = 4,  /* the Java MergeFunction would have thrown; message says which */
-    PG_ERR_INTERNAL = 5,
+    PG_ERR_INTERNAL = 5,        /* a limit of the device path: a merge tile overflowed, a var-len column passed 2 GiB */
     PG_ERR_FORMAT = 6           /* malformed / unsupported file bytes */
 };
 

@@ -390,6 +390,45 @@ void RunBuilder::finish(uint64_t *out_runs, int64_t bytes_h2d, pg_section_info *
     }
 }
 
+SectionFrame::SectionFrame(std::shared_ptr<const Schema> s, int n_runs, const char *who)
+    : stream(copy_stream()), scratch(stream), b(std::move(s), n_runs, scratch, who) {}
+
+pg_status SectionFrame::start(const uint8_t *read_cols, const char *const *names) {
+    PG_CUDA(cudaEventCreate(&tm.e0));
+    PG_CUDA(cudaEventCreate(&tm.e1));
+    PG_CUDA(cudaEventRecord(tm.e0, stream));
+    return b.read_columns(read_cols, names);
+}
+
+pg_status SectionFrame::place(const pg_file_desc *files, int n_files) {
+    d_file.assign(n_files, nullptr);
+    for (int f = 0; f < n_files; f++) {
+        file_bytes += files[f].size;
+        if (files[f].mem == PG_MEM_DEVICE) { d_file[f] = files[f].bytes; continue; }
+        { pg_status st = file_image(scratch, files[f].bytes, files[f].size, b.who, &d_file[f]); if (st) return st; }
+        h2d += files[f].size;
+    }
+    return PG_OK;
+}
+
+pg_status SectionFrame::finish(const int32_t *d_err, uint64_t *out_runs, pg_section_info *info) {
+    PG_CUDA(cudaEventRecord(tm.e1, stream));
+    int32_t herr = 0;
+    SmallReads rb(stream);
+    { pg_status rs = rb.add(&herr, d_err, 4); if (!rs) rs = rb.finish(); if (rs) return rs; }
+    PG_CUDA(cudaGetLastError());
+    { pg_status st = kernel_error(herr, b.who); if (st) return st; }
+    b.finish(out_runs, h2d, info);
+    if (info) {
+        info->file_bytes = file_bytes;
+        info->page_bytes = page_bytes;
+        info->n_files = (int32_t)d_file.size();
+        info->launches = launches;
+        info->ms_decode = tm.ms();
+    }
+    return PG_OK;
+}
+
 // drop the current batch; the arena itself is kept for the next execute unless `release_memory`
 static void free_outputs(Merge *m, bool release_memory = false) {
     m->out_cols.clear();
@@ -627,37 +666,46 @@ static pg_status build_descriptors(Merge *m) {
     return PG_OK;
 }
 
-static const char *kernel_error_message(int code) {
-    switch (code) {
-        case KERR_TILE_OVERFLOW:
-            return "internal: a merge tile overflowed (does a run contain duplicate keys? "
-                   "SortMergeReader.java:37 requires unique keys per reader)";
-        case KERR_PU_DELETE:
-            return "By default, Partial update can not accept delete records, you can choose one of the "
-                   "following solutions:\n1. Configure 'ignore-delete' to ignore delete records.\n"
-                   "2. Configure 'partial-update.remove-record-on-delete' to remove the whole row when "
-                   "receiving delete records.\n3. Configure 'sequence-group's to retract partial columns. "
-                   "Also configure 'partial-update.remove-record-on-sequence-group' to remove the whole "
-                   "row when receiving deleted records of `specified sequence group`.";
-        case KERR_FIRST_ROW_RETRACT:
-            return "By default, First row merge engine can not accept DELETE/UPDATE_BEFORE records.\n"
-                   "You can config 'ignore-delete' to ignore the DELETE/UPDATE_BEFORE records.";
-        case KERR_AGG_RETRACT:
-            return "Aggregate function does not support retraction, If you allow this function to ignore "
-                   "retraction messages, you can configure 'fields.${field_name}.ignore-retract'='true'.";
-        case KERR_OFFSET_OVERFLOW:
-            return "a var-len output column exceeds 2 GiB (int32 offsets); merge fewer rows per call";
-        case KERR_DIV_ZERO:
-            return "ArithmeticException: / by zero";
-        case KERR_DEC_DIV_ZERO:
-            return "ArithmeticException: Division by zero";
-        case KERR_DEC_DIV_UNDEFINED:
-            return "ArithmeticException: Division undefined";
-        case KERR_DEC_NON_TERMINATING:
-            return "ArithmeticException: Non-terminating decimal expansion; no exact representable decimal result.";
-        default:
-            return "unknown kernel error";
-    }
+pg_status kernel_error(int code, const char *who) {
+    static const struct { int code; pg_status st; const char *msg; } kErrors[] = {
+        // what the Java merge functions throw, verbatim
+        {KERR_PU_DELETE, PG_ERR_MERGE_FUNCTION,
+         "By default, Partial update can not accept delete records, you can choose one of the "
+         "following solutions:\n1. Configure 'ignore-delete' to ignore delete records.\n"
+         "2. Configure 'partial-update.remove-record-on-delete' to remove the whole row when "
+         "receiving delete records.\n3. Configure 'sequence-group's to retract partial columns. "
+         "Also configure 'partial-update.remove-record-on-sequence-group' to remove the whole "
+         "row when receiving deleted records of `specified sequence group`."},
+        {KERR_FIRST_ROW_RETRACT, PG_ERR_MERGE_FUNCTION,
+         "By default, First row merge engine can not accept DELETE/UPDATE_BEFORE records.\n"
+         "You can config 'ignore-delete' to ignore the DELETE/UPDATE_BEFORE records."},
+        {KERR_AGG_RETRACT, PG_ERR_MERGE_FUNCTION,
+         "Aggregate function does not support retraction, If you allow this function to ignore "
+         "retraction messages, you can configure 'fields.${field_name}.ignore-retract'='true'."},
+        {KERR_DIV_ZERO, PG_ERR_MERGE_FUNCTION, "ArithmeticException: / by zero"},
+        {KERR_DEC_DIV_ZERO, PG_ERR_MERGE_FUNCTION, "ArithmeticException: Division by zero"},
+        {KERR_DEC_DIV_UNDEFINED, PG_ERR_MERGE_FUNCTION, "ArithmeticException: Division undefined"},
+        {KERR_DEC_NON_TERMINATING, PG_ERR_MERGE_FUNCTION,
+         "ArithmeticException: Non-terminating decimal expansion; no exact representable decimal result."},
+        // limits of the device path
+        {KERR_TILE_OVERFLOW, PG_ERR_INTERNAL,
+         "a merge tile overflowed (does a run contain duplicate keys? SortMergeReader.java:37 requires unique keys per reader)"},
+        {KERR_OFFSET_OVERFLOW, PG_ERR_INTERNAL, "a var-len column exceeds 2 GiB of payload"},
+        // file bytes
+        {KERR_BAD_PAGE, PG_ERR_FORMAT, "a page or stream does not decode (malformed file or unsupported encoding)"},
+        {KERR_PQ_HEADER, PG_ERR_FORMAT, "malformed or truncated page header"},
+        {KERR_PQ_NO_DICT, PG_ERR_FORMAT, "dictionary-encoded page without dictionary"},
+        {KERR_PQ_ROWS, PG_ERR_FORMAT, "page row counts do not add up"},
+        {KERR_PQ_DICT_ID, PG_ERR_FORMAT, "dictionary id outside the dictionary"},
+        {KERR_PQ_ENCODING, PG_ERR_UNSUPPORTED,
+         "a page uses a value encoding the device decoder does not implement (PLAIN, dictionary, DELTA_BINARY_PACKED "
+         "integers and RLE booleans are decoded)"},
+        {KERR_PQ_LEVELS, PG_ERR_UNSUPPORTED, "repetition levels / BIT_PACKED definition levels are not decoded on device"},
+    };
+    if (code == KERR_NONE) return PG_OK;
+    for (const auto &e : kErrors)
+        if (e.code == code) return fail(e.st, e.st == PG_ERR_MERGE_FUNCTION ? std::string(e.msg) : std::string(who) + ": " + e.msg);
+    return fail(PG_ERR_INTERNAL, std::string(who) + ": unknown kernel error " + std::to_string(code));
 }
 
 // ------------------------------------------------------------------ one merge
@@ -812,11 +860,7 @@ static pg_status execute(Merge *m) {
         if (!rs) rs = rb.finish();
         if (rs) return rs;
     }
-    if (*m->h_err != KERR_NONE) {
-        return fail(*m->h_err == KERR_TILE_OVERFLOW || *m->h_err == KERR_OFFSET_OVERFLOW ? PG_ERR_INTERNAL
-                                                                                        : PG_ERR_MERGE_FUNCTION,
-                    kernel_error_message(*m->h_err));
-    }
+    if (*m->h_err != KERR_NONE) return kernel_error(*m->h_err, "merge");
 
     // ---- output buffers
     const int64_t n_out = m->h_totals[0];
@@ -916,7 +960,7 @@ static pg_status execute(Merge *m) {
     m->has_batch = true;
     if (*m->h_err != KERR_NONE) {
         free_outputs(m);
-        return fail(PG_ERR_MERGE_FUNCTION, kernel_error_message(*m->h_err));
+        return kernel_error(*m->h_err, "merge");
     }
     for (int c = 0; c < nc; c++)
         if (m->cols[c].width == 0 && m->emit[c]) {

@@ -155,61 +155,32 @@ static bool orc_type_ok(int pg_t, const orc::Type &ty) {
     }
 }
 
-// the tails of the section's device-resident files come back through small reads (readback.cu), so that they do not
-// wait behind another thread's large copies
-struct DeviceRanges : orc::RangeReader {
-    DeviceRanges(cudaStream_t sm, std::vector<const uint8_t *> bytes) : bytes(std::move(bytes)), rb(sm) {}
-    void read(int file, uint64_t off, uint64_t n, uint8_t *dst) override {
-        if (st == PG_OK) st = rb.add(dst, bytes[file] + off, (size_t)n);
-    }
-    void flush() override {
-        if (st == PG_OK) st = rb.finish();
-        if (st != PG_OK) throw std::runtime_error("orc: a read-back of the file tails failed");
-    }
-    std::vector<const uint8_t *> bytes;
-    SmallReads rb;
-    pg_status st = PG_OK;                              // a CUDA error (its message is set)
-};
-
 static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, const pg_file_desc *files, int nf, int n_runs,
                                     const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
                                     pg_section_info *info) {
     const int nc = s->n_cols();
-    cudaStream_t sm = copy_stream();
-    Scratch scratch(sm);                               // file images, tables, scratch and the runs until registered
-    RunBuilder b(s, n_runs, scratch, "orc");
-    SectionTimer tm;
-    PG_CUDA(cudaEventCreate(&tm.e0));
-    PG_CUDA(cudaEventCreate(&tm.e1));
-    PG_CUDA(cudaEventRecord(tm.e0, sm));
-    { pg_status st = b.read_columns(read_cols, names); if (st) return st; }
+    SectionFrame fr(s, n_runs, "orc");
+    RunBuilder &b = fr.b;
+    cudaStream_t sm = fr.stream;
+    { pg_status st = fr.start(read_cols, names); if (st) return st; }
 
-    // ---- file bytes on the device, file tails on the host, column resolution, plans
+    // ---- file tails on the host (those of device-resident files through small reads), column resolution, plans,
+    // file bytes on the device
     std::vector<orc::FileTail> tails(nf);
     std::vector<orc::Plan> plans(nf);
-    std::vector<const uint8_t *> d_file(nf, nullptr);
-    int64_t file_bytes = 0, h2d = 0, page_bytes = 0;
     bool any_compressed = false, any_zstd = false;
     // (a codec or type this decoder does not cover is a refusal, not a malformed file)
     auto parse_error = [](const std::exception &e) {
         const bool refusal = strstr(e.what(), "is not decoded") != nullptr || strstr(e.what(), "not supported") != nullptr;
         return fail(refusal ? PG_ERR_UNSUPPORTED : PG_ERR_FORMAT, e.what());
     };
-    {
-        std::vector<int> dev;                          // the device-resident files: their tails in one batch of reads
-        std::vector<uint64_t> sizes;
-        std::vector<const uint8_t *> bytes;
-        for (int f = 0; f < nf; f++)
-            if (files[f].mem == PG_MEM_DEVICE) { dev.push_back(f); sizes.push_back((uint64_t)files[f].size); bytes.push_back(files[f].bytes); }
-        if (!dev.empty()) {
-            DeviceRanges rd(sm, std::move(bytes));
-            try {
-                std::vector<orc::FileTail> t = orc::read_tails(rd, sizes);
-                for (size_t i = 0; i < dev.size(); i++) tails[dev[i]] = std::move(t[i]);
-            } catch (const std::exception &e) {
-                if (rd.st) return rd.st;
-                return parse_error(e);
-            }
+    DeviceRanges rd(sm, files, nf);
+    if (!rd.files.empty()) {
+        try {
+            std::vector<orc::FileTail> t = orc::read_tails(rd, rd.sizes);
+            for (size_t i = 0; i < rd.files.size(); i++) tails[rd.files[i]] = std::move(t[i]);
+        } catch (const std::exception &e) {
+            return rd.st ? rd.st : parse_error(e);
         }
     }
     for (int f = 0; f < nf; f++) {
@@ -240,13 +211,8 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
         } catch (const std::exception &e) {
             return parse_error(e);
         }
-        file_bytes += files[f].size;
-        if (files[f].mem == PG_MEM_DEVICE) d_file[f] = files[f].bytes;
-        else {
-            { pg_status st = file_image(scratch, files[f].bytes, files[f].size, "orc", &d_file[f]); if (st) return st; }
-            h2d += files[f].size;
-        }
     }
+    { pg_status st = fr.place(files, nf); if (st) return st; }
     { pg_status st = b.check_runs(); if (st) return st; }
 
     // ---- output columns.  ORC columns are nullable by format: every column the read schema calls nullable gets a
@@ -266,19 +232,19 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
     std::vector<int32_t> h_task_out;
     uint64_t dict_entries = 0;
     for (int f = 0; f < nf; f++) dict_entries += plans[f].dict_entries;
-    int32_t *d_dict_off = (int32_t *)scratch.take(4 * (size_t)(dict_entries + 1) + 256);
+    int32_t *d_dict_off = (int32_t *)fr.scratch.take(4 * (size_t)(dict_entries + 1) + 256);
     if (!d_dict_off) return oom("orc", "the dictionary offsets", 4 * (size_t)(dict_entries + 1));
     uint64_t dict_base = 0;
     for (int f = 0; f < nf; f++) {
         const int s0 = (int)h_streams.size();
         for (const orc::PlanStream &ps : plans[f].streams) {
             OrcStream st{};
-            st.src = d_file[f] + ps.offset;
+            st.src = fr.d_file[f] + ps.offset;
             st.length = (int64_t)ps.length;
             st.codec = tails[f].compression;
             st.block_size = (int32_t)tails[f].block_size;
             h_streams.push_back(st);
-            page_bytes += (int64_t)ps.length;
+            fr.page_bytes += (int64_t)ps.length;
         }
         auto idx = [&](int i) { return i < 0 ? -1 : s0 + i; };
         for (const orc::PlanTask &p : plans[f].tasks) {
@@ -310,7 +276,7 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
     const int inflate_ctas = !any_compressed ? std::max(1, std::min(sms, (n_streams + kOrcWarps - 1) / kOrcWarps))
                                                   : std::max(1, std::min(sms * 4, (n_streams + kOrcWarps - 1) / kOrcWarps));
     const size_t tb_lit = any_zstd ? align256((size_t)inflate_ctas * kOrcWarps * (size_t)(zs::kMaxBlock + 64)) : 256;
-    unsigned char *tb = (unsigned char *)scratch.take(tb_s + tb_t + tb_r + tb_o + tb_p + tb_lit + 1024);
+    unsigned char *tb = (unsigned char *)fr.scratch.take(tb_s + tb_t + tb_r + tb_o + tb_p + tb_lit + 1024);
     if (!tb) return oom("orc", "the stream and task tables", tb_s + tb_t + tb_r + tb_o + tb_p + tb_lit);
     OrcStream *d_streams = (OrcStream *)tb;
     orcdev::Task *d_tasks = (orcdev::Task *)(tb + tb_s);
@@ -322,7 +288,6 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
     int32_t *d_counter = d_err + 4;
     int64_t *d_sc_total = (int64_t *)(d_err + 8);
     PG_CUDA(cudaMemsetAsync(d_err, 0, 64, sm));
-    int launches = 0;
     // (tables go through small_h2d: a kernel reads them out of mapped host memory, so they do not queue behind an
     // asynchronous upload of the next section on the copy engine)
     if (n_streams) { pg_status ts = small_h2d(d_streams, h_streams.data(), sizeof(OrcStream) * n_streams, sm); if (ts) return ts; }
@@ -337,7 +302,7 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
     if (any_compressed && n_streams) {
         k_orc_walk<<<(n_streams + 127) / 128, 128, 0, sm>>>(d_streams, n_streams, d_err);
         k_orc_scan<<<1, kOrcScanThreads, 0, sm>>>(d_streams, n_streams, d_sc_total);
-        launches += 2;
+        fr.launches += 2;
         int32_t herr = 0;
         int64_t sc_bytes = 0;
         {
@@ -345,26 +310,25 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
             pg_status rs = rb.add(&herr, d_err, 4);
             if (!rs) rs = rb.add(&sc_bytes, d_sc_total, 8);
             if (!rs) rs = rb.finish();
+            if (!rs) rs = kernel_error(herr, "orc");
             if (rs) return rs;
         }
-        if (herr != KERR_NONE) return fail(PG_ERR_FORMAT, "orc: truncated compression chunk");
-        d_sc = (uint8_t *)scratch.take((size_t)sc_bytes + 256);
+        d_sc = (uint8_t *)fr.scratch.take((size_t)sc_bytes + 256);
         if (!d_sc) return oom("orc", "the stream scratch", (size_t)sc_bytes);
     }
     if (n_streams) {
         k_orc_inflate<<<inflate_ctas, kOrcWarps * 32, 0, sm>>>(d_streams, n_streams, d_sc, d_lit, d_counter, d_err);
-        launches++;
+        fr.launches++;
     }
     if (n_tasks) {
         k_orc_task<0><<<(n_tasks + 31) / 32, 32, 0, sm>>>(d_tasks, d_refs, d_streams, n_tasks, d_err);
-        launches++;
+        fr.launches++;
     }
     // ---- var-len columns: lengths -> offsets, exact payload sizes (one read-back), payload
     std::vector<int32_t> totals(b.out.size(), 0);          // per (run, column)
-    int32_t herr = 0;
     if (std::any_of(b.out.begin(), b.out.end(), [](const OutColumn &o) { return o.offsets != nullptr; })) {
         const int64_t max_n = *std::max_element(b.run_rows.begin(), b.run_rows.end());
-        int64_t *d_sums = (int64_t *)scratch.take(8 * (size_t)(max_n / 4096 + 4));
+        int64_t *d_sums = (int64_t *)fr.scratch.take(8 * (size_t)(max_n / 4096 + 4));
         if (!d_sums) return oom("orc", "the offsets scan", 8 * (size_t)(max_n / 4096 + 4));
         SmallReads rb(sm);                                 // the read-back: exact payload sizes
         for (size_t i = 0; i < b.out.size(); i++) {
@@ -372,14 +336,11 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
             if (!o.offsets) continue;
             const int64_t n = b.run_rows[i / nc];
             launch_offsets_scan(o.offsets, n, d_sums, d_err, sm);
-            launches += n > 0 ? 3 : 0;
+            fr.launches += n > 0 ? 3 : 0;
             { pg_status rs = rb.add(&totals[i], o.offsets + n, 4); if (rs) return rs; }
         }
-        { pg_status rs = rb.add(&herr, d_err, 4); if (!rs) rs = rb.finish(); if (rs) return rs; }
-        if (herr != KERR_NONE)
-            return fail(herr == KERR_OFFSET_OVERFLOW ? PG_ERR_INTERNAL : PG_ERR_FORMAT,
-                        herr == KERR_OFFSET_OVERFLOW ? "orc: a var-len column exceeds 2 GiB of payload"
-                                                     : "orc: a stream does not decode (malformed file or unsupported encoding)");
+        int32_t herr = 0;
+        { pg_status rs = rb.add(&herr, d_err, 4); if (!rs) rs = rb.finish(); if (!rs) rs = kernel_error(herr, "orc"); if (rs) return rs; }
         { pg_status st = b.alloc_payload(std::vector<int64_t>(totals.begin(), totals.end())); if (st) return st; }
         std::vector<uint8_t *> h_payload(b.out.size());   // (k_orc_set_payload reads the var-len entries only)
         for (size_t i = 0; i < b.out.size(); i++) h_payload[i] = (uint8_t *)b.out[i].data;
@@ -387,27 +348,13 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
         if (n_tasks) {
             k_orc_set_payload<<<(n_tasks + 127) / 128, 128, 0, sm>>>(d_tasks, n_tasks, d_task_out, d_payload);
             k_orc_task<1><<<(n_tasks + 31) / 32, 32, 0, sm>>>(d_tasks, d_refs, d_streams, n_tasks, d_err);
-            launches += 2;
+            fr.launches += 2;
         }
     }
-    PG_CUDA(cudaEventRecord(tm.e1, sm));
-    {
-        SmallReads rb(sm);
-        pg_status rs = rb.add(&herr, d_err, 4);
-        if (!rs) rs = rb.finish();
-        if (rs) return rs;
-    }
-    PG_CUDA(cudaGetLastError());
-    if (herr != KERR_NONE) return fail(PG_ERR_FORMAT, "orc: a stream does not decode (malformed file or unsupported encoding)");
-    b.finish(out_runs, h2d, info);
+    { pg_status st = fr.finish(d_err, out_runs, info); if (st) return st; }
     if (info) {
-        info->file_bytes = file_bytes;
-        info->page_bytes = page_bytes;
-        info->n_files = nf;
         info->n_chunks = n_tasks;
         info->n_data_pages = n_streams;
-        info->launches = launches;
-        info->ms_decode = tm.ms();
     }
     return PG_OK;
 }

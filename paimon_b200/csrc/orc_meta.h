@@ -10,7 +10,11 @@
 #include <string>
 #include <vector>
 
+#include "range_reader.h"
+
 namespace orc {
+
+using pg::RangeReader;     // (range_reader.h: shared with the Parquet footer reader)
 
 enum Compression { C_NONE = 0, C_ZLIB = 1, C_SNAPPY = 2, C_LZO = 3, C_LZ4 = 4, C_ZSTD = 5 };
 enum TypeKind { K_BOOLEAN = 0, K_BYTE = 1, K_SHORT = 2, K_INT = 3, K_LONG = 4, K_FLOAT = 5, K_DOUBLE = 6, K_STRING = 7,
@@ -70,13 +74,6 @@ void parse_stripe_footer(FileTail &t, size_t i, const uint8_t *stored);
 
 FileTail parse_file(const uint8_t *file, int64_t size);
 
-// Byte ranges of the files of a section: read() queues the copy of [off, off + n) of file `file` into dst, flush()
-// delivers every queued range (one round trip).
-struct RangeReader {
-    virtual ~RangeReader() = default;
-    virtual void read(int file, uint64_t off, uint64_t n, uint8_t *dst) = 0;
-    virtual void flush() = 0;
-};
 constexpr uint64_t kTailRead = 16384;
 // The tails of files of sizes[f] bytes read through rd in at most three rounds, however many files there are: the
 // last min(size, 16 KiB) bytes and the magic of every file; the rest of the Footers that did not fit; the stripe

@@ -1367,73 +1367,6 @@ static pg_status map_file_schema(RunBuilder &b, const pq::FileMetaData &m, int r
     return PG_OK;
 }
 
-static pg_status kernel_error_status(int code) {
-    switch (code) {
-        case KERR_NONE: return PG_OK;
-        case KERR_PQ_ENCODING:
-            return fail(PG_ERR_UNSUPPORTED, "parquet: a page uses a value encoding the device decoder does not implement "
-                                            "(PLAIN, dictionary, DELTA_BINARY_PACKED integers and RLE booleans are decoded)");
-        case KERR_PQ_LEVELS:
-            return fail(PG_ERR_UNSUPPORTED, "parquet: repetition levels / BIT_PACKED definition levels are not decoded on device");
-        case KERR_PQ_NO_DICT: return fail(PG_ERR_FORMAT, "parquet: dictionary-encoded page without dictionary");
-        case KERR_PQ_ROWS: return fail(PG_ERR_FORMAT, "parquet: page row counts do not add up");
-        case KERR_PQ_HEADER: return fail(PG_ERR_FORMAT, "parquet: malformed or truncated page header");
-        case KERR_PQ_DICT_ID: return fail(PG_ERR_FORMAT, "parquet: dictionary id outside the dictionary");
-        case KERR_OFFSET_OVERFLOW: return fail(PG_ERR_INTERNAL, "parquet: a var-len column exceeds 2 GiB of payload");
-        default: return fail(PG_ERR_FORMAT, "parquet: a page does not expand to its declared size");
-    }
-}
-
-struct SectionFile {
-    const uint8_t *bytes;
-    int64_t size;
-    int mem;                      // PG_MEM_HOST / PG_MEM_DEVICE
-    int run;
-    const pq::FileMetaData *meta; // already parsed (single-file reader), or NULL
-};
-
-// the footers of the files that come without one: device-resident files bring theirs to the host (two small copies per
-// file, two syncs per section), host files are parsed in place
-static pg_status fetch_footers(const std::vector<SectionFile> &files, cudaStream_t sm, std::vector<pq::FileMetaData> &own_meta,
-                               std::vector<const pq::FileMetaData *> &meta) {
-    const int nf = (int)files.size();
-    std::vector<int> need;
-    for (int f = 0; f < nf; f++) {
-        if (files[f].meta) meta[f] = files[f].meta;
-        else if (files[f].mem == PG_MEM_DEVICE) need.push_back(f);
-    }
-    std::vector<uint8_t> tails(8 * need.size() + 8);
-    SmallReads rb(sm);
-    for (size_t i = 0; i < need.size(); i++) {
-        pg_status rs = rb.add(tails.data() + 8 * i, files[need[i]].bytes + files[need[i]].size - 8, 8);
-        if (rs) return rs;
-    }
-    if (!need.empty()) { pg_status rs = rb.finish(); if (rs) return rs; }
-    std::vector<std::vector<uint8_t>> footers(need.size());
-    try {
-        for (size_t i = 0; i < need.size(); i++) {
-            const int64_t flen = pq::footer_length(tails.data() + 8 * i);
-            if (flen + 12 > files[need[i]].size) return fail(PG_ERR_FORMAT, "parquet: bad footer length");
-            footers[i].resize((size_t)flen + 8);
-            pg_status rs = rb.add(footers[i].data(), files[need[i]].bytes + files[need[i]].size - 8 - flen, (size_t)flen);
-            if (rs) return rs;
-        }
-        if (!need.empty()) { pg_status rs = rb.finish(); if (rs) return rs; }
-        for (size_t i = 0; i < need.size(); i++) {
-            own_meta[need[i]] = pq::parse_footer_thrift(footers[i].data(), (int64_t)footers[i].size() - 8);
-            meta[need[i]] = &own_meta[need[i]];
-        }
-        for (int f = 0; f < nf; f++)
-            if (!meta[f]) {
-                own_meta[f] = pq::parse_footer(files[f].bytes, files[f].size);
-                meta[f] = &own_meta[f];
-            }
-    } catch (const std::exception &e) {
-        return fail(PG_ERR_FORMAT, e.what());
-    }
-    return PG_OK;
-}
-
 // the chunk table, ordered (run, column, file, row group) so that the pages of a (run, column) end up contiguous, and
 // the (run, var-len column) pairs
 struct ChunkTables {
@@ -1443,13 +1376,12 @@ struct ChunkTables {
     int64_t pair_rows = 0;
 };
 
-static pg_status build_chunk_tables(const Schema *s, const std::vector<SectionFile> &files,
-                                    const std::vector<const uint8_t *> &d_file, const std::vector<const pq::FileMetaData *> &meta,
-                                    const RunBuilder &b, ChunkTables &t) {
+static pg_status build_chunk_tables(const Schema *s, const pg_file_desc *files, const std::vector<const uint8_t *> &d_file,
+                                    const std::vector<const pq::FileMetaData *> &meta, const RunBuilder &b, ChunkTables &t) {
     const int nc = s->n_cols();
     const int n_runs = (int)b.run_rows.size();
     std::vector<std::vector<int>> run_files(n_runs);
-    for (int f = 0; f < (int)files.size(); f++) run_files[files[f].run].push_back(f);
+    for (int f = 0; f < (int)meta.size(); f++) run_files[files[f].run].push_back(f);
     for (int r = 0; r < n_runs; r++) {
         for (int c = 0; c < nc; c++) {
             if (!b.read[c]) continue;
@@ -1580,37 +1512,35 @@ static pg_status expand_pages(cudaStream_t sm, bool byte_arrays, PqPage *d_pages
     return PG_OK;
 }
 
-static pg_status decode_section(const std::shared_ptr<const Schema> &s, const std::vector<SectionFile> &files,
-                                int n_runs, const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
-                                pg_section_info *info) {
+// footer0: the footer of files[0], already parsed (the single-file reader), or NULL
+static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg_file_desc *files, int nf, int n_runs,
+                                const char *const *names, const uint8_t *read_cols, uint64_t *out_runs,
+                                pg_section_info *info, const pq::FileMetaData *footer0 = nullptr) {
     const int nc = s->n_cols();
-    const int nf = (int)files.size();
-    cudaStream_t sm = copy_stream();
-    Scratch scratch(sm);                               // file images, tables, scratch and the runs until registered
-    RunBuilder b(s, n_runs, scratch, "parquet");
-    int launches = 0;
-    SectionTimer tm;
-    PG_CUDA(cudaEventCreate(&tm.e0));
-    PG_CUDA(cudaEventCreate(&tm.e1));
-    { pg_status st = b.read_columns(read_cols, names); if (st) return st; }
+    SectionFrame fr(s, n_runs, "parquet");
+    RunBuilder &b = fr.b;
+    cudaStream_t sm = fr.stream;
+    { pg_status st = fr.start(read_cols, names); if (st) return st; }
 
-    // ---- file bytes on the device, footers on the host
-    std::vector<const uint8_t *> d_file(nf, nullptr);
+    // ---- file bytes on the device, footers on the host (those of device-resident files through small reads)
+    { pg_status st = fr.place(files, nf); if (st) return st; }
     std::vector<pq::FileMetaData> own_meta(nf);
     std::vector<const pq::FileMetaData *> meta(nf, nullptr);
-    int64_t file_bytes = 0, h2d = 0;
-    PG_CUDA(cudaEventRecord(tm.e0, sm));
-    for (int f = 0; f < nf; f++) {
-        const SectionFile &sf = files[f];
-        if (sf.size < 12) return fail(PG_ERR_FORMAT, "parquet: missing PAR1 magic (encrypted or not a Parquet file)");
-        file_bytes += sf.size;
-        if (sf.mem == PG_MEM_DEVICE) d_file[f] = sf.bytes;
-        else {
-            { pg_status st = file_image(scratch, sf.bytes, sf.size, "parquet", &d_file[f]); if (st) return st; }
-            h2d += sf.size;
+    if (footer0) meta[0] = footer0;
+    DeviceRanges rd(sm, files, nf);
+    try {
+        if (!rd.files.empty()) {
+            std::vector<pq::FileMetaData> m = pq::read_footers(rd, rd.sizes);
+            for (size_t i = 0; i < rd.files.size(); i++) own_meta[rd.files[i]] = std::move(m[i]);
         }
+        for (int f = 0; f < nf; f++) {
+            if (meta[f]) continue;
+            if (files[f].mem == PG_MEM_HOST) own_meta[f] = pq::parse_footer(files[f].bytes, files[f].size);
+            meta[f] = &own_meta[f];
+        }
+    } catch (const std::exception &e) {
+        return rd.st ? rd.st : fail(PG_ERR_FORMAT, e.what());
     }
-    { pg_status st = fetch_footers(files, sm, own_meta, meta); if (st) return st; }
     std::vector<uint8_t> any_optional(nc, 0);
     for (int f = 0; f < nf; f++) {
         pg_status st = map_file_schema(b, *meta[f], files[f].run);
@@ -1622,7 +1552,7 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const st
     }
     { pg_status st = b.check_runs(); if (st) return st; }
     ChunkTables ct;
-    { pg_status st = build_chunk_tables(s.get(), files, d_file, meta, b, ct); if (st) return st; }
+    { pg_status st = build_chunk_tables(s.get(), files, fr.d_file, meta, b, ct); if (st) return st; }
     const int n_chunks = (int)ct.chunks.size(), n_pairs = (int)ct.pairs.size();
 
     // ---- output columns (the rows of files that lack a column stay NULL and get defined contents)
@@ -1642,7 +1572,7 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const st
     const size_t tb_outs = align256(sizeof(PqOut) * outs.size());
     const size_t tb_pairs = align256(sizeof(PqPair) * (size_t)std::max(n_pairs, 1));
     const size_t tb_tot = align256(sizeof(int64_t) * (size_t)(8 + n_pairs));
-    unsigned char *tb = (unsigned char *)scratch.take(tb_chunks + tb_outs + tb_pairs + tb_tot + 256);
+    unsigned char *tb = (unsigned char *)fr.scratch.take(tb_chunks + tb_outs + tb_pairs + tb_tot + 256);
     if (!tb) return oom("parquet", "the chunk tables", tb_chunks + tb_outs + tb_pairs + tb_tot);
     PqChunk *d_chunks = (PqChunk *)tb;
     PqOut *d_outs = (PqOut *)(tb + tb_chunks);
@@ -1659,18 +1589,18 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const st
     if (n_chunks) {
         k_pq_walk<false><<<(n_chunks + 63) / 64, 64, 0, sm>>>(d_chunks, n_chunks, nullptr, nullptr, nullptr, d_err);
         k_pq_chunk_scan<<<1, kScanThreads, 0, sm>>>(d_chunks, n_chunks, d_totals);
-        launches += 2;
+        fr.launches += 2;
         {
             SmallReads rb(sm);                           // read-back 1: how many pages the section has
             pg_status rs = rb.add(h_tot, d_totals, sizeof(int64_t) * 8);
             if (!rs) rs = rb.finish();
+            if (!rs) rs = kernel_error((int)(h_tot[6] & 0xffffffff), "parquet");
             if (rs) return rs;
         }
-        const int herr = (int)(h_tot[6] & 0xffffffff);
-        if (herr != KERR_NONE) return kernel_error_status(herr);
     }
     const int64_t n_pages = h_tot[0], n_dicts = h_tot[1], sc_bytes = h_tot[2], dict_entries = h_tot[3],
-                  ids_entries = h_tot[4], page_bytes = h_tot[5];
+                  ids_entries = h_tot[4];
+    fr.page_bytes = h_tot[5];
     if (n_pages > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet: too many pages in one section");
 
     // ---- page table + scratch, fill pass, inflate
@@ -1688,7 +1618,7 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const st
         zs_ctas = (int)std::min<int64_t>((int64_t)sms * 5, (n_pages + n_dicts + kZsWarps - 1) / kZsWarps);
     }
     const size_t sb_zs = align256((size_t)zs_ctas * kZsWarps * (size_t)(zs::kMaxBlock + 64));
-    unsigned char *sbuf = (unsigned char *)scratch.take(sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs + 256);
+    unsigned char *sbuf = (unsigned char *)fr.scratch.take(sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs + 256);
     if (!sbuf) return oom("parquet", "the page table and scratch", sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs);
     PqPage *d_pages = (PqPage *)sbuf;
     PqPage *d_dicts = (PqPage *)(sbuf + sb_pages);
@@ -1702,40 +1632,39 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const st
     std::vector<int64_t> pair_tot(std::max(n_pairs, 1), 0);
     if (np > 0) {
         k_pq_walk<true><<<(n_chunks + 63) / 64, 64, 0, sm>>>(d_chunks, n_chunks, d_pages, d_dicts, d_sc, d_err);
-        launches++;
+        fr.launches++;
         if (ct.any_snappy || ct.any_lz4) {
             const int64_t th = (int64_t)(np + nd) * 32;
             k_pq_snappy_lz4<<<(unsigned)((th + 127) / 128), 128, 0, sm>>>(d_pages, np, d_dicts, nd, d_chunks, d_err);
-            launches++;
+            fr.launches++;
         }
         if (ct.any_zstd && zs_ctas > 0) {
             k_pq_zstd<<<zs_ctas, kZsWarps * 32, 0, sm>>>(d_pages, np, d_dicts, nd, d_chunks, d_zs_lit, (int32_t *)(d_totals + 7), d_err);
-            launches++;
+            fr.launches++;
         }
         if (ct.any_delta) {
             k_pq_delta<<<(unsigned)(((int64_t)np * 32 + 127) / 128), 128, 0, sm>>>(d_pages, np, d_chunks, d_err);
-            launches++;
+            fr.launches++;
         }
         if (dict_entries > 0) {
             k_pq_walk_dicts<<<(nd + kWalkWarps - 1) / kWalkWarps, kWalkWarps * 32, 0, sm>>>(
                 d_dicts, nd, d_chunks, d_dict_off, d_dict_len, d_err);
-            launches++;
+            fr.launches++;
         }
         k_pq_levels<<<(unsigned)(((int64_t)np * 32 + 127) / 128), 128, 0, sm>>>(d_pages, np, d_dicts, d_chunks, d_outs, nc,
                                                                             d_ids, d_dict_len, d_err);
-        launches++;
+        fr.launches++;
         if (n_pairs) {
             k_pq_scan_pages<<<(n_pairs * 32 + 127) / 128, 128, 0, sm>>>(d_pages, d_chunks, d_pairs, n_pairs, d_totals + 8, d_err);
-            launches++;
+            fr.launches++;
             {
                 SmallReads rb(sm);                       // read-back 2: exact payload sizes of the var-len columns
                 pg_status rs = rb.add(pair_tot.data(), d_totals + 8, sizeof(int64_t) * n_pairs);
                 if (!rs) rs = rb.add(h_tot, d_totals, sizeof(int64_t) * 8);
                 if (!rs) rs = rb.finish();
+                if (!rs) rs = kernel_error((int)(h_tot[6] & 0xffffffff), "parquet");
                 if (rs) return rs;
             }
-            const int herr = (int)(h_tot[6] & 0xffffffff);
-            if (herr != KERR_NONE) return kernel_error_status(herr);
         }
     }
 
@@ -1749,35 +1678,18 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const st
     }
     if (np > 0) {
         pg_status st = expand_pages(sm, n_pairs > 0, d_pages, np, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                    d_dict_len, d_err, &launches);
+                                    d_dict_len, d_err, &fr.launches);
         if (st) return st;
     }
     if (any_empty && n_pairs) {
         k_pq_zero_first_offset<<<(n_runs * nc + 127) / 128, 128, 0, sm>>>(d_outs, n_runs * nc);
-        launches++;
+        fr.launches++;
     }
-    PG_CUDA(cudaEventRecord(tm.e1, sm));
-    {
-        SmallReads rb(sm);
-        pg_status rs = rb.add(h_tot, d_totals, sizeof(int64_t) * 8);
-        if (!rs) rs = rb.finish();
-        if (rs) return rs;
-    }
-    PG_CUDA(cudaGetLastError());
-    {
-        const int herr = (int)(h_tot[6] & 0xffffffff);
-        if (herr != KERR_NONE) return kernel_error_status(herr);
-    }
-    b.finish(out_runs, h2d, info);
+    { pg_status st = fr.finish(d_err, out_runs, info); if (st) return st; }
     if (info) {
-        info->file_bytes = file_bytes;
-        info->page_bytes = page_bytes;
-        info->n_files = nf;
         info->n_chunks = n_chunks;
         info->n_data_pages = np;
         info->n_dictionary_pages = nd;
-        info->launches = launches;
-        info->ms_decode = tm.ms();
     }
     return PG_OK;
 }
@@ -1813,12 +1725,12 @@ static pg_status pq_open(uint64_t schema, const uint8_t *bytes, int64_t size, ui
     pg_status st = map_file_schema(b, rd->meta, 0);
     if (st) return st;
     // the chunk table and the count pass of the section decode, over the host bytes
-    const std::vector<SectionFile> files{SectionFile{bytes, size, PG_MEM_HOST, 0, &rd->meta}};
+    const pg_file_desc file{bytes, size, PG_MEM_HOST, 0};
     ChunkTables ct;
-    st = build_chunk_tables(s.get(), files, {bytes}, {&rd->meta}, b, ct);
+    st = build_chunk_tables(s.get(), &file, {bytes}, {&rd->meta}, b, ct);
     if (st) return st;
     for (int c = 0; c < (int)ct.chunks.size(); c++) {
-        st = kernel_error_status(pq_walk_chunk<false>(ct.chunks.data(), c, nullptr, nullptr, nullptr));
+        st = kernel_error(pq_walk_chunk<false>(ct.chunks.data(), c, nullptr, nullptr, nullptr), "parquet");
         if (st) return st;
         rd->n_data_pages += ct.chunks[c].n_pages;
         rd->n_dict_pages += ct.chunks[c].n_dicts;
@@ -1830,9 +1742,9 @@ static pg_status pq_open(uint64_t schema, const uint8_t *bytes, int64_t size, ui
 }
 
 static pg_status pq_read_run(PqReader *rd, uint64_t *out_run) {
-    std::vector<SectionFile> files{SectionFile{rd->file.data(), (int64_t)rd->file.size(), PG_MEM_HOST, 0, &rd->meta}};
+    const pg_file_desc file{rd->file.data(), (int64_t)rd->file.size(), PG_MEM_HOST, 0};
     pg_section_info info;
-    pg_status st = decode_section(rd->schema, files, 1, nullptr, nullptr, out_run, &info);
+    pg_status st = decode_section(rd->schema, &file, 1, 1, nullptr, nullptr, out_run, &info, &rd->meta);
     if (st) return st;
     rd->ms_decode = info.ms_decode;
     rd->launches = info.launches;
@@ -1955,7 +1867,8 @@ static pg_status apply_deletion_vector(uint64_t run_h, const uint8_t *deleted, i
                                                                         d_src, b.out[c].offsets, (uint8_t *)b.out[c].data, m);
     PG_CUDA(cudaStreamSynchronize(sm));
     PG_CUDA(cudaGetLastError());
-    if (herr != KERR_NONE) return fail(PG_ERR_INTERNAL, "deletion vector: a var-len column exceeds 2 GiB of payload");
+    st = kernel_error(herr, "deletion vector");
+    if (st) return st;
     b.finish(out_run, 0, nullptr);
     return PG_OK;
 }
@@ -2000,9 +1913,7 @@ pg_status pg_parquet_read_section(uint64_t schema, const pg_file_desc *files, in
     if (st || n_runs == 0) return st;
     st = ensure_device();
     if (st) return st;
-    std::vector<SectionFile> fs(n_files);
-    for (int i = 0; i < n_files; i++) fs[i] = SectionFile{files[i].bytes, files[i].size, files[i].mem, files[i].run, nullptr};
-    return decode_section(s, fs, n_runs, column_names, read_columns, out_runs, info);
+    return decode_section(s, files, n_files, n_runs, column_names, read_columns, out_runs, info);
 }
 
 pg_status pg_run_apply_deletion_vector(uint64_t run, const uint8_t *deleted_bitmap, int64_t n_bits, uint64_t *out_run) {

@@ -175,8 +175,6 @@ RowGroup read_row_group(Reader &r) {
     return g;
 }
 
-}  // namespace
-
 FileMetaData parse_footer_thrift(const uint8_t *footer, int64_t flen) {
     Reader r(footer, flen);
     FileMetaData m;
@@ -211,12 +209,35 @@ int64_t footer_length(const uint8_t *tail8) {
     return (int64_t)((uint32_t)tail8[0] | ((uint32_t)tail8[1] << 8) | ((uint32_t)tail8[2] << 16) | ((uint32_t)tail8[3] << 24));
 }
 
+}  // namespace
+
 FileMetaData parse_footer(const uint8_t *file, int64_t size) {
     if (size < 12 || file[0] != 'P' || file[1] != 'A' || file[2] != 'R' || file[3] != '1')
         throw std::runtime_error("parquet: missing PAR1 magic (encrypted or not a Parquet file)");
     const int64_t flen = footer_length(file + size - 8);
     if (flen + 12 > size) throw std::runtime_error("parquet: bad footer length");
     return parse_footer_thrift(file + size - 8 - flen, flen);
+}
+
+std::vector<FileMetaData> read_footers(RangeReader &rd, const std::vector<uint64_t> &sizes) {
+    const size_t nf = sizes.size();
+    std::vector<uint8_t> tails(8 * nf);
+    for (size_t f = 0; f < nf; f++) {
+        if (sizes[f] < 12) throw std::runtime_error("parquet: missing PAR1 magic (encrypted or not a Parquet file)");
+        rd.read((int)f, sizes[f] - 8, 8, &tails[8 * f]);
+    }
+    rd.flush();
+    std::vector<std::vector<uint8_t>> footers(nf);
+    for (size_t f = 0; f < nf; f++) {
+        const int64_t flen = footer_length(&tails[8 * f]);
+        if ((uint64_t)flen + 12 > sizes[f]) throw std::runtime_error("parquet: bad footer length");
+        footers[f].resize((size_t)flen);
+        rd.read((int)f, sizes[f] - 8 - (uint64_t)flen, (uint64_t)flen, footers[f].data());
+    }
+    rd.flush();
+    std::vector<FileMetaData> m(nf);
+    for (size_t f = 0; f < nf; f++) m[f] = parse_footer_thrift(footers[f].data(), (int64_t)footers[f].size());
+    return m;
 }
 
 }  // namespace pq

@@ -11,7 +11,11 @@
 #include <string>
 #include <vector>
 
+#include "range_reader.h"
+
 namespace pq {
+
+using pg::RangeReader;     // (range_reader.h: shared with the ORC tail reader)
 
 enum PhysType { T_BOOLEAN = 0, T_INT32 = 1, T_INT64 = 2, T_INT96 = 3, T_FLOAT = 4, T_DOUBLE = 5, T_BYTE_ARRAY = 6,
                 T_FIXED_LEN_BYTE_ARRAY = 7 };
@@ -63,12 +67,13 @@ struct FileMetaData {
     std::string created_by;
 };
 
-// Throws std::runtime_error on malformed input.
+// Both throw std::runtime_error on malformed input.
+// A file in host memory, whole.
 FileMetaData parse_footer(const uint8_t *file, int64_t size);
-// the pieces of parse_footer, for files whose bytes live on the device: the last 8 bytes of the file
-// ([footer length:4 LE]["PAR1"]) -> footer length; the Thrift FileMetaData bytes in front of them -> metadata
-int64_t footer_length(const uint8_t *tail8);
-FileMetaData parse_footer_thrift(const uint8_t *footer, int64_t flen);
+// The footers of files of sizes[f] bytes whose bytes are elsewhere (device memory), read through rd in two rounds:
+// the last 8 bytes of every file ([footer length:4 LE]["PAR1"]), then every footer.  No range is queued before it is
+// checked against its file.  Unlike parse_footer, the leading "PAR1" is not read.
+std::vector<FileMetaData> read_footers(RangeReader &rd, const std::vector<uint64_t> &sizes);
 
 inline void put_varint(std::vector<uint8_t> &b, uint64_t v) {
     while (v >= 0x80) { b.push_back((uint8_t)(v | 0x80)); v >>= 7; }

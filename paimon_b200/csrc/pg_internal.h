@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "paimon_gpu.h"
+#include "range_reader.h"
 
 namespace pg {
 
@@ -31,7 +32,7 @@ constexpr uint16_t kPlanEmit = 0x4000;
 constexpr uint16_t kPlanHead = 0x8000;
 enum : int { OP_NOOP = 0, OP_UPD = 1, OP_SET = 2, OP_RETRACT = 3 };
 
-// error codes raised by kernels (first one wins), decoded in api.cu
+// error codes raised by kernels (first one wins); kernel_error turns them into statuses
 enum : int {
     KERR_NONE = 0,
     KERR_TILE_OVERFLOW = 1,          // internal: a tile exceeded kTileMax (duplicate keys inside a run?)
@@ -232,6 +233,29 @@ struct SectionTimer {
     }
 };
 
+// The host frame of one section decode (api.cu), shared by the Parquet and ORC decoders: the calling thread's copy
+// stream, the call's Scratch and RunBuilder, the ms_decode events, the launch count and the section's files on the
+// device.  The format decoder builds its tables and launches its kernels between start() and finish().
+struct SectionFrame {
+    SectionFrame(std::shared_ptr<const Schema> s, int n_runs, const char *who);
+    // records the first event of ms_decode, then RunBuilder::read_columns
+    pg_status start(const uint8_t *read_cols, const char *const *names);
+    // d_file[f]: the bytes of file f on the device, a copy (file_image) of a host file, a device file in place
+    pg_status place(const pg_file_desc *files, int n_files);
+    // after the last launch: records the second event, reads the error word d_err back (one SmallReads) and turns it
+    // into a status, registers the runs, and fills *info (if any) but for the format's own counts: n_chunks,
+    // n_data_pages and n_dictionary_pages
+    pg_status finish(const int32_t *d_err, uint64_t *out_runs, pg_section_info *info);
+
+    const cudaStream_t stream;
+    Scratch scratch;                 // file images, tables, scratch and the runs until registered
+    RunBuilder b;
+    SectionTimer tm;
+    int launches = 0;
+    std::vector<const uint8_t *> d_file;
+    int64_t file_bytes = 0, h2d = 0, page_bytes = 0;     // (page_bytes: set by the format decoder)
+};
+
 // ---- handle tables: one per handle kind.  A handle carries its kind's tag in the top byte (1 schema, 2 merge spec,
 // 3 run, 4 merge; 5 Parquet reader, 6 encoded Parquet or ORC file, 7 upload), so a handle of one kind is never found by
 // another kind's entry points.
@@ -339,6 +363,10 @@ inline bool is_varlen(int t) { return t == PG_STRING || t == PG_BINARY; }
 
 void set_error(const std::string &msg);
 pg_status fail(pg_status code, const std::string &msg);
+// The status of a kernel error word (api.cu): PG_OK for KERR_NONE.  What a merge function raises is
+// PG_ERR_MERGE_FUNCTION with the message Java throws; the rest is a format, unsupported or internal status with a
+// message behind "<who>: ".
+pg_status kernel_error(int code, const char *who);
 
 #define PG_CUDA(expr)                                                                      \
     do {                                                                                   \
@@ -466,6 +494,20 @@ class SmallReads {
     cudaStream_t stream_;
     std::vector<Item> items_;
     size_t used_ = 0;
+};
+
+// The byte ranges of the device-resident files of a section through SmallReads (orc::read_tails, pq::read_footers).
+// files[i] is the index in the section of the i-th device-resident file, sizes[i] its size.  flush() throws when a
+// read-back fails; st then holds its status (the message is set).
+struct DeviceRanges : RangeReader {
+    DeviceRanges(cudaStream_t s, const pg_file_desc *section, int n_files);
+    void read(int file, uint64_t off, uint64_t n, uint8_t *dst) override;
+    void flush() override;
+    const pg_file_desc *section;
+    std::vector<int> files;
+    std::vector<uint64_t> sizes;
+    SmallReads rb;
+    pg_status st = PG_OK;
 };
 
 }  // namespace pg

@@ -8,6 +8,7 @@
 // device-mapped host memory instead; the host reads them after synchronising the stream.
 #include <algorithm>
 #include <cstring>
+#include <stdexcept>
 #include <utility>
 #include <vector>
 
@@ -107,6 +108,20 @@ pg_status SmallReads::finish() {
     items_.clear();
     used_ = 0;
     return PG_OK;
+}
+
+DeviceRanges::DeviceRanges(cudaStream_t s, const pg_file_desc *section, int n_files) : section(section), rb(s) {
+    for (int f = 0; f < n_files; f++)
+        if (section[f].mem == PG_MEM_DEVICE) { files.push_back(f); sizes.push_back((uint64_t)section[f].size); }
+}
+
+void DeviceRanges::read(int file, uint64_t off, uint64_t n, uint8_t *dst) {
+    if (st == PG_OK) st = rb.add(dst, section[files[file]].bytes + off, (size_t)n);
+}
+
+void DeviceRanges::flush() {
+    if (st == PG_OK) st = rb.finish();
+    if (st != PG_OK) throw std::runtime_error("a read-back of the file metadata failed");
 }
 
 }  // namespace pg

@@ -5,10 +5,10 @@ NVFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Iinclude -Ipaimon_
 SRCS := paimon_b200/csrc/merge.cu paimon_b200/csrc/emit.cu paimon_b200/csrc/api.cu \
 	paimon_b200/csrc/parquet_decode.cu paimon_b200/csrc/parquet_encode.cu paimon_b200/csrc/parquet_meta.cc \
 	paimon_b200/csrc/arrow_export.cu paimon_b200/csrc/upload.cu paimon_b200/csrc/readback.cu paimon_b200/csrc/orc_decode.cu paimon_b200/csrc/orc_meta.cc \
-	paimon_b200/csrc/orc_encode.cu paimon_b200/csrc/encoded_file.cu
+	paimon_b200/csrc/orc_encode.cu paimon_b200/csrc/encoded_file.cu paimon_b200/csrc/file_index.cu
 HDRS := include/paimon_gpu.h paimon_b200/csrc/pg_internal.h paimon_b200/csrc/device_utils.cuh paimon_b200/csrc/parquet_meta.h \
 	paimon_b200/csrc/zstd_device.cuh paimon_b200/csrc/zstd_encode_device.cuh paimon_b200/csrc/inflate_device.cuh paimon_b200/csrc/lz4_device.cuh paimon_b200/csrc/snappy_device.cuh paimon_b200/csrc/orc_device.cuh paimon_b200/csrc/orc_meta.h \
-	paimon_b200/csrc/orc_encode_device.cuh paimon_b200/csrc/encoded_file.h \
+	paimon_b200/csrc/orc_encode_device.cuh paimon_b200/csrc/encoded_file.h paimon_b200/csrc/xxhash64_device.cuh \
 	paimon_b200/csrc/scan_kernels.cuh paimon_b200/csrc/range_reader.h
 LIB := paimon_b200/libpaimon_gpu.so
 
@@ -28,6 +28,7 @@ $(LIB): $(OBJS)
 
 ptxas-info: $(SRCS) $(HDRS)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c -o /dev/null paimon_b200/csrc/merge.cu
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c -o /dev/null paimon_b200/csrc/file_index.cu
 
 # the JNI shim against the JNI specification's signatures (no JDK in the image: jni/stub/jni.h)
 jni-check:

@@ -463,6 +463,37 @@ typedef struct {
 pg_status pg_orc_encode(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
                         const pg_orc_write_options *options, uint64_t *out_file);
 
+/* ---- compaction output: the bloom-filter file index of a data file ----------------------------------------
+ * What KeyValueDataFileWriter builds row by row for a table with 'file-index.bloom-filter.columns'
+ * (paimon-core/.../io/KeyValueDataFileWriter.java:103-113, DataFileIndexWriter.java): one BloomFilter64 per indexed
+ * value column over the rows of the file (paimon-common/.../fileindex/bloomfilter/BloomFilterFileIndex.java,
+ * utils/BloomFilter64.java).  `source`, `row0` (a multiple of 8) and `n_rows` (< 0 = to the end) mean what they mean for
+ * pg_parquet_encode, so the index of a file covers exactly the rows of that file.  Per spec, NULLs are skipped and every
+ * other value is hashed by its physical type as FastHash does: integers sign-extended, FLOAT / DOUBLE by their bits with
+ * NaN folded to the canonical NaN, all through Thomas Wang's 64-bit hash; STRING / BINARY by XXH64 (seed 0) of their
+ * bytes.  DATE / TIME and TIMESTAMP hash the stored INT32 / INT64 (a TIMESTAMP(p <= 3) column holds epoch millis, as
+ * Parquet's TIMESTAMP_MILLIS does, a TIMESTAMP(4..6) one epoch micros: what FastHash hashes for each).  DECIMAL columns are
+ * INT64 here too, and the caller must refuse them ("Does not support decimal"), as BloomFilterFileIndex does.
+ * host_out[i] receives the serialized filter of specs[i] (BloomFilterFileIndex.Writer.serializedBytes: the hash
+ * function count as a big-endian int32, then the numBits / 8 bytes of the bit set, bit p in byte p >> 3 at bit p & 7);
+ * capacity[i] is checked against pg_bloom_filter_size.  The bytes of every column go into the FileIndexFormat container
+ * by the caller (see INTEGRATION.md).
+ * A BOOLEAN column returns PG_ERR_UNSUPPORTED; a column outside the schema, items <= 0, fpp outside (0, 1), a bit set
+ * of 2^31 bits or more, a too small capacity and a row range outside the batch or not starting at a multiple of 8 return
+ * PG_ERR_INVALID. */
+typedef struct {
+    int32_t column;      /* file column index (value field v is n_key + 2 + v) */
+    int32_t items;       /* 'file-index.bloom-filter.<column>.items' (BloomFilterFileIndex default 1000000) */
+    double fpp;          /* 'file-index.bloom-filter.<column>.fpp' (default 0.1) */
+} pg_bloom_filter_spec;
+
+/* Host only, no device needed: the serialized size (4 + numBits / 8) and hash function count of a filter, sized as
+ * BloomFilter64(items, fpp) does: nb = (int)(-items ln fpp / (ln 2)^2), numBits = nb + 8 - nb % 8,
+ * k = max(1, round(numBits / items ln 2)).  The same PG_ERR_INVALID cases as pg_bloom_filter_build. */
+pg_status pg_bloom_filter_size(int32_t items, double fpp, int64_t *bytes, int32_t *num_hash_functions);
+pg_status pg_bloom_filter_build(uint64_t source, int64_t row0, int64_t n_rows, int32_t n,
+                                const pg_bloom_filter_spec *specs, uint8_t *const *host_out, const int64_t *capacity);
+
 /* IntervalPartition over int64 (min,max) key bounds of data files: section and run id per file */
 pg_status pg_interval_partition(int32_t n_files, const int64_t *min_key, const int64_t *max_key,
                                 int32_t *section_of, int32_t *run_of, int32_t *n_sections);

@@ -605,6 +605,49 @@ JNIEXPORT jlongArray JNICALL Java_org_apache_paimon_gpu_NativeMerge_fileColumnSt
     return out;
 }
 
+// BloomFilter64(items, fpp) sizing: long[2] = {serialized bytes, hash function count}; the Java side allocates a
+// direct ByteBuffer of that many bytes per indexed column for bloomFilterBuild
+JNIEXPORT jlongArray JNICALL Java_org_apache_paimon_gpu_NativeMerge_bloomFilterSize(JNIEnv *env, jclass, jint items,
+                                                                                    jdouble fpp) {
+    int64_t bytes = 0;
+    int32_t k = 0;
+    pg_status rc = pg_bloom_filter_size(items, fpp, &bytes, &k);
+    if (rc != PG_OK) { throw_for(env, rc); return nullptr; }
+    jlong v[2] = {bytes, k};
+    jlongArray out = env->NewLongArray(2);
+    env->SetLongArrayRegion(out, 0, 2, v);
+    return out;
+}
+
+// the serialized bloom filter of each (column, items, fpp) over rows [row0, row0 + nRows) of a merge or run handle,
+// into out[i] (direct ByteBuffers): the per-column bytes DataFileIndexWriter hands to FileIndexFormat.Writer
+JNIEXPORT jint JNICALL Java_org_apache_paimon_gpu_NativeMerge_bloomFilterBuild(JNIEnv *env, jclass, jlong source,
+                                                                              jlong row0, jlong nRows, jintArray columns,
+                                                                              jintArray items, jdoubleArray fpp,
+                                                                              jobjectArray out) {
+    const jsize n = env->GetArrayLength(columns);
+    if (env->GetArrayLength(items) != n || env->GetArrayLength(fpp) != n || env->GetArrayLength(out) != n) {
+        env->ThrowNew(env->FindClass("java/lang/IllegalArgumentException"), "bloomFilterBuild: array lengths differ");
+        return 0;
+    }
+    std::vector<jint> c((size_t)n), it((size_t)n);
+    std::vector<jdouble> f((size_t)n);
+    env->GetIntArrayRegion(columns, 0, n, c.data());
+    env->GetIntArrayRegion(items, 0, n, it.data());
+    env->GetDoubleArrayRegion(fpp, 0, n, f.data());
+    std::vector<pg_bloom_filter_spec> specs((size_t)n);
+    std::vector<uint8_t *> dst((size_t)n);
+    std::vector<int64_t> cap((size_t)n);
+    for (jsize i = 0; i < n; i++) {
+        specs[i] = pg_bloom_filter_spec{c[i], it[i], f[i]};
+        jobject buf = env->GetObjectArrayElement(out, i);
+        dst[i] = (uint8_t *)env->GetDirectBufferAddress(buf);
+        cap[i] = env->GetDirectBufferCapacity(buf);
+    }
+    PG_CHECK(pg_bloom_filter_build((uint64_t)source, row0, nRows, n, specs.data(), dst.data(), cap.data()));
+    return 0;
+}
+
 // IntervalPartition.partition over (min, max) key bounds: int[2 * n + 1] = {sections, section of file i, run of file i}
 JNIEXPORT jintArray JNICALL Java_org_apache_paimon_gpu_NativeMerge_intervalPartition(JNIEnv *env, jclass, jlongArray minKey,
                                                                                      jlongArray maxKey) {

@@ -40,6 +40,7 @@ struct JNIEnv {
     jintArray NewIntArray(jsize len);
     jdoubleArray NewDoubleArray(jsize len);
     void SetDoubleArrayRegion(jdoubleArray array, jsize start, jsize len, const jdouble *buf);
+    void GetDoubleArrayRegion(jdoubleArray array, jsize start, jsize len, jdouble *buf);
     void *GetDirectBufferAddress(jobject buf);
     jlong GetDirectBufferCapacity(jobject buf);
     const char *GetStringUTFChars(jstring str, jboolean *isCopy);

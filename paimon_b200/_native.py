@@ -96,6 +96,10 @@ class PgOrcWriteOptions(C.Structure):
                 ("compression_block_size", C.c_int64), ("types", C.POINTER(PgOrcColumnType))]
 
 
+class PgBloomFilterSpec(C.Structure):
+    _fields_ = [("column", C.c_int32), ("items", C.c_int32), ("fpp", C.c_double)]
+
+
 class PaimonGpuError(RuntimeError):
     """A non-zero pg_status.  `.status` holds the code (PG_ERR_*)."""
 
@@ -169,6 +173,9 @@ _SIGNATURES = {
                                                  C.c_void_p, C.c_void_p]),
     "pg_parquet_file_fetch": (C.c_int32, [C.c_uint64, C.c_void_p, C.c_int64]),
     "pg_parquet_file_free": (C.c_int32, [C.c_uint64]),
+    "pg_bloom_filter_size": (C.c_int32, [C.c_int32, C.c_double, C.POINTER(C.c_int64), C.POINTER(C.c_int32)]),
+    "pg_bloom_filter_build": (C.c_int32, [C.c_uint64, C.c_int64, C.c_int64, C.c_int32, C.POINTER(PgBloomFilterSpec),
+                                          C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
 }
 
 _lib: Optional[C.CDLL] = None

@@ -19,6 +19,7 @@ from typing import Dict, List, Optional, Sequence, Tuple
 import numpy as np
 
 from . import _native as N
+from .file_index import DataFileIndexWriter, FileIndexOptions
 from .format import LocalFileIO
 from .merge_function import MergeFunctionFactory
 from .merge_tree_readers import (DataFileMeta, IntervalPartition, KeyValueFileReaderFactory, MergeTreeReaders,
@@ -112,11 +113,16 @@ class KeyValueDataFileWriter:
     one data file of `file_format` ('parquet' or 'orc') and returns its DataFileMeta.  `compression` names the codec
     ('none' or 'zstd', compressed on the device; the library refuses the others), `zstd_level` is
     file.compression.zstd-level.  Parquet takes `row_group_rows` / `page_rows`, ORC `stripe_rows` /
-    `compression_block_size` and writes the logical types of the schema (OrcTypeUtil.convertToOrcType)."""
+    `compression_block_size` and writes the logical types of the schema (OrcTypeUtil.convertToOrcType).  With
+    `file_index` (the table's 'file-index.*' options) the file gets the bloom filters of its value columns, built on
+    the device over the rows of the file, as DataFileMeta.embedded_index or the side file of extra_files
+    (KeyValueDataFileWriter.java:103-113,156-181); options the device cannot build are refused here, before any
+    device work."""
 
     def __init__(self, schema: KeyValueSchema, path: str, level: int, file_io: Optional[LocalFileIO] = None,
                  row_group_rows: int = 0, page_rows: int = 0, compression: str = "none", zstd_level: int = 1,
-                 file_format: str = "parquet", stripe_rows: int = 0, compression_block_size: int = 0):
+                 file_format: str = "parquet", stripe_rows: int = 0, compression_block_size: int = 0,
+                 file_index: Optional[FileIndexOptions] = None):
         self.schema = schema
         self.path = path
         self.level = level
@@ -136,6 +142,9 @@ class KeyValueDataFileWriter:
                                                                    for f in fields])
             self.orc_opts = N.PgOrcWriteOptions(stripe_rows, self.codec, self.zstd_level, compression_block_size,
                                                 self._orc_types)
+        self.index_writer = None
+        if file_index is not None and not file_index.is_empty():
+            self.index_writer = DataFileIndexWriter(schema, file_index)
         self.lib = N.load()
 
     def write(self, source_handle: int, row0: int = 0, n_rows: int = -1) -> WrittenFile:
@@ -172,6 +181,9 @@ class KeyValueDataFileWriter:
                            min_sequence_number=int(meta.min_sequence_number),
                            max_sequence_number=int(meta.max_sequence_number), level=self.level,
                            delete_row_count=int(meta.delete_row_count))
+        if self.index_writer is not None:
+            index = self.index_writer.write(self.file_io, self.path, source_handle, row0, n_file)
+            dfm.embedded_index, dfm.extra_files = index.embedded_index, index.extra_files
         return WrittenFile(dfm, stats[self.schema.n_key + 2:], float(meta.ms_encode), int(meta.n_pages))
 
     def _key_row(self, source_handle: int, row: int):
@@ -229,8 +241,9 @@ class MergeTreeCompactRewriter:
     """rewriteCompaction(outputLevel, dropDelete, sections): every section is merged on the device, the merged
     batch never leaves HBM before it is encoded (MergeTreeCompactRewriter.java:78-116).  With `options` (table
     options), the files written at the output level take the format format_for_level(options, level) and, for
-    parquet, the codec compression_for_level(options, level), for orc orc_compression_for_level(options, level);
-    without, they are uncompressed Parquet (or the writer arguments' file_format)."""
+    parquet, the codec compression_for_level(options, level), for orc orc_compression_for_level(options, level),
+    and the 'file-index.*' options give every file its bloom filters (refused before any device work when the device
+    cannot build them); without, they are uncompressed Parquet (or the writer arguments' file_format)."""
 
     def __init__(self, schema: KeyValueSchema, mf_factory: MergeFunctionFactory, directory: str,
                  user_defined_seq_comparator=None, file_io: Optional[LocalFileIO] = None, device: int = 0,
@@ -265,6 +278,10 @@ class MergeTreeCompactRewriter:
                  writer_args["compression_block_size"]) = orc_compression_for_level(self.options, output_level)
             else:
                 writer_args["compression"], writer_args["zstd_level"] = compression_for_level(self.options, output_level)
+            file_index = FileIndexOptions.from_options(self.options)
+            if not file_index.is_empty():
+                DataFileIndexWriter(self.schema, file_index)          # refuses before any device work
+                writer_args["file_index"] = file_index
         rolling = RollingFileWriter(self.schema, self.directory, output_level, self.target_file_rows, self.file_io,
                                     prefix=f"compact-l{output_level}", **writer_args)
         for section in sections:

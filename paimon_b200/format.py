@@ -39,6 +39,10 @@ class LocalFileIO:
         import os
         return os.path.getsize(path)
 
+    def write_bytes(self, path: str, data: bytes) -> None:
+        with open(path, "wb") as f:
+            f.write(data)
+
 
 @dataclass
 class FormatReaderContext:

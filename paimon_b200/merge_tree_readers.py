@@ -42,6 +42,8 @@ class DataFileMeta:
     max_sequence_number: int = 0
     level: int = 0
     delete_row_count: int = 0
+    embedded_index: Optional[bytes] = None     # the file index when it is small enough for the manifest
+    extra_files: List[str] = field(default_factory=list)   # else its side file '<file_name>.index'
 
 
 def comparable_key(k):

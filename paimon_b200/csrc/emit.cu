@@ -648,6 +648,9 @@ k_emit(EmitArgs ea) {
             int *wpre = (int *)(vsrc + kTileMax);                                   // per warp: 33 ints
             const uint8_t **wsrc = (const uint8_t **)(wpre + ((kEmitWarps * 33 + 1) & ~1));   // 8-byte aligned
             int *wend = (int *)(wsrc + kEmitWarps * 32);                             // per warp: 32 ints
+            int64_t *wtot = (int64_t *)(wend + kEmitWarps * 32);                     // per warp: its byte total
+            static_assert(kTileMax * 2 + ((kEmitWarps * 33 + 1) & ~1) * 4 + kEmitWarps * 32 * (8 + 4) + kEmitWarps * 8 <=
+                              (kTileMax + 64) * 4, "var-len scratch fits the upper half of a stage at k = 1");
             const uint8_t *const *cd_data = cdata + s * PG_MAX_RUNS;
             // Rows are dealt to warps in contiguous chunks of RW rows (RW a multiple of 32, aligned to the
             // output's 32-row validity words), so that offsets come from warp-level scans and the only
@@ -655,8 +658,9 @@ k_emit(EmitArgs ea) {
             const int span = tv.o_shift + n_out;
             const int RW = (((span + kEmitWarps - 1) / kEmitWarps) + 31) & ~31;
             const int wbeg = -tv.o_shift + warp * RW;
-            // pass 1: source member per output row, byte total of this warp's rows
-            int my_bytes = 0;
+            // pass 1: source member per output row, byte total of this warp's rows.  Every value is below 2 GiB,
+            // but a warp's or a tile's rows together need not be: the totals are 64-bit.
+            int64_t my_bytes = 0;
             for (int ob0 = wbeg; ob0 < wbeg + RW && ob0 < n_out; ob0 += 32) {
                 const int ob = ob0 + lane;
                 if (ob >= 0 && ob < n_out) {
@@ -675,16 +679,22 @@ k_emit(EmitArgs ea) {
             }
 #pragma unroll
             for (int d = 16; d > 0; d >>= 1) my_bytes += __shfl_xor_sync(0xffffffffu, my_bytes, d);
-            if (lane == 0) ws[warp] = my_bytes;
+            if (lane == 0) wtot[warp] = my_bytes;
             __syncthreads();
             if (ci < 60) TS(8 + 4 * ci + 0);
             // warp 0: exclusive scan of the 16 warp totals + decoupled look-back over earlier tiles
             uint64_t *state = ea.vl_state + (int64_t)cd.varlen_index * ea.n_tiles;
             if (warp == 0) {
-                int x = lane < kEmitWarps ? ws[lane] : 0;
-                int xi = warp_scan_incl(x);
-                const int tile_bytes = __shfl_sync(0xffffffffu, xi, 31);
-                if (lane < kEmitWarps) ws[lane] = xi - x;
+                const int64_t x = lane < kEmitWarps ? wtot[lane] : 0;
+                int64_t xi = x;
+#pragma unroll
+                for (int d = 1; d < kEmitWarps; d <<= 1) {
+                    const int64_t y = __shfl_up_sync(0xffffffffu, xi, d);
+                    if (lane >= d) xi += y;
+                }
+                const uint64_t tile_bytes = (uint64_t)__shfl_sync(0xffffffffu, xi, kEmitWarps - 1);
+                // (only read by pass 2, which runs only when the tile ends below 2 GiB: then these fit in int)
+                if (lane < kEmitWarps) ws[lane] = (int)(xi - x);
                 uint64_t excl = 0;
                 if (lane == 0 && tile > 0) {
                     __threadfence();
@@ -727,26 +737,33 @@ k_emit(EmitArgs ea) {
                 }
                 if (lane == 0) {
                     __threadfence();
-                    atomicExch((unsigned long long *)&state[tile], kFlagPrefix | (excl + (uint64_t)tile_bytes));
-                    s_i64[0] = (int64_t)excl;
+                    const uint64_t tot = excl + tile_bytes;
+                    atomicExch((unsigned long long *)&state[tile], kFlagPrefix | tot);
+                    // Offsets are int32: a tile that ends past 2 GiB refuses the batch and stores nothing (its
+                    // payload could lie past the buffer, its in-tile offsets past int).  Its prefix is published
+                    // all the same, so every later tile sees the overflow too.
+                    const bool fits = tot <= 0x7fffffffull;
+                    if (!fits) atomicCAS(ea.err, KERR_NONE, KERR_OFFSET_OVERFLOW);
+                    s_i64[0] = fits ? (int64_t)excl : -1;
                     if (tile == ea.n_tiles - 1) {
-                        uint64_t tot = excl + (uint64_t)tile_bytes;
                         ea.totals[1 + cd.varlen_index] = (int64_t)tot;
-                        if (tot > 0x7fffffffull) atomicCAS(ea.err, KERR_NONE, KERR_OFFSET_OVERFLOW);
-                        oc.offsets[ea.totals[0]] = (int32_t)tot;
+                        if (fits) oc.offsets[ea.totals[0]] = (int32_t)tot;
                     }
                 }
             }
             __syncthreads();
             if (ci < 60) TS(8 + 4 * ci + 1);
             const int64_t byte_base = s_i64[0];
-            uint8_t *dbase = (uint8_t *)oc.data + byte_base;
-            // pass 2: offsets, validity, payload copy — warp-local
+            uint8_t *dbase = (uint8_t *)oc.data + (byte_base < 0 ? 0 : byte_base);
+            // pass 2: offsets, validity, payload copy — warp-local.  Byte positions inside the tile fit in int (the
+            // tile ends below 2 GiB), but the 8-lane copy below steps up to 31 bytes past a row's end: its indexes
+            // are 64-bit.
             int carry = ws[warp];
             int *my_pre = wpre + warp * 33;
             int *my_end = wend + warp * 32;
             const uint8_t **my_src = wsrc + warp * 32;
-            for (int ob0 = wbeg; ob0 < wbeg + RW && ob0 < n_out; ob0 += 32) {
+            const int ob_end = byte_base < 0 ? wbeg : min(wbeg + RW, n_out);      // a tile past 2 GiB stores nothing
+            for (int ob0 = wbeg; ob0 < ob_end; ob0 += 32) {
                 const int ob = ob0 + lane;
                 const bool active = ob >= 0 && ob < n_out;
                 int len = 0;
@@ -786,7 +803,7 @@ k_emit(EmitArgs ea) {
                     const uint8_t *pa = nullptr, *pb = nullptr;
                     if (ra < n_pay) { a0 = my_pre[ra]; a1 = my_end[ra]; pa = my_src[ra] - a0; }
                     if (rb < n_pay) { b0 = my_pre[rb]; b1 = my_end[rb]; pb = my_src[rb] - b0; }
-                    const int ia = a0 + (lane & 7), ib = b0 + (lane & 7);
+                    const int64_t ia = (int64_t)a0 + (lane & 7), ib = (int64_t)b0 + (lane & 7);
                     uint8_t xa0 = 0, xa1 = 0, xa2 = 0, xb0 = 0, xb1 = 0, xb2 = 0;
                     if (ia < a1) xa0 = pa[ia];
                     if (ia + 8 < a1) xa1 = pa[ia + 8];
@@ -800,8 +817,8 @@ k_emit(EmitArgs ea) {
                     if (ib < b1) dbase[ib] = xb0;
                     if (ib + 8 < b1) dbase[ib + 8] = xb1;
                     if (ib + 16 < b1) dbase[ib + 16] = xb2;
-                    for (int b = ia + 24; b < a1; b += 8) dbase[b] = pa[b];
-                    for (int b = ib + 24; b < b1; b += 8) dbase[b] = pb[b];
+                    for (int64_t b = ia + 24; b < a1; b += 8) dbase[b] = pa[b];
+                    for (int64_t b = ib + 24; b < b1; b += 8) dbase[b] = pb[b];
                 }
                 __syncwarp();
             }

@@ -29,6 +29,7 @@ $(LIB): $(OBJS)
 ptxas-info: $(SRCS) $(HDRS)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c -o /dev/null paimon_b200/csrc/merge.cu
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c -o /dev/null paimon_b200/csrc/file_index.cu
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c -o /dev/null paimon_b200/csrc/parquet_encode.cu
 
 # the JNI shim against the JNI specification's signatures (no JDK in the image: jni/stub/jni.h)
 jni-check:

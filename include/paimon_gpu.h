@@ -390,10 +390,17 @@ pg_status pg_run_apply_deletion_vector(uint64_t run, const uint8_t *deleted_bitm
  * MergeTreeCompactRewriter.rewriteCompaction (:78-116).  `source` is a merge handle holding a batch or a run
  * handle; rows [row0, row0 + n_rows) are encoded (row0 a multiple of 8, n_rows < 0 = to the end), so a rolling
  * writer (RollingFileWriterImpl.java:64-105) cuts one batch into several files.  Written: data pages V1, PLAIN,
- * uncompressed, definition levels for nullable columns, per-chunk statistics. */
+ * uncompressed, definition levels for nullable columns, per-chunk statistics and, with options->page_index = 1, the
+ * page index parquet-mr writes: per column chunk a ColumnIndex (each page's null flag, min, max and null count, the
+ * boundary order; STRING / BINARY bounds truncated to 64 bytes; none for a chunk with a NaN) and an OffsetIndex (each
+ * page's offset, size and first row in its row group), all ColumnIndexes and then all OffsetIndexes between the last
+ * row group and the footer.  The page bounds are computed on the device.
+ * ABI version 2 grew this struct by its trailing field page_index: callers built against the two-field struct must
+ * be rebuilt. */
 typedef struct {
     int64_t row_group_rows;        /* 0 = 1 Mi rows */
     int64_t page_rows;             /* 0 = 32 Ki rows; rounded up to a multiple of 8 */
+    int64_t page_index;            /* 0 = none (NULL options: none), 1 = ColumnIndex + OffsetIndex; else PG_ERR_INVALID */
 } pg_parquet_write_options;
 
 typedef struct {

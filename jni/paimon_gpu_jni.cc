@@ -263,14 +263,15 @@ JNIEXPORT jint JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetFree(JNIEnv
     return 0;
 }
 
-// Compaction output encode: rows [row0, row0 + nRows) of a merge batch / run -> one Parquet file on the device
+// Compaction output encode: rows [row0, row0 + nRows) of a merge batch / run -> one Parquet file on the device;
+// pageIndex writes the ColumnIndex / OffsetIndex of every column chunk (pg_parquet_write_options.page_index)
 JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetEncode(JNIEnv *env, jclass, jlong source,
                                                                              jobjectArray names, jlong row0,
                                                                              jlong nRows, jlong rowGroupRows,
-                                                                             jlong pageRows) {
+                                                                             jlong pageRows, jboolean pageIndex) {
     std::vector<std::string> keep;
     std::vector<const char *> ptrs = utf_names(env, names, keep);
-    pg_parquet_write_options opt{rowGroupRows, pageRows};
+    pg_parquet_write_options opt{rowGroupRows, pageRows, pageIndex ? 1 : 0};
     uint64_t h = 0;
     PG_CHECK(pg_parquet_encode((uint64_t)source, ptrs.data(), row0, nRows, &opt, &h));
     return (jlong)h;
@@ -280,11 +281,11 @@ JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetEncode(JNI
 JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetEncodeCompressed(JNIEnv *env, jclass, jlong source,
                                                                                        jobjectArray names, jlong row0,
                                                                                        jlong nRows, jlong rowGroupRows,
-                                                                                       jlong pageRows, jint codec,
-                                                                                       jint level) {
+                                                                                       jlong pageRows, jboolean pageIndex,
+                                                                                       jint codec, jint level) {
     std::vector<std::string> keep;
     std::vector<const char *> ptrs = utf_names(env, names, keep);
-    pg_parquet_write_options opt{rowGroupRows, pageRows};
+    pg_parquet_write_options opt{rowGroupRows, pageRows, pageIndex ? 1 : 0};
     uint64_t h = 0;
     PG_CHECK(pg_parquet_encode_compressed((uint64_t)source, ptrs.data(), row0, nRows, &opt, codec, level, &h));
     return (jlong)h;

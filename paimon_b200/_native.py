@@ -78,7 +78,7 @@ class PgSectionInfo(C.Structure):
 
 
 class PgParquetWriteOptions(C.Structure):
-    _fields_ = [("row_group_rows", C.c_int64), ("page_rows", C.c_int64)]
+    _fields_ = [("row_group_rows", C.c_int64), ("page_rows", C.c_int64), ("page_index", C.c_int64)]
 
 
 class PgFileMeta(C.Structure):

@@ -117,12 +117,13 @@ class KeyValueDataFileWriter:
     `file_index` (the table's 'file-index.*' options) the file gets the bloom filters of its value columns, built on
     the device over the rows of the file, as DataFileMeta.embedded_index or the side file of extra_files
     (KeyValueDataFileWriter.java:103-113,156-181); options the device cannot build are refused here, before any
-    device work."""
+    device work.  With `page_index` a Parquet file carries the ColumnIndex and OffsetIndex of every column chunk
+    (the page bounds computed on the device), as parquet-mr writes them; ORC files ignore it."""
 
     def __init__(self, schema: KeyValueSchema, path: str, level: int, file_io: Optional[LocalFileIO] = None,
                  row_group_rows: int = 0, page_rows: int = 0, compression: str = "none", zstd_level: int = 1,
                  file_format: str = "parquet", stripe_rows: int = 0, compression_block_size: int = 0,
-                 file_index: Optional[FileIndexOptions] = None):
+                 file_index: Optional[FileIndexOptions] = None, page_index: bool = False):
         self.schema = schema
         self.path = path
         self.level = level
@@ -135,7 +136,7 @@ class KeyValueDataFileWriter:
             raise ValueError(f"unknown {self.file_format} file compression {compression!r}")
         self.codec = codecs[compression.lower()]
         self.zstd_level = int(zstd_level)
-        self.opts = N.PgParquetWriteOptions(row_group_rows, page_rows)
+        self.opts = N.PgParquetWriteOptions(row_group_rows, page_rows, int(bool(page_index)))
         if self.file_format == "orc":
             fields = schema.file_fields()
             self._orc_types = (N.PgOrcColumnType * len(fields))(*[N.PgOrcColumnType(*orc_column_type(f.type))
@@ -210,15 +211,17 @@ class KeyValueDataFileWriter:
 
 class RollingFileWriter:
     """Cuts one batch into files of at most `target_file_rows` rows (the reference rolls on the byte size of the
-    output stream, RollingFileWriterImpl.java:85-100; rows are what the device knows before encoding)."""
+    output stream, RollingFileWriterImpl.java:85-100; rows are what the device knows before encoding).  Every file
+    takes `writer_args` (KeyValueDataFileWriter's arguments) and `page_index`."""
 
     def __init__(self, schema: KeyValueSchema, directory: str, level: int, target_file_rows: int,
-                 file_io: Optional[LocalFileIO] = None, prefix: str = "data", **writer_args):
+                 file_io: Optional[LocalFileIO] = None, prefix: str = "data", page_index: bool = False,
+                 **writer_args):
         self.schema, self.directory, self.level = schema, directory, level
         self.target = max(8, (int(target_file_rows) + 7) & ~7)       # files start at multiples of 8 rows
         self.file_io = file_io
         self.prefix = prefix
-        self.writer_args = writer_args
+        self.writer_args = dict(writer_args, page_index=page_index)
         self.suffix = writer_args.get("file_format", "parquet").lower()
         self.results: List[WrittenFile] = []
 
@@ -243,11 +246,14 @@ class MergeTreeCompactRewriter:
     options), the files written at the output level take the format format_for_level(options, level) and, for
     parquet, the codec compression_for_level(options, level), for orc orc_compression_for_level(options, level),
     and the 'file-index.*' options give every file its bloom filters (refused before any device work when the device
-    cannot build them); without, they are uncompressed Parquet (or the writer arguments' file_format)."""
+    cannot build them); without, they are uncompressed Parquet (or the writer arguments' file_format).  With
+    `page_index` the files of Parquet output levels carry the page index (ColumnIndex and OffsetIndex); ORC output
+    levels write no row indexes and ignore it."""
 
     def __init__(self, schema: KeyValueSchema, mf_factory: MergeFunctionFactory, directory: str,
                  user_defined_seq_comparator=None, file_io: Optional[LocalFileIO] = None, device: int = 0,
-                 target_file_rows: int = 4 << 20, options: Optional[Dict[str, object]] = None, **writer_args):
+                 target_file_rows: int = 4 << 20, options: Optional[Dict[str, object]] = None,
+                 page_index: bool = False, **writer_args):
         self.schema = schema
         self.mf_factory = mf_factory
         self.directory = directory
@@ -257,6 +263,7 @@ class MergeTreeCompactRewriter:
         self.device = device
         self.target_file_rows = target_file_rows
         self.options = options
+        self.page_index = page_index
         self.writer_args = writer_args
 
     def rewrite(self, output_level: int, drop_delete: bool, sections: Sequence[Sequence[SortedRun]]) -> CompactResult:
@@ -282,8 +289,10 @@ class MergeTreeCompactRewriter:
             if not file_index.is_empty():
                 DataFileIndexWriter(self.schema, file_index)          # refuses before any device work
                 writer_args["file_index"] = file_index
+        parquet = writer_args.get("file_format", "parquet").lower() == "parquet"
         rolling = RollingFileWriter(self.schema, self.directory, output_level, self.target_file_rows, self.file_io,
-                                    prefix=f"compact-l{output_level}", **writer_args)
+                                    prefix=f"compact-l{output_level}", page_index=self.page_index and parquet,
+                                    **writer_args)
         for section in sections:
             for run in section:
                 result.before += run.files

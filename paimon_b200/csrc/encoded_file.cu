@@ -218,14 +218,22 @@ pg_status finish_encode(SectionTimer &tm, std::unique_ptr<EncodedFile> ef, int l
 FileStats::FileStats(const Schema &s)
     : n_key_(s.n_key), cols_(s.n_cols(), ColStats{INT64_MAX, INT64_MIN, 0, 0}), nan_(s.n_cols(), 0) {}
 
-ColStats FileStats::add(int col, const EncColumn &ec, const int64_t *sw, int64_t rows) {
-    const bool fp = ec.type == PG_FLOAT || ec.type == PG_DOUBLE;
+ColStats piece_stats(const EncColumn &ec, const int64_t *sw, int64_t rows) {
     ColStats p;
     p.null_count = rows - sw[2];
     p.has_minmax = ec.width > 0 && sw[2] > 0 && !sw[4];
     p.min = sw[0];
     p.max = sw[1];
-    if (fp && p.has_minmax) { p.min = zero_as(p.min, -0.0); p.max = zero_as(p.max, 0.0); }
+    if ((ec.type == PG_FLOAT || ec.type == PG_DOUBLE) && p.has_minmax) {
+        p.min = zero_as(p.min, -0.0);
+        p.max = zero_as(p.max, 0.0);
+    }
+    return p;
+}
+
+ColStats FileStats::add(int col, const EncColumn &ec, const int64_t *sw, int64_t rows) {
+    const bool fp = ec.type == PG_FLOAT || ec.type == PG_DOUBLE;
+    const ColStats p = piece_stats(ec, sw, rows);
     nan_[col] |= sw[4] != 0;
     if (col == n_key_ + 1) deletes_ += sw[3];
     // the merge keeps the zero rule: the zero min it can take is -0.0, the zero max +0.0

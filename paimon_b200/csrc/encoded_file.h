@@ -43,6 +43,10 @@ inline int64_t zero_as(int64_t bits, double zero) {
     return bits;
 }
 
+// The statistics of a piece of `rows` rows from its k_pw_stats words: no min / max if var-len, all null or holding a
+// NaN; a FLOAT / DOUBLE zero min as -0.0, a zero max as +0.0 (parquet.thrift), so both zeros lie inside.
+ColStats piece_stats(const EncColumn &ec, const int64_t *sw, int64_t rows);
+
 using Part = std::pair<int64_t, std::vector<uint8_t>>;  // a host-built piece of the file: (offset, bytes)
 
 struct EncodedFile {
@@ -79,8 +83,7 @@ pg_status patch(Scratch &scratch, const std::vector<Part> &parts, uint8_t *dst, 
 // of each column (a Parquet column chunk, or one column of an ORC stripe).
 struct FileStats {
     explicit FileStats(const Schema &s);
-    // Folds in a piece of `rows` rows of column `col` and returns its statistics: no min / max if var-len, all null or
-    // holding a NaN; a FLOAT / DOUBLE zero min as -0.0, a zero max as +0.0 (parquet.thrift), so both zeros lie inside.
+    // Folds in a piece of `rows` rows of column `col` and returns its piece_stats.
     ColStats add(int col, const EncColumn &ec, const int64_t *sw, int64_t rows);
     // ef.stats, with no min / max where any piece held a NaN (NaN sorts above every value under Double.compare);
     // delete_row_count (the retracts of the _VALUE_KIND column) and min / max_sequence_number

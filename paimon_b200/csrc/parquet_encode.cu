@@ -13,7 +13,9 @@
 //        nullable -> OPTIONAL (max definition level 1), NOT NULL -> REQUIRED)
 //
 // Layout written: PAR1 | per row group, per column: data pages V1, PLAIN, uncompressed or one zstd frame per page
-// body (pg_parquet_encode_compressed) | FileMetaData | len | PAR1.
+// body (pg_parquet_encode_compressed) | with page_index: every ColumnIndex, then every OffsetIndex (parquet-mr's
+// order) | FileMetaData | len | PAR1.  Page bounds come from k_pw_stats, run per page (the chunk statistics are
+// folded from the page words on the host), and for STRING / BINARY from k_pw_minmax_bytes.
 // Pages start at multiples of 8 rows, so a nullable column's definition levels (bit width 1, bit-packed LSB first)
 // ARE the bytes of the Arrow validity bitmap: they are copied, not re-encoded.  Values of non-null rows are
 // compacted by a block-wide scan; BYTE_ARRAY values are written as [len:int32][bytes].
@@ -138,6 +140,85 @@ k_pw_encode(const EncColumn *cols, const EncJob *jobs, uint8_t *file) {
     }
 }
 
+// ------------------------------------------------------------------ page index: bounds of var-len pages
+
+constexpr int kTruncate = 64;     // parquet-mr's default column-index truncation length
+constexpr int kHeadBytes = kTruncate + 1;
+
+struct BytesBound {               // per page of a var-len column: its least [0] and its greatest [1] non-null value
+    int64_t row[2];               // -1: the page has no non-null value
+    int32_t start[2], len[2];     // where the value's bytes lie in the column's payload, and how many
+    uint8_t head[2][kHeadBytes];  // its first min(len, kHeadBytes) bytes
+};
+
+// a candidate bound of a var-len page: its row (-1 = none) and where its bytes lie in the column's payload, kept in
+// registers so that a comparison reads the payload of the row it is offered only
+struct Cand { int64_t row; int32_t start, len; };
+
+// unsigned-byte lexicographic order, a proper prefix first: < 0, 0 or > 0
+__device__ __forceinline__ int cmp_values(const uint8_t *data, const Cand &a, const Cand &b) {
+    const uint8_t *pa = data + a.start, *pb = data + b.start;
+    const int n = min(a.len, b.len);
+    for (int i = 0; i < n; i++)
+        if (pa[i] != pb[i]) return (int)pa[i] - (int)pb[i];
+    return a.len - b.len;
+}
+
+// x replaces lo when it is smaller, hi when it is greater
+__device__ __forceinline__ void take_bounds(const uint8_t *data, Cand &lo, Cand &hi, const Cand &xlo, const Cand &xhi) {
+    if (xlo.row >= 0 && (lo.row < 0 || cmp_values(data, xlo, lo) < 0)) lo = xlo;
+    if (xhi.row >= 0 && (hi.row < 0 || cmp_values(data, xhi, hi) > 0)) hi = xhi;
+}
+
+__device__ __forceinline__ Cand shfl_xor(const Cand &c, int d) {
+    return Cand{__shfl_xor_sync(0xffffffffu, c.row, d), __shfl_xor_sync(0xffffffffu, c.start, d),
+                __shfl_xor_sync(0xffffffffu, c.len, d)};
+}
+
+// One CTA per var-len page (jobs[which[blockIdx.x]]): the rows of its least and greatest non-null value, found by a
+// strided scan per thread, a shuffle reduction per warp and one across the warps, and the first kHeadBytes bytes of
+// each, so that the host reads the bounds back in one small read.
+__global__ void __launch_bounds__(256)
+k_pw_minmax_bytes(const EncColumn *cols, const EncJob *jobs, const int32_t *which, BytesBound *out) {
+    const EncJob j = jobs[which[blockIdx.x]];
+    const EncColumn c = cols[j.col];
+    const uint8_t *data = (const uint8_t *)c.data;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    Cand lo{-1, 0, 0}, hi{-1, 0, 0};
+    for (int i = threadIdx.x; i < j.n_rows; i += blockDim.x) {
+        const int64_t row = j.row0 + i;
+        if (!valid_bit(c.validity, row)) continue;
+        const int32_t st = c.offsets[row];
+        const Cand x{row, st, c.offsets[row + 1] - st};
+        take_bounds(data, lo, hi, x, x);
+    }
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+        const Cand xlo = shfl_xor(lo, d), xhi = shfl_xor(hi, d);
+        take_bounds(data, lo, hi, xlo, xhi);
+    }
+    __shared__ Cand s_lo[8], s_hi[8];
+    if (lane == 0) { s_lo[warp] = lo; s_hi[warp] = hi; }
+    __syncthreads();
+    if (warp) return;
+    const int nw = blockDim.x >> 5;
+    if (lane < nw) { lo = s_lo[lane]; hi = s_hi[lane]; }
+    else lo.row = hi.row = -1;
+#pragma unroll
+    for (int d = 4; d > 0; d >>= 1) {
+        const Cand xlo = shfl_xor(lo, d), xhi = shfl_xor(hi, d);
+        take_bounds(data, lo, hi, xlo, xhi);
+    }
+    BytesBound &o = out[blockIdx.x];
+    for (int k = 0; k < 2; k++) {
+        Cand b = k ? hi : lo;
+        b = Cand{__shfl_sync(0xffffffffu, b.row, 0), __shfl_sync(0xffffffffu, b.start, 0),
+                 __shfl_sync(0xffffffffu, b.len, 0)};
+        if (lane == 0) { o.row[k] = b.row; o.start[k] = b.start; o.len[k] = b.len; }
+        for (int i = lane; i < min(b.len, kHeadBytes); i += 32) o.head[k][i] = data[b.start + i];
+    }
+}
+
 static int parquet_type_of(int t) {
     switch (t) {
         case PG_BOOL: return pq::T_BOOLEAN;
@@ -150,17 +231,25 @@ static int parquet_type_of(int t) {
 }
 
 // The column chunks and data pages of a file, built in one pass over (row group, column, page).  jobs[p] and
-// sjobs[k] are what the kernels read for pages[p] and chunks[k], in arrays that go to the device as they are.
+// sjobs[p] are what the kernels read for pages[p], in arrays that go to the device as they are.
 struct Page {
     std::vector<uint8_t> prefix;  // RLE-hybrid definition levels: [length:int32][run header varint]; empty = REQUIRED
     int64_t def_bytes = 0;        // prefix and level bytes
     int64_t body = 0;             // page body bytes
     int64_t stored = 0;           // bytes in the file: the body, or its zstd frame
+    int64_t null_count = 0;
+    bool nan = false;             // a non-null value is NaN
+    std::vector<uint8_t> min, max;  // ColumnIndex bounds, PLAIN-encoded; empty for a page of NULLs only
+    int64_t header_off = 0, header_bytes = 0;  // PageLocation: offset, and with `stored`, compressed_page_size
 };
 struct Chunk {
+    int col;
+    int64_t row0, n_rows;         // its rows (row0: the batch row its row group starts at)
     size_t page0, page1;          // its pages
     ColStats st;                  // the footer's Statistics
     int64_t first_page = 0, total_uncompressed = 0, total_compressed = 0;
+    int64_t column_index_off = -1, offset_index_off = -1;   // -1: not written
+    int32_t column_index_len = 0, offset_index_len = 0;
 };
 struct Plan {
     int64_t n_groups = 0;
@@ -188,27 +277,73 @@ static Plan make_plan(const Schema &s, const std::vector<DevColumn> &dcols, int6
     for (int64_t g = 0; g < pl.n_groups; g++) {
         const int64_t g0 = row0 + g * group_rows, g1 = std::min(row0 + n_rows, g0 + group_rows);
         for (int c = 0; c < nc; c++) {
-            pl.sjobs.push_back(StatJob{c, 0, g0, g1 - g0});
             const size_t page0 = pl.jobs.size();
-            for (int64_t p0 = g0; p0 < g1; p0 += page_rows)
-                pl.jobs.push_back(EncJob{c, (int32_t)(std::min(g1, p0 + page_rows) - p0), p0, -1, 0});
-            pl.chunks.push_back(Chunk{page0, pl.jobs.size(), ColStats{}});
+            for (int64_t p0 = g0; p0 < g1; p0 += page_rows) {
+                const int64_t n = std::min(g1, p0 + page_rows) - p0;
+                pl.jobs.push_back(EncJob{c, (int32_t)n, p0, -1, 0});
+                pl.sjobs.push_back(StatJob{c, 0, p0, n});
+            }
+            pl.chunks.push_back(Chunk{c, g0, g1 - g0, page0, pl.jobs.size(), ColStats{}});
         }
     }
     pl.pages.resize(pl.jobs.size());
     return pl;
 }
 
+// The k_pw_stats words of a chunk from those of its pages: min of the mins, max of the maxes (as doubles for FLOAT /
+// DOUBLE: the words of a page without a non-NaN value are +inf / -inf), summed counts, NaN OR-ed.
+static void fold_page_words(const EncColumn &ec, const int64_t *sw, size_t n_pages, int64_t *out) {
+    const bool fp = ec.type == PG_FLOAT || ec.type == PG_DOUBLE;
+    for (int w = 0; w < kStatWords; w++) out[w] = sw[w];
+    for (size_t p = 1; p < n_pages; p++) {
+        const int64_t *x = sw + kStatWords * p;
+        if (fp) {
+            double a, b, lo, hi;
+            memcpy(&a, &out[0], 8); memcpy(&b, &out[1], 8); memcpy(&lo, &x[0], 8); memcpy(&hi, &x[1], 8);
+            a = std::min(a, lo); b = std::max(b, hi);
+            memcpy(&out[0], &a, 8); memcpy(&out[1], &b, 8);
+        } else {
+            out[0] = std::min(out[0], x[0]);
+            out[1] = std::max(out[1], x[1]);
+        }
+        out[2] += x[2];
+        out[3] += x[3];
+        out[4] |= x[4];
+    }
+}
+
+// a fixed-width bound PLAIN-encoded in the column's physical type: INT8 / INT16 / INT32 as 4 bytes, BOOLEAN as 1,
+// FLOAT as 4 (`v` holds the double)
+static std::vector<uint8_t> plain_bound(const EncColumn &ec, int64_t v) {
+    uint8_t b[8];
+    size_t n = ec.width == 8 ? 8 : 4;
+    if (ec.type == PG_FLOAT) {
+        double d; memcpy(&d, &v, 8);
+        const float f = (float)d; memcpy(b, &f, 4);
+    } else if (ec.type == PG_BOOL) {
+        n = 1; b[0] = (uint8_t)v;
+    } else if (n == 4) {
+        const int32_t x = (int32_t)v; memcpy(b, &x, 4);
+    } else memcpy(b, &v, 8);
+    return std::vector<uint8_t>(b, b + n);
+}
+
 // The device's counts -> each page's level prefix and body size, each chunk's statistics (folded into the file's by
-// `fs`).  counts: per page, non-null rows and payload bytes (k_pw_count); stats: per chunk, kStatWords (k_pw_stats).
+// `fs`) and, for a fixed-width column, each page's ColumnIndex entry.  counts: per page, non-null rows and payload
+// bytes (k_pw_count); stats: per page, kStatWords (k_pw_stats).
 static pg_status fold_counts(Plan &pl, const int64_t *counts, const int64_t *stats, FileStats &fs) {
-    for (size_t k = 0; k < pl.chunks.size(); k++) {
-        const EncColumn &ec = pl.cols[pl.sjobs[k].col];
-        Chunk &ch = pl.chunks[k];
-        ch.st = fs.add(pl.sjobs[k].col, ec, &stats[kStatWords * k], pl.sjobs[k].n_rows);
+    for (Chunk &ch : pl.chunks) {
+        const EncColumn &ec = pl.cols[ch.col];
+        int64_t words[kStatWords];
+        fold_page_words(ec, &stats[kStatWords * ch.page0], ch.page1 - ch.page0, words);
+        ch.st = fs.add(ch.col, ec, words, ch.n_rows);
         for (size_t p = ch.page0; p < ch.page1; p++) {
             Page &pg = pl.pages[p];
             const int64_t nn = counts[2 * p], vb = counts[2 * p + 1];
+            const ColStats ps = piece_stats(ec, &stats[kStatWords * p], pl.jobs[p].n_rows);
+            pg.null_count = ps.null_count;
+            pg.nan = stats[kStatWords * p + 4] != 0;
+            if (ps.has_minmax) { pg.min = plain_bound(ec, ps.min); pg.max = plain_bound(ec, ps.max); }
             if (ec.optional) {                                 // one bit-packed run of bit width 1
                 const int64_t groups = (pl.jobs[p].n_rows + 7) / 8;
                 std::vector<uint8_t> run;
@@ -262,18 +397,191 @@ static std::vector<uint8_t> page_header(const Page &pg, int32_t n_rows) {
 
 // Statistics max_value / min_value: a chunk's bounds, PLAIN-encoded in the column's physical type
 static void write_min_max(pq::ThriftWriter &w, const EncColumn &ec, const ColStats &st) {
-    uint8_t mn[8], mx[8];
-    size_t n = ec.width == 8 ? 8 : 4;
-    if (ec.type == PG_FLOAT) {
-        double a, b; memcpy(&a, &st.min, 8); memcpy(&b, &st.max, 8);
-        float fa = (float)a, fb = (float)b; memcpy(mn, &fa, 4); memcpy(mx, &fb, 4);
-    } else if (ec.type == PG_BOOL) {
-        n = 1; mn[0] = (uint8_t)st.min; mx[0] = (uint8_t)st.max;
-    } else if (n == 4) {
-        int32_t a = (int32_t)st.min, b = (int32_t)st.max; memcpy(mn, &a, 4); memcpy(mx, &b, 4);
-    } else { memcpy(mn, &st.min, 8); memcpy(mx, &st.max, 8); }
-    w.bin(5, mx, n);
-    w.bin(6, mn, n);
+    const std::vector<uint8_t> mn = plain_bound(ec, st.min), mx = plain_bound(ec, st.max);
+    w.bin(5, mx.data(), mx.size());
+    w.bin(6, mn.data(), mn.size());
+}
+
+// ------------------------------------------------------------------ page index (ColumnIndex, OffsetIndex)
+
+// The var-len bounds of the ColumnIndex, truncated to kTruncate bytes as parquet-mr truncates them.  `v` holds the
+// first min(len, kHeadBytes) bytes of a value of `len` bytes.  A longer min becomes its prefix (STRING: cut back to a
+// code-point boundary); a longer max becomes that prefix up to its last position that can be incremented, incremented
+// (BINARY: a byte below 0xFF; STRING: a code point below U+10FFFF, the surrogates skipped), so min <= value <= max
+// holds.  When no position can be incremented the max is the whole value, and *whole is set.
+static int utf8_cut(const uint8_t *v, bool utf8) {
+    int n = kTruncate;
+    if (utf8)
+        while (n > 0 && (v[n] & 0xC0) == 0x80) n--;
+    return n;
+}
+
+static std::vector<uint8_t> truncate_min(const uint8_t *v, int len, bool utf8) {
+    return std::vector<uint8_t>(v, v + (len <= kTruncate ? len : utf8_cut(v, utf8)));
+}
+
+// the code point of the UTF-8 sequence v[s, e), -1 if it is not one well-formed sequence
+static int32_t utf8_decode(const uint8_t *v, int s, int e) {
+    const int n = e - s;
+    const uint8_t b0 = v[s];
+    int want;
+    int32_t cp;
+    if (b0 < 0x80) { want = 1; cp = b0; }
+    else if ((b0 & 0xE0) == 0xC0) { want = 2; cp = b0 & 0x1F; }
+    else if ((b0 & 0xF0) == 0xE0) { want = 3; cp = b0 & 0x0F; }
+    else if ((b0 & 0xF8) == 0xF0) { want = 4; cp = b0 & 0x07; }
+    else return -1;
+    if (n != want) return -1;
+    for (int i = 1; i < n; i++) {
+        if ((v[s + i] & 0xC0) != 0x80) return -1;
+        cp = (cp << 6) | (v[s + i] & 0x3F);
+    }
+    static const int32_t least[5] = {0, 0, 0x80, 0x800, 0x10000};
+    if (cp < least[n] || cp > 0x10FFFF || (cp >= 0xD800 && cp <= 0xDFFF)) return -1;
+    return cp;
+}
+
+static void utf8_encode(std::vector<uint8_t> &b, int32_t cp) {
+    if (cp < 0x80) b.push_back((uint8_t)cp);
+    else if (cp < 0x800) { b.push_back((uint8_t)(0xC0 | (cp >> 6))); b.push_back((uint8_t)(0x80 | (cp & 0x3F))); }
+    else if (cp < 0x10000) {
+        b.push_back((uint8_t)(0xE0 | (cp >> 12)));
+        b.push_back((uint8_t)(0x80 | ((cp >> 6) & 0x3F)));
+        b.push_back((uint8_t)(0x80 | (cp & 0x3F)));
+    } else {
+        b.push_back((uint8_t)(0xF0 | (cp >> 18)));
+        b.push_back((uint8_t)(0x80 | ((cp >> 12) & 0x3F)));
+        b.push_back((uint8_t)(0x80 | ((cp >> 6) & 0x3F)));
+        b.push_back((uint8_t)(0x80 | (cp & 0x3F)));
+    }
+}
+
+static std::vector<uint8_t> truncate_max(const uint8_t *v, int len, bool utf8, bool *whole) {
+    *whole = false;
+    if (len <= kTruncate) return std::vector<uint8_t>(v, v + len);
+    int end = utf8_cut(v, utf8);
+    while (end > 0) {
+        if (!utf8) {
+            if (v[end - 1] != 0xFF) {
+                std::vector<uint8_t> out(v, v + end);
+                out.back()++;
+                return out;
+            }
+            end--;
+            continue;
+        }
+        int s = end - 1;
+        while (s > 0 && end - s < 4 && (v[s] & 0xC0) == 0x80) s--;
+        int32_t cp = utf8_decode(v, s, end);
+        if (cp < 0) { end--; continue; }                        // not a code point: that byte is skipped
+        if (cp < 0x10FFFF) {
+            std::vector<uint8_t> out(v, v + s);
+            utf8_encode(out, cp + 1 == 0xD800 ? 0xE000 : cp + 1);
+            return out;
+        }
+        end = s;
+    }
+    *whole = true;
+    return {};
+}
+
+// two PLAIN-encoded bounds in the column's order: signed integers, numeric FLOAT / DOUBLE, unsigned bytes
+template <typename T> static int cmp_as(const std::vector<uint8_t> &a, const std::vector<uint8_t> &b) {
+    T x, y;
+    memcpy(&x, a.data(), sizeof(T)); memcpy(&y, b.data(), sizeof(T));
+    return (x > y) - (x < y);
+}
+static int cmp_bound(const EncColumn &ec, const std::vector<uint8_t> &a, const std::vector<uint8_t> &b) {
+    switch (ec.type) {
+        case PG_FLOAT: return cmp_as<float>(a, b);
+        case PG_DOUBLE: return cmp_as<double>(a, b);
+        case PG_BOOL: return cmp_as<uint8_t>(a, b);
+        default:
+            if (ec.width == 0) return a < b ? -1 : (b < a ? 1 : 0);
+            return ec.width == 8 ? cmp_as<int64_t>(a, b) : cmp_as<int32_t>(a, b);
+    }
+}
+
+enum BoundaryOrder { B_UNORDERED = 0, B_ASCENDING = 1, B_DESCENDING = 2 };
+
+// ColumnIndex of a chunk: null_pages, min_values, max_values, boundary_order (over the non-null pages), null_counts
+static std::vector<uint8_t> column_index(const Plan &pl, const Chunk &ch) {
+    const EncColumn &ec = pl.cols[ch.col];
+    bool asc = true, desc = true;
+    const Page *prev = nullptr;
+    for (size_t p = ch.page0; p < ch.page1; p++) {
+        const Page &pg = pl.pages[p];
+        if (pg.null_count == pl.jobs[p].n_rows) continue;
+        if (prev) {
+            const int lo = cmp_bound(ec, prev->min, pg.min), hi = cmp_bound(ec, prev->max, pg.max);
+            asc = asc && lo <= 0 && hi <= 0;
+            desc = desc && lo >= 0 && hi >= 0;
+        }
+        prev = &pg;
+    }
+    const size_t n = ch.page1 - ch.page0;
+    pq::ThriftWriter w;
+    w.list(1, pq::CT_TRUE, n);                                 // (bool elements: 1 true, 2 false)
+    for (size_t p = ch.page0; p < ch.page1; p++)
+        w.b.push_back(pl.pages[p].null_count == pl.jobs[p].n_rows ? pq::CT_TRUE : pq::CT_FALSE);
+    w.list(2, pq::CT_BINARY, n);
+    for (size_t p = ch.page0; p < ch.page1; p++) w.binary(pl.pages[p].min.data(), pl.pages[p].min.size());
+    w.list(3, pq::CT_BINARY, n);
+    for (size_t p = ch.page0; p < ch.page1; p++) w.binary(pl.pages[p].max.data(), pl.pages[p].max.size());
+    w.i32(4, asc ? B_ASCENDING : desc ? B_DESCENDING : B_UNORDERED);
+    w.list(5, pq::CT_I64, n);
+    for (size_t p = ch.page0; p < ch.page1; p++) w.zigzag(pl.pages[p].null_count);
+    w.end();
+    return std::move(w.b);
+}
+
+// OffsetIndex of a chunk: per page {offset, compressed_page_size, first_row_index (in the row group)}
+static std::vector<uint8_t> offset_index(const Plan &pl, const Chunk &ch) {
+    pq::ThriftWriter w;
+    w.list(1, pq::CT_STRUCT, ch.page1 - ch.page0);
+    for (size_t p = ch.page0; p < ch.page1; p++) {
+        const Page &pg = pl.pages[p];
+        w.struct_elem();
+        w.i64(1, pg.header_off);
+        w.i32(2, (int32_t)(pg.header_bytes + pg.stored));
+        w.i64(3, pl.jobs[p].row0 - ch.row0);
+        w.end();
+    }
+    w.end();
+    return std::move(w.b);
+}
+
+// The ColumnIndex bounds of the var-len pages pl.jobs[which[i]] from their k_pw_minmax_bytes records bb[i].  A max
+// that has to be written whole is read in one more round of small reads.
+static pg_status varlen_bounds(Plan &pl, const std::vector<int32_t> &which, const std::vector<BytesBound> &bb) {
+    struct Whole { int32_t page; std::vector<uint8_t> bytes; const uint8_t *src; };
+    std::vector<Whole> whole;
+    for (size_t i = 0; i < which.size(); i++) {
+        const BytesBound &b = bb[i];
+        if (b.row[0] < 0) continue;                            // NULLs only
+        const EncColumn &ec = pl.cols[pl.jobs[which[i]].col];
+        const bool utf8 = ec.type == PG_STRING;
+        Page &pg = pl.pages[which[i]];
+        bool need_whole;
+        pg.min = truncate_min(b.head[0], b.len[0], utf8);
+        pg.max = truncate_max(b.head[1], b.len[1], utf8, &need_whole);
+        if (need_whole)
+            whole.push_back({which[i], std::vector<uint8_t>((size_t)b.len[1]), (const uint8_t *)ec.data + b.start[1]});
+    }
+    if (whole.empty()) return PG_OK;
+    SmallReads rd(0);
+    for (Whole &x : whole)
+        if (pg_status st = rd.add(x.bytes.data(), x.src, x.bytes.size())) return st;
+    if (pg_status st = rd.finish()) return st;
+    for (Whole &x : whole) pl.pages[x.page].max = std::move(x.bytes);
+    return PG_OK;
+}
+
+// A chunk gets a ColumnIndex unless a page holds a NaN (parquet-mr drops the column index of such a chunk)
+static bool has_column_index(const Plan &pl, const Chunk &ch) {
+    for (size_t p = ch.page0; p < ch.page1; p++)
+        if (pl.pages[p].nan) return false;
+    return true;
 }
 
 // FileMetaData, its length and "PAR1": the end of the file
@@ -316,7 +624,7 @@ static std::vector<uint8_t> footer(const Plan &pl, const char *const *names, int
             w.list(2, pq::CT_I32, 2); w.zigzag(pq::E_PLAIN); w.zigzag(pq::E_RLE);
             w.list(3, pq::CT_BINARY, 1); w.binary(col_names[c].data(), col_names[c].size());
             w.i32(4, zstd ? pq::C_ZSTD : pq::C_UNCOMPRESSED);
-            w.i64(5, pl.sjobs[k].n_rows);
+            w.i64(5, ch.n_rows);
             w.i64(6, ch.total_uncompressed);
             w.i64(7, ch.total_compressed);
             w.i64(9, ch.first_page);
@@ -325,10 +633,18 @@ static std::vector<uint8_t> footer(const Plan &pl, const char *const *names, int
             if (ch.st.has_minmax) write_min_max(w, pl.cols[c], ch.st);
             w.end();
             w.end();                                           // ColumnMetaData
+            if (ch.offset_index_off >= 0) {
+                w.i64(4, ch.offset_index_off);
+                w.i32(5, ch.offset_index_len);
+            }
+            if (ch.column_index_off >= 0) {
+                w.i64(6, ch.column_index_off);
+                w.i32(7, ch.column_index_len);
+            }
             w.end();                                           // ColumnChunk
         }
         w.i64(2, group_bytes);
-        w.i64(3, pl.sjobs[(size_t)g * nc].n_rows);             // the rows of the group: those of any of its chunks
+        w.i64(3, pl.chunks[(size_t)g * nc].n_rows);            // the rows of the group: those of any of its chunks
         w.end();
     }
     w.str(6, "paimon-b200 (libpaimon_gpu)");
@@ -349,6 +665,9 @@ static std::vector<uint8_t> footer(const Plan &pl, const char *const *names, int
 
 static pg_status encode(uint64_t source, const char *const *names, int64_t row0, int64_t n_rows,
                         const pg_parquet_write_options *opt, int codec, uint64_t *out_file) {
+    if (opt && opt->page_index != 0 && opt->page_index != 1)
+        return fail(PG_ERR_INVALID, "parquet encode: page_index " + std::to_string(opt->page_index) + " is not 0 or 1");
+    const bool page_index = opt && opt->page_index == 1;
     BatchColumns batch;                                      // held until the encode below is done
     pg_status st = encode_source(source, "parquet encode", row0, &n_rows, &batch);
     if (st) return st;
@@ -359,31 +678,49 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     if ((st = start_encode(tm))) return st;
 
     Plan pl = make_plan(*s, batch.cols, row0, n_rows, opt);
-    const size_t nj = pl.jobs.size(), nsj = pl.sjobs.size();
-    std::vector<int64_t> counts(2 * nj + 2), stats(kStatWords * (nsj + 1));
+    const size_t nj = pl.jobs.size();
+    std::vector<int32_t> vpages;                             // the var-len pages, whose bounds k_pw_minmax_bytes finds
+    for (size_t p = 0; page_index && p < nj; p++)
+        if (pl.cols[pl.jobs[p].col].width == 0) vpages.push_back((int32_t)p);
+    const size_t nv = vpages.size();
+    std::vector<int64_t> counts(2 * nj + 2), stats(kStatWords * (nj + 1));
+    std::vector<BytesBound> bounds(nv);
     Scratch scratch(0);                                      // temporaries, released on every path out of this function
     EncColumn *d_cols = (EncColumn *)scratch.take(sizeof(EncColumn) * nc);
     EncJob *d_jobs = (EncJob *)scratch.take(sizeof(EncJob) * std::max<size_t>(nj, 1));
-    StatJob *d_sjobs = (StatJob *)scratch.take(sizeof(StatJob) * std::max<size_t>(nsj, 1));
+    StatJob *d_sjobs = (StatJob *)scratch.take(sizeof(StatJob) * std::max<size_t>(nj, 1));
     int64_t *d_counts = (int64_t *)scratch.take(sizeof(int64_t) * (2 * nj + 2));
-    int64_t *d_stats = (int64_t *)scratch.take(sizeof(int64_t) * kStatWords * (nsj + 1));
-    if (!d_cols || !d_jobs || !d_sjobs || !d_counts || !d_stats)
+    int64_t *d_stats = (int64_t *)scratch.take(sizeof(int64_t) * kStatWords * (nj + 1));
+    int32_t *d_vpages = (int32_t *)scratch.take(sizeof(int32_t) * std::max<size_t>(nv, 1));
+    BytesBound *d_bounds = (BytesBound *)scratch.take(sizeof(BytesBound) * std::max<size_t>(nv, 1));
+    if (!d_cols || !d_jobs || !d_sjobs || !d_counts || !d_stats || !d_vpages || !d_bounds)
         return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the page tables");
     PG_CUDA(cudaMemcpy(d_cols, pl.cols.data(), sizeof(EncColumn) * nc, cudaMemcpyHostToDevice));
     int launches = 0;
     if (nj) {
         PG_CUDA(cudaMemcpy(d_jobs, pl.jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
-        PG_CUDA(cudaMemcpy(d_sjobs, pl.sjobs.data(), sizeof(StatJob) * nsj, cudaMemcpyHostToDevice));
+        PG_CUDA(cudaMemcpy(d_sjobs, pl.sjobs.data(), sizeof(StatJob) * nj, cudaMemcpyHostToDevice));
         k_pw_count<<<(unsigned)nj, 256>>>(d_cols, d_jobs, d_counts);
-        launch_pw_stats(d_cols, d_sjobs, (int)nsj, d_stats);
+        launch_pw_stats(d_cols, d_sjobs, (int)nj, d_stats);
         launches += 2;
+        if (nv) {
+            PG_CUDA(cudaMemcpy(d_vpages, vpages.data(), sizeof(int32_t) * nv, cudaMemcpyHostToDevice));
+            k_pw_minmax_bytes<<<(unsigned)nv, 256>>>(d_cols, d_jobs, d_vpages, d_bounds);
+            launches++;
+        }
         PG_CUDA(cudaMemcpy(counts.data(), d_counts, sizeof(int64_t) * 2 * nj, cudaMemcpyDeviceToHost));
-        PG_CUDA(cudaMemcpy(stats.data(), d_stats, sizeof(int64_t) * kStatWords * nsj, cudaMemcpyDeviceToHost));
+        PG_CUDA(cudaMemcpy(stats.data(), d_stats, sizeof(int64_t) * kStatWords * nj, cudaMemcpyDeviceToHost));
+        if (nv) {
+            SmallReads rd(0);
+            if ((st = rd.add(bounds.data(), d_bounds, sizeof(BytesBound) * nv)) || (st = rd.finish())) return st;
+            launches++;
+        }
     }
     auto ef = std::make_unique<EncodedFile>();
     FileStats fs(*s);
     if ((st = fold_counts(pl, counts.data(), stats.data(), fs))) return st;
     fs.finish(*ef);
+    if ((st = varlen_bounds(pl, vpages, bounds))) return st;
 
     // ---- zstd: bodies into a scratch image, one frame per body; the frame sizes come back before the layout
     const bool zstd = codec == pq::C_ZSTD;
@@ -410,17 +747,20 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         for (size_t p = 0; p < nj; p++) pl.pages[p].stored = frame_bytes[p];
     }
 
-    // ---- layout: "PAR1", per page its header and its stored body, the footer
+    // ---- layout: "PAR1", per page its header and its stored body, with the page index every ColumnIndex and then
+    // every OffsetIndex (row group major, then column), the footer
     int64_t pos = 4;
     ef->host_parts.push_back({0, {'P', 'A', 'R', '1'}});
     std::vector<int64_t> body_off(nj);
     for (Chunk &ch : pl.chunks) {
         ch.first_page = pos;
         for (size_t p = ch.page0; p < ch.page1; p++) {
-            const Page &pg = pl.pages[p];
+            Page &pg = pl.pages[p];
             std::vector<uint8_t> header = page_header(pg, pl.jobs[p].n_rows);
             const int64_t hb = (int64_t)header.size();
             ef->host_parts.push_back({pos, std::move(header)});
+            pg.header_off = pos;
+            pg.header_bytes = hb;
             body_off[p] = pos + hb;
             pos += hb + pg.stored;
             ch.total_uncompressed += hb + pg.body;
@@ -428,6 +768,23 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         }
     }
     ef->data_end = pos;
+    if (page_index) {
+        for (Chunk &ch : pl.chunks) {
+            if (!has_column_index(pl, ch)) continue;
+            std::vector<uint8_t> ci = column_index(pl, ch);
+            ch.column_index_off = pos;
+            ch.column_index_len = (int32_t)ci.size();
+            pos += (int64_t)ci.size();
+            ef->host_parts.push_back({ch.column_index_off, std::move(ci)});
+        }
+        for (Chunk &ch : pl.chunks) {
+            std::vector<uint8_t> oi = offset_index(pl, ch);
+            ch.offset_index_off = pos;
+            ch.offset_index_len = (int32_t)oi.size();
+            pos += (int64_t)oi.size();
+            ef->host_parts.push_back({ch.offset_index_off, std::move(oi)});
+        }
+    }
     ef->host_parts.push_back({pos, footer(pl, names, n_rows, zstd)});
     ef->file_bytes = pos + (int64_t)ef->host_parts.back().second.size();
 

@@ -8,7 +8,7 @@ SRCS := paimon_b200/csrc/merge.cu paimon_b200/csrc/emit.cu paimon_b200/csrc/api.
 	paimon_b200/csrc/orc_encode.cu paimon_b200/csrc/encoded_file.cu paimon_b200/csrc/file_index.cu
 HDRS := include/paimon_gpu.h paimon_b200/csrc/pg_internal.h paimon_b200/csrc/device_utils.cuh paimon_b200/csrc/parquet_meta.h \
 	paimon_b200/csrc/zstd_device.cuh paimon_b200/csrc/zstd_encode_device.cuh paimon_b200/csrc/inflate_device.cuh paimon_b200/csrc/lz4_device.cuh paimon_b200/csrc/snappy_device.cuh paimon_b200/csrc/orc_device.cuh paimon_b200/csrc/orc_meta.h \
-	paimon_b200/csrc/orc_encode_device.cuh paimon_b200/csrc/encoded_file.h paimon_b200/csrc/xxhash64_device.cuh \
+	paimon_b200/csrc/orc_encode_device.cuh paimon_b200/csrc/encoded_file.h paimon_b200/csrc/xxhash64_device.cuh paimon_b200/csrc/murmur3_device.cuh \
 	paimon_b200/csrc/scan_kernels.cuh paimon_b200/csrc/range_reader.h
 LIB := paimon_b200/libpaimon_gpu.so
 
@@ -30,6 +30,7 @@ ptxas-info: $(SRCS) $(HDRS)
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c -o /dev/null paimon_b200/csrc/merge.cu
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c -o /dev/null paimon_b200/csrc/file_index.cu
 	$(NVCC) $(NVFLAGS) -Xptxas -v -c -o /dev/null paimon_b200/csrc/parquet_encode.cu
+	$(NVCC) $(NVFLAGS) -Xptxas -v -c -o /dev/null paimon_b200/csrc/orc_encode.cu
 
 # the JNI shim against the JNI specification's signatures (no JDK in the image: jni/stub/jni.h)
 jni-check:

@@ -447,11 +447,11 @@ pg_status pg_parquet_file_free(uint64_t file);
  * pg_parquet_file_meta (n_row_groups counts stripes, n_pages streams), _column_stats (same meaning), _fetch,
  * _device_image and _free accept it.
  * Written: ORC v1 ("0.12"), a flat struct named by `column_names`, streams DIRECT / DIRECT_V2 (integer RLE v2 without
- * PATCHED_BASE, byte RLE, PRESENT only in stripes with a null), no row indexes or bloom filters, per-stripe and file
- * column statistics.  Compression kinds ZLIB / SNAPPY / LZO / LZ4 / BROTLI, zstd levels 0 and >= 2, TIMESTAMP, CHAR
- * and nested kinds, and a VARCHAR(n) value longer than n characters return PG_ERR_UNSUPPORTED; a compression kind
- * outside 0..6, a block size >= 2^23 or negative, and a kind that does not fit the column's physical type return
- * PG_ERR_INVALID. */
+ * PATCHED_BASE, byte RLE, PRESENT only in stripes with a null), per-stripe and file column statistics, and no row
+ * indexes or bloom filters (pg_orc_encode_indexed writes them).  Compression kinds ZLIB / SNAPPY / LZO / LZ4 / BROTLI,
+ * zstd levels 0 and >= 2, TIMESTAMP, CHAR and nested kinds, and a VARCHAR(n) value longer than n characters return
+ * PG_ERR_UNSUPPORTED; a compression kind outside 0..6, a block size >= 2^23 or negative, and a kind that does not fit
+ * the column's physical type return PG_ERR_INVALID. */
 typedef struct {
     int32_t kind;        /* ORC TypeKind (orc_proto): BOOLEAN 0, BYTE 1, SHORT 2, INT 3, LONG 4, FLOAT 5, DOUBLE 6,
                             STRING 7, BINARY 8, DECIMAL 14, DATE 15, VARCHAR 16 */
@@ -469,6 +469,30 @@ typedef struct {
 
 pg_status pg_orc_encode(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
                         const pg_orc_write_options *options, uint64_t *out_file);
+
+/* ---- the same encode with a row index and bloom filters ----------------------------------------------------
+ * What orc-core's WriterImpl writes with 'orc.create.index' (orc.row.index.stride rows per row group) and
+ * 'orc.bloom.filter.columns' / 'orc.bloom.filter.fpp' (paimon-format/.../orc/OrcConf.java): Paimon's ORC reader skips
+ * the row groups a scan's filter rules out.  Row groups are counted from each stripe's first row; the last one of a
+ * stripe may be short.  Every stripe starts with, per column (root first), a ROW_INDEX stream — per row group the
+ * positions of its first value in each of the column's streams (ORC v1 "Row Group Index") and the same statistics the
+ * stripe carries — and, for a bloom column, a BLOOM_FILTER_UTF8 stream: per row group one filter sized as orc-core sizes
+ * it for `row_index_stride` entries at `bloom_fpp`, built on the device.  The Footer carries the stride.
+ * pg_orc_encode is this call with a NULL `index`; a NULL index or a stride of 0 writes the same bytes.
+ * PG_ERR_INVALID: a stride that is negative or below 1000 (orc-core's minimum), bloom columns without a stride or
+ * with n_bloom_columns < 0, a bloom column outside the schema or listed twice, with bloom columns a bloom_fpp outside
+ * (0, 1).  PG_ERR_UNSUPPORTED, before any device work: a stride that is not a multiple of 8, a BOOLEAN or DECIMAL
+ * bloom column, a filter larger than one CTA's shared memory (227 KiB). */
+typedef struct {
+    int64_t row_index_stride;        /* 0 = no index (pg_orc_encode's bytes); else >= 1000 and a multiple of 8 */
+    int32_t n_bloom_columns;         /* 0 = no bloom filters; needs row_index_stride > 0 */
+    const int32_t *bloom_columns;    /* file column indexes */
+    double bloom_fpp;                /* 'orc.bloom.filter.fpp', in (0, 1) */
+} pg_orc_index_options;
+
+pg_status pg_orc_encode_indexed(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
+                                const pg_orc_write_options *options, const pg_orc_index_options *index,
+                                uint64_t *out_file);
 
 /* ---- compaction output: the bloom-filter file index of a data file ----------------------------------------
  * What KeyValueDataFileWriter builds row by row for a table with 'file-index.bloom-filter.columns'

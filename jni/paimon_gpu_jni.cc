@@ -290,15 +290,9 @@ JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetEncodeComp
     PG_CHECK(pg_parquet_encode_compressed((uint64_t)source, ptrs.data(), row0, nRows, &opt, codec, level, &h));
     return (jlong)h;
 }
-// The same rows as one ORC file: compression = ORC CompressionKind (0 NONE, 5 ZSTD), blockSize = orc.compress.size
-// (0 = 256 KiB); types = 4 ints per column (kind, precision, scale, max length; pg_orc_column_type), or null for the
-// kinds of the physical types.  The result is a file handle for fileMeta / fileFetch / fileFree like Parquet's.
-JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_orcEncode(JNIEnv *env, jclass, jlong source,
-                                                                         jobjectArray names, jlong row0, jlong nRows,
-                                                                         jlong stripeRows, jint compression, jint level,
-                                                                         jlong blockSize, jintArray types) {
-    std::vector<std::string> keep;
-    std::vector<const char *> ptrs = utf_names(env, names, keep);
+// types = 4 ints per column (kind, precision, scale, max length; pg_orc_column_type), or null for the kinds of the
+// physical types
+static std::vector<pg_orc_column_type> orc_types(JNIEnv *env, jintArray types) {
     std::vector<pg_orc_column_type> cols;
     if (types) {
         const jsize n = env->GetArrayLength(types);
@@ -306,9 +300,43 @@ JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_orcEncode(JNIEnv 
         env->GetIntArrayRegion(types, 0, n, v.data());
         for (jsize i = 0; i + 3 < n; i += 4) cols.push_back(pg_orc_column_type{v[i], v[i + 1], v[i + 2], v[i + 3]});
     }
+    return cols;
+}
+// The same rows as one ORC file: compression = ORC CompressionKind (0 NONE, 5 ZSTD), blockSize = orc.compress.size
+// (0 = 256 KiB); types as orc_types reads them.  The result is a file handle for fileMeta / fileFetch / fileFree like
+// Parquet's.
+JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_orcEncode(JNIEnv *env, jclass, jlong source,
+                                                                         jobjectArray names, jlong row0, jlong nRows,
+                                                                         jlong stripeRows, jint compression, jint level,
+                                                                         jlong blockSize, jintArray types) {
+    std::vector<std::string> keep;
+    std::vector<const char *> ptrs = utf_names(env, names, keep);
+    std::vector<pg_orc_column_type> cols = orc_types(env, types);
     pg_orc_write_options opt{stripeRows, compression, level, blockSize, types ? cols.data() : nullptr};
     uint64_t h = 0;
     PG_CHECK(pg_orc_encode((uint64_t)source, ptrs.data(), row0, nRows, &opt, &h));
+    return (jlong)h;
+}
+// orcEncode with a row index of rowIndexStride rows per row group (orc.row.index.stride; 0 = none) and bloom filters
+// of the file columns bloomColumns (orc.bloom.filter.columns, resolved to indexes; null = none) at bloomFpp
+// (orc.bloom.filter.fpp): pg_orc_encode_indexed.
+JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_orcEncodeIndexed(
+        JNIEnv *env, jclass, jlong source, jobjectArray names, jlong row0, jlong nRows, jlong stripeRows,
+        jint compression, jint level, jlong blockSize, jintArray types, jlong rowIndexStride, jintArray bloomColumns,
+        jdouble bloomFpp) {
+    std::vector<std::string> keep;
+    std::vector<const char *> ptrs = utf_names(env, names, keep);
+    std::vector<pg_orc_column_type> cols = orc_types(env, types);
+    pg_orc_write_options opt{stripeRows, compression, level, blockSize, types ? cols.data() : nullptr};
+    std::vector<jint> bloom;
+    if (bloomColumns) {
+        bloom.resize((size_t)env->GetArrayLength(bloomColumns));
+        env->GetIntArrayRegion(bloomColumns, 0, (jsize)bloom.size(), bloom.data());
+    }
+    std::vector<int32_t> bloom32(bloom.begin(), bloom.end());
+    pg_orc_index_options index{rowIndexStride, (int32_t)bloom32.size(), bloom32.data(), bloomFpp};
+    uint64_t h = 0;
+    PG_CHECK(pg_orc_encode_indexed((uint64_t)source, ptrs.data(), row0, nRows, &opt, &index, &h));
     return (jlong)h;
 }
 JNIEXPORT jlongArray JNICALL Java_org_apache_paimon_gpu_NativeMerge_fileMeta(JNIEnv *env, jclass, jlong file) {

@@ -96,6 +96,11 @@ class PgOrcWriteOptions(C.Structure):
                 ("compression_block_size", C.c_int64), ("types", C.POINTER(PgOrcColumnType))]
 
 
+class PgOrcIndexOptions(C.Structure):
+    _fields_ = [("row_index_stride", C.c_int64), ("n_bloom_columns", C.c_int32),
+                ("bloom_columns", C.POINTER(C.c_int32)), ("bloom_fpp", C.c_double)]
+
+
 class PgBloomFilterSpec(C.Structure):
     _fields_ = [("column", C.c_int32), ("items", C.c_int32), ("fpp", C.c_double)]
 
@@ -168,6 +173,9 @@ _SIGNATURES = {
                                                  C.POINTER(C.c_uint64)]),
     "pg_orc_encode": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,
                                   C.POINTER(PgOrcWriteOptions), C.POINTER(C.c_uint64)]),
+    "pg_orc_encode_indexed": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,
+                                          C.POINTER(PgOrcWriteOptions), C.POINTER(PgOrcIndexOptions),
+                                          C.POINTER(C.c_uint64)]),
     "pg_parquet_file_meta": (C.c_int32, [C.c_uint64, C.POINTER(PgFileMeta)]),
     "pg_parquet_file_column_stats": (C.c_int32, [C.c_uint64, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int32),
                                                  C.c_void_p, C.c_void_p]),

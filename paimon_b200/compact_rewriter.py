@@ -12,6 +12,7 @@ device; the host writes the encoded bytes through the FileIO and assembles the D
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence, Tuple
@@ -103,6 +104,66 @@ def orc_compression_for_level(options: Optional[Dict[str, object]], level: int) 
     return codec, zstd_level, int(options.get("orc.compress.size", 0))
 
 
+# orc-core's smallest row index stride (WriterImpl.MIN_ROW_INDEX_STRIDE), and the largest bloom filter the device
+# builds: the shared memory of one CTA (kBloomMaxBytes in orc_encode.cu)
+ORC_MIN_ROW_INDEX_STRIDE = 1000
+ORC_BLOOM_MAX_BYTES = 227 << 10
+
+
+def orc_bloom_bits(entries: int, fpp: float) -> int:
+    """The bits of an ORC bloom filter for `entries` values at `fpp`, as orc-core's BloomFilter sizes it."""
+    nb = int(-entries * math.log(fpp) / (math.log(2) ** 2))
+    return nb + 64 - nb % 64
+
+
+def orc_index_options(schema: KeyValueSchema, stride: int, bloom_columns: Sequence[str], fpp: float):
+    """pg_orc_index_options for a row index of `stride` rows per row group and bloom filters of the value fields
+    `bloom_columns`.  The refusals of pg_orc_encode_indexed are raised here, before any device work."""
+    stride, bloom_columns = int(stride), list(bloom_columns)
+    invalid = None
+    if stride < 0 or 0 < stride < ORC_MIN_ROW_INDEX_STRIDE:
+        invalid = f"row index stride {stride} is negative or below {ORC_MIN_ROW_INDEX_STRIDE}"
+    elif bloom_columns and stride == 0:
+        invalid = "bloom filters need a row index stride"
+    elif bloom_columns and not 0 < fpp < 1:
+        invalid = f"bloom filter fpp {fpp} outside (0, 1)"
+    elif len(set(bloom_columns)) != len(bloom_columns):
+        invalid = f"bloom filter columns {bloom_columns} list a column twice"
+    if invalid:
+        raise N.PaimonGpuError(1, f"orc encode: {invalid}")
+    if stride % 8:
+        raise N.UnsupportedOnDevice(2, f"orc encode: row index stride {stride} is not a multiple of 8")
+    by_name = {f.name: i for i, f in enumerate(schema.value_type.fields)}
+    cols = []
+    for name in bloom_columns:
+        if name not in by_name:
+            raise N.PaimonGpuError(1, f"orc encode: bloom filter column {name!r} is not a value field")
+        t = schema.value_type.fields[by_name[name]].type
+        if orc_column_type(t)[0] in (0, 14):                               # BOOLEAN, DECIMAL
+            raise N.UnsupportedOnDevice(2, f"orc encode: bloom filter column {name!r} is {t}")
+        cols.append(schema.n_key + 2 + by_name[name])
+    if cols and orc_bloom_bits(stride, fpp) // 8 > ORC_BLOOM_MAX_BYTES:
+        raise N.UnsupportedOnDevice(2, f"orc encode: a bloom filter of {stride} rows at fpp {fpp} is larger than "
+                                       f"{ORC_BLOOM_MAX_BYTES} bytes")
+    arr = (C.c_int32 * max(len(cols), 1))(*cols)
+    opts = N.PgOrcIndexOptions(stride, len(cols), arr, float(fpp))
+    opts._keep = arr
+    return opts
+
+
+def orc_index_for_level(options: Optional[Dict[str, object]]) -> Dict[str, object]:
+    """The row index arguments of KeyValueDataFileWriter for an ORC output level, from the table options as orc-core
+    reads them: 'orc.create.index' (default true), 'orc.row.index.stride' (default 10000), 'orc.bloom.filter.columns'
+    (comma-separated, no default) and 'orc.bloom.filter.fpp' (default 0.01) (OrcConf.java:57-67,140-201).  Without an
+    index there are no bloom filters either."""
+    options = options or {}
+    if str(options.get("orc.create.index", "true")).lower() != "true":
+        return dict(row_index_stride=0, bloom_filter_columns=())
+    cols = [c.strip() for c in str(options.get("orc.bloom.filter.columns", "")).split(",") if c.strip()]
+    return dict(row_index_stride=int(options.get("orc.row.index.stride", 10000)), bloom_filter_columns=tuple(cols),
+                bloom_filter_fpp=float(options.get("orc.bloom.filter.fpp", 0.01)))
+
+
 def file_column_names(schema: KeyValueSchema) -> List[str]:
     """[_KEY_*, _SEQUENCE_NUMBER, _VALUE_KIND, value...] (KeyValue.schema, KeyValue.java:130-138)."""
     return [f.name for f in schema.file_fields()]
@@ -118,12 +179,17 @@ class KeyValueDataFileWriter:
     the device over the rows of the file, as DataFileMeta.embedded_index or the side file of extra_files
     (KeyValueDataFileWriter.java:103-113,156-181); options the device cannot build are refused here, before any
     device work.  With `page_index` a Parquet file carries the ColumnIndex and OffsetIndex of every column chunk
-    (the page bounds computed on the device), as parquet-mr writes them; ORC files ignore it."""
+    (the page bounds computed on the device), as parquet-mr writes them; ORC files ignore it.  An ORC file takes
+    `row_index_stride` (rows per row group of its row index, 0 = none), `bloom_filter_columns` (value-field names
+    with a bloom filter per row group, built on the device) and `bloom_filter_fpp`, as orc-core writes them for
+    'orc.row.index.stride', 'orc.bloom.filter.columns' and 'orc.bloom.filter.fpp'; Parquet files ignore them.  Index
+    options the device cannot write are refused here, before any device work."""
 
     def __init__(self, schema: KeyValueSchema, path: str, level: int, file_io: Optional[LocalFileIO] = None,
                  row_group_rows: int = 0, page_rows: int = 0, compression: str = "none", zstd_level: int = 1,
                  file_format: str = "parquet", stripe_rows: int = 0, compression_block_size: int = 0,
-                 file_index: Optional[FileIndexOptions] = None, page_index: bool = False):
+                 file_index: Optional[FileIndexOptions] = None, page_index: bool = False,
+                 row_index_stride: int = 0, bloom_filter_columns: Sequence[str] = (), bloom_filter_fpp: float = 0.01):
         self.schema = schema
         self.path = path
         self.level = level
@@ -143,6 +209,7 @@ class KeyValueDataFileWriter:
                                                                    for f in fields])
             self.orc_opts = N.PgOrcWriteOptions(stripe_rows, self.codec, self.zstd_level, compression_block_size,
                                                 self._orc_types)
+            self.orc_index = orc_index_options(schema, row_index_stride, bloom_filter_columns, bloom_filter_fpp)
         self.index_writer = None
         if file_index is not None and not file_index.is_empty():
             self.index_writer = DataFileIndexWriter(schema, file_index)
@@ -153,7 +220,8 @@ class KeyValueDataFileWriter:
         arr = (C.c_char_p * len(names))(*[n.encode() for n in names])
         fh = C.c_uint64(0)
         if self.file_format == "orc":
-            N.check(self.lib.pg_orc_encode(source_handle, arr, row0, n_rows, C.byref(self.orc_opts), C.byref(fh)))
+            N.check(self.lib.pg_orc_encode_indexed(source_handle, arr, row0, n_rows, C.byref(self.orc_opts),
+                                                   C.byref(self.orc_index), C.byref(fh)))
         elif self.codec == 0:
             N.check(self.lib.pg_parquet_encode(source_handle, arr, row0, n_rows, C.byref(self.opts), C.byref(fh)))
         else:
@@ -248,12 +316,13 @@ class MergeTreeCompactRewriter:
     and the 'file-index.*' options give every file its bloom filters (refused before any device work when the device
     cannot build them); without, they are uncompressed Parquet (or the writer arguments' file_format).  With
     `page_index` the files of Parquet output levels carry the page index (ColumnIndex and OffsetIndex); ORC output
-    levels write no row indexes and ignore it."""
+    levels ignore it.  With `row_index` the files of ORC output levels carry a row index and bloom filters as the
+    table options ask for them (orc_index_for_level); Parquet output levels ignore it."""
 
     def __init__(self, schema: KeyValueSchema, mf_factory: MergeFunctionFactory, directory: str,
                  user_defined_seq_comparator=None, file_io: Optional[LocalFileIO] = None, device: int = 0,
                  target_file_rows: int = 4 << 20, options: Optional[Dict[str, object]] = None,
-                 page_index: bool = False, **writer_args):
+                 page_index: bool = False, row_index: bool = False, **writer_args):
         self.schema = schema
         self.mf_factory = mf_factory
         self.directory = directory
@@ -264,6 +333,7 @@ class MergeTreeCompactRewriter:
         self.target_file_rows = target_file_rows
         self.options = options
         self.page_index = page_index
+        self.row_index = row_index
         self.writer_args = writer_args
 
     def rewrite(self, output_level: int, drop_delete: bool, sections: Sequence[Sequence[SortedRun]]) -> CompactResult:
@@ -290,6 +360,10 @@ class MergeTreeCompactRewriter:
                 DataFileIndexWriter(self.schema, file_index)          # refuses before any device work
                 writer_args["file_index"] = file_index
         parquet = writer_args.get("file_format", "parquet").lower() == "parquet"
+        if self.row_index and not parquet:
+            writer_args.update(orc_index_for_level(self.options))
+            orc_index_options(self.schema, writer_args["row_index_stride"], writer_args["bloom_filter_columns"],
+                              writer_args.get("bloom_filter_fpp", 0.01))   # refuses before any device work
         rolling = RollingFileWriter(self.schema, self.directory, output_level, self.target_file_rows, self.file_io,
                                     prefix=f"compact-l{output_level}", page_index=self.page_index and parquet,
                                     **writer_args)

@@ -458,9 +458,41 @@ std::vector<uint8_t> compress_section(const std::vector<uint8_t> &raw, int codec
     return out;
 }
 
+std::vector<uint8_t> row_index(const OutType &t, const std::vector<std::vector<uint64_t>> &positions,
+                               const std::vector<ColumnStats> &stats) {
+    PbWriter w;
+    for (size_t e = 0; e < stats.size(); e++) {
+        PbWriter entry;
+        if (!positions[e].empty()) {
+            PbWriter packed;
+            for (uint64_t p : positions[e]) packed.varint(p);
+            entry.bytes(1, packed.b.data(), packed.b.size());
+        }
+        const std::vector<uint8_t> cs = column_statistics(t, stats[e]);
+        entry.bytes(2, cs.data(), cs.size());
+        w.msg(1, entry);
+    }
+    return std::move(w.b);
+}
+
+std::vector<uint8_t> bloom_filter_index(int k, const uint64_t *words, size_t n_words, size_t n_filters) {
+    PbWriter w;
+    std::vector<uint8_t> le(8 * n_words);
+    for (size_t f = 0; f < n_filters; f++) {
+        for (size_t i = 0; i < n_words; i++)
+            for (int b = 0; b < 8; b++) le[8 * i + b] = (uint8_t)(words[f * n_words + i] >> (8 * b));
+        PbWriter m;
+        m.u64(1, (uint64_t)k);
+        m.bytes(3, le.data(), le.size());
+        w.msg(1, m);
+    }
+    return std::move(w.b);
+}
+
 std::vector<uint8_t> file_tail(const std::vector<OutType> &types, const std::vector<std::string> &names,
                                const std::vector<OutStripe> &stripes, const std::vector<ColumnStats> &file_stats,
-                               uint64_t rows, uint64_t content_length, int codec, uint64_t block_size) {
+                               uint64_t rows, uint64_t content_length, int codec, uint64_t block_size,
+                               uint64_t row_index_stride) {
     std::vector<OutType> all(1);
     all[0].kind = K_STRUCT;
     all.insert(all.end(), types.begin(), types.end());
@@ -479,7 +511,7 @@ std::vector<uint8_t> file_tail(const std::vector<OutType> &types, const std::vec
     for (const OutStripe &s : stripes) {
         PbWriter m;
         m.u64(1, s.offset);
-        m.u64(2, 0);
+        m.u64(2, s.index_length);
         m.u64(3, s.data_length);
         m.u64(4, s.footer_length);
         m.u64(5, s.rows);
@@ -503,7 +535,7 @@ std::vector<uint8_t> file_tail(const std::vector<OutType> &types, const std::vec
         const std::vector<uint8_t> cs = column_statistics(all[c], file_stats[c]);
         f.bytes(7, cs.data(), cs.size());
     }
-    f.u64(8, 0);                                         // rowIndexStride: no row indexes
+    f.u64(8, row_index_stride);                          // rowIndexStride, 0 = no row indexes
     const std::vector<uint8_t> meta_c = compress_section(meta.b, codec, block_size);
     const std::vector<uint8_t> foot_c = compress_section(f.b, codec, block_size);
     PbWriter ps;                                         // PostScript

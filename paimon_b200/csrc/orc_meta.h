@@ -111,8 +111,8 @@ Plan plan_file(const FileTail &t, int64_t size, const std::vector<int> &file_col
 // host builds of the decode path.
 Plan plan_file(const FileTail &t, const uint8_t *file, int64_t size, const std::vector<int> &file_col_of);
 
-// ---- writer side: the stripe footers and the file tail (Metadata, Footer, PostScript, PostScript length) of a flat
-// file, written DIRECT / DIRECT_V2 without row indexes
+// ---- writer side: the stripe footers, the row index sections and the file tail (Metadata, Footer, PostScript,
+// PostScript length) of a flat file, written DIRECT / DIRECT_V2
 struct PbWriter {
     std::vector<uint8_t> b;
     void varint(uint64_t v);
@@ -147,7 +147,7 @@ struct OutStream {
     uint64_t length = 0;
 };
 struct OutStripe {
-    uint64_t offset = 0, data_length = 0, footer_length = 0, rows = 0;
+    uint64_t offset = 0, index_length = 0, data_length = 0, footer_length = 0, rows = 0;
     std::vector<ColumnStats> stats;   // [0] = the root struct
 };
 
@@ -160,10 +160,18 @@ std::vector<uint8_t> stripe_footer(const std::vector<OutStream> &streams, const 
 // a section stored under the file's compression: NONE = the bytes; ZSTD = chunks of at most block_size bytes, each one
 // zstd frame behind a 3-byte header, or the original bytes when the frame is not smaller
 std::vector<uint8_t> compress_section(const std::vector<uint8_t> &raw, int codec, uint64_t block_size);
+// a RowIndex: per row group an entry with its positions (none: the field is left out) and its statistics
+std::vector<uint8_t> row_index(const OutType &t, const std::vector<std::vector<uint64_t>> &positions,
+                               const std::vector<ColumnStats> &stats);
+// a BloomFilterIndex of n_filters BLOOM_FILTER_UTF8 filters of k hash functions, filter f the 64-bit little-endian
+// words [f * n_words, (f + 1) * n_words)
+std::vector<uint8_t> bloom_filter_index(int k, const uint64_t *words, size_t n_words, size_t n_filters);
 // Metadata, Footer, PostScript and its length byte.  types / names: the columns (the root struct is added);
-// file_stats[0] = the root; content_length: the bytes in front of the Metadata ("ORC" and the stripes)
+// file_stats[0] = the root; content_length: the bytes in front of the Metadata ("ORC" and the stripes);
+// row_index_stride: 0 = no row index
 std::vector<uint8_t> file_tail(const std::vector<OutType> &types, const std::vector<std::string> &names,
                                const std::vector<OutStripe> &stripes, const std::vector<ColumnStats> &file_stats,
-                               uint64_t rows, uint64_t content_length, int codec, uint64_t block_size);
+                               uint64_t rows, uint64_t content_length, int codec, uint64_t block_size,
+                               uint64_t row_index_stride = 0);
 
 }  // namespace orc

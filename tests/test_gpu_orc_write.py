@@ -23,7 +23,7 @@ from paimon_b200.merge_tree_readers import DataFileMeta, IntervalPartition, Merg
 from paimon_b200.sort_merge_reader import SortedRunReader, SortMergeReader, _SchemaHandle
 from paimon_b200.types import DataField, KeyValueSchema, RowType, is_varlen, orc_column_type
 
-from parquet_util import write_kv_parquet
+from parquet_util import arrow_to_column, write_kv_parquet
 
 pytestmark = pytest.mark.gpu
 
@@ -60,10 +60,11 @@ def orc_table_to_batch(schema, table):
         arr = table.column(name).combine_chunks()
         if pa.types.is_date32(arr.type):
             arr = arr.cast(pa.int32())
-        vals = arr.to_pylist()
         if pa.types.is_decimal(arr.type):
-            vals = [None if v is None else int(v.scaleb(arr.type.scale)) for v in vals]
-        cols.append(Column.from_pylist(f.physical, vals))
+            vals = [None if v is None else int(v.scaleb(arr.type.scale)) for v in arr.to_pylist()]
+            cols.append(Column.from_pylist(f.physical, vals))
+        else:
+            cols.append(arrow_to_column(f.physical, arr))
     return KeyValueBatch(schema, cols)
 
 

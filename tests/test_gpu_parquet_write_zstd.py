@@ -1,6 +1,7 @@
 """zstd-compressed compaction output on the device (pg_parquet_encode_compressed, codec 6): the files read back with
 pyarrow and with the device decoder, their footers carry ZSTD and both size totals, every frame decompresses on the
-host to the body the uncompressed encode writes for that page, the bytes are deterministic, codec 0 is the
+host to the body the uncompressed encode writes for that page and equals the frame the host build of the encoder
+writes for that body, the bytes are deterministic, codec 0 is the
 uncompressed encode, the refusals, the rewriter's per-level codec choice, and the ratio against libzstd level 1."""
 import ctypes as C
 import random
@@ -23,6 +24,7 @@ from paimon_b200.types import DataField, KeyValueSchema, RowType
 
 from parquet_util import arrow_to_batch, write_kv_parquet
 from test_gpu_parquet_write import all_types_schema, random_rows
+from test_zstd_encode_cpu import compress, zse  # noqa: F401  (zse: the host build of the encoder, a fixture)
 
 pytestmark = pytest.mark.gpu
 
@@ -111,8 +113,9 @@ def pages_of(file_bytes):
     return out
 
 
-def check_against_uncompressed(schema, batch, path, **writer_args):
-    """The zstd encode against the uncompressed one of the same batch; returns the zstd file's metadata."""
+def check_against_uncompressed(schema, batch, path, zse, **writer_args):
+    """The zstd encode against the uncompressed one of the same batch; returns the zstd file's metadata.  `zse` is
+    the host build of the frame encoder (test_zstd_encode_cpu): every device frame must equal its frame."""
     raw, raw_meta = encode(schema, batch, None, **writer_args)
     z, z_meta = encode(schema, batch, 6, **writer_args)
     z2, _ = encode(schema, batch, 6, **writer_args)
@@ -128,6 +131,7 @@ def check_against_uncompressed(schema, batch, path, **writer_args):
     for (ru, rbody), (zu, frame) in zip(rp, zp):
         assert ru == zu == len(rbody)
         assert ZSTD.decompress(frame, decompressed_size=zu, asbytes=True) == rbody
+        assert compress(zse, rbody) == frame                        # the host build writes the same bytes
         assert len(frame) <= len(rbody) + 6 + 8 + 3 * (len(rbody) // (128 << 10) + 1)
     # metadata: codec, both totals, statistics identical to the uncompressed file's
     zm, rm = pq.ParquetFile(path).metadata, pq.ParquetFile(pa.BufferReader(raw)).metadata
@@ -156,10 +160,10 @@ def check_against_uncompressed(schema, batch, path, **writer_args):
 
 @pytest.mark.parametrize("n", [0, 1, 7, 8, 9, 255, 1000, 4097])
 @pytest.mark.parametrize("writer_args", [dict(), dict(page_rows=64, row_group_rows=256)])
-def test_pyarrow_reads_zstd_pages_the_device_writes(tmp_path, n, writer_args):
+def test_pyarrow_reads_zstd_pages_the_device_writes(tmp_path, zse, n, writer_args):
     schema = all_types_schema()
     batch = KeyValueBatch.from_rows(schema, random_rows(random.Random(n + 17), n))
-    check_against_uncompressed(schema, batch, str(tmp_path / "z.parquet"), **writer_args)
+    check_against_uncompressed(schema, batch, str(tmp_path / "z.parquet"), zse, **writer_args)
 
 
 def _bulk_schema():
@@ -182,11 +186,11 @@ def _bulk_table(schema, n, seed):
     return pa.Table.from_arrays(cols, schema=pa.schema(fields))
 
 
-def test_large_pages_many_blocks_per_frame(tmp_path):
+def test_large_pages_many_blocks_per_frame(tmp_path, zse):
     """8-byte pages over 128 KiB, multi-MiB string pages (many blocks per frame), all-NULL and BOOLEAN pages."""
     schema = _bulk_schema()
     batch = arrow_to_batch(schema, _bulk_table(schema, 300_000, 1))
-    z = check_against_uncompressed(schema, batch, str(tmp_path / "big.parquet"), page_rows=150_000)
+    z = check_against_uncompressed(schema, batch, str(tmp_path / "big.parquet"), zse, page_rows=150_000)
     sizes = [u for u, _ in pages_of(z)]
     assert max(sizes) > 2 << 20 and sum(1 for s in sizes if s > 128 << 10) >= 8
 

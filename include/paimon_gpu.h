@@ -196,7 +196,9 @@ pg_status pg_merge_spec_free(uint64_t spec);
  * freed after the call).  PG_MEM_DEVICE: the pointers are device pointers that the caller keeps
  * alive until pg_run_free and until no merge or view uses the run any more; every buffer must be 16-byte aligned and
  * readable up to the next multiple of 16 bytes (true for any cudaMalloc'ed / framework-allocated buffer): the kernels
- * stage column segments with 16-byte bulk async copies. */
+ * stage column segments with 16-byte bulk async copies.  Var-len offsets may start anywhere, in both memory kinds (a
+ * slice of a longer column): `data` is byte 0 of the offsets' space, the run's payload is [offsets[0], offsets[n_rows]),
+ * and offsets that decrease from offsets[0] to offsets[n_rows] are refused with PG_ERR_INVALID. */
 pg_status pg_run_open(uint64_t schema, const pg_run_desc *run, int32_t mem, uint64_t *out_run);
 pg_status pg_run_free(uint64_t run);
 

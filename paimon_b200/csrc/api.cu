@@ -1166,9 +1166,13 @@ pg_status pg_run_open(uint64_t schema, const pg_run_desc *desc, int32_t mem, uin
             run->cols[c] = DevColumn{pc.data, pc.offsets, pc.validity};
             if (is_varlen(s->field(c).type) && n > 0) {
                 if (!pc.offsets) return fail(PG_ERR_INVALID, "var-len column without offsets");
-                int32_t last = 0;
-                PG_CUDA(cudaMemcpy(&last, pc.offsets + n, sizeof(int32_t), cudaMemcpyDeviceToHost));
-                run->varlen_bytes[c] = last;
+                // offsets may start anywhere, `data` is byte 0 of their space: one read of offsets[0] and offsets[n]
+                int32_t b[2] = {0, 0};
+                PG_CUDA(cudaMemcpy2D(b, sizeof(int32_t), pc.offsets, sizeof(int32_t) * (size_t)n, sizeof(int32_t), 2,
+                                     cudaMemcpyDeviceToHost));
+                if (b[1] < b[0]) return fail(PG_ERR_INVALID, "decreasing offsets");
+                run->varlen_base[c] = b[0];
+                run->varlen_bytes[c] = b[1] - b[0];
             }
         }
     } else if (mem == PG_MEM_HOST) {

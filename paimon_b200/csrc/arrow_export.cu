@@ -86,7 +86,9 @@ static pg_status export_arrow(uint64_t source, const char *const *names, int64_t
     }
     const int nc = (int)present.size();
     auto field_of = [&](int i) { return s->field(present[i]); };
-    const int64_t lo = row0 & ~(int64_t)7;              // validity bitmaps are byte-granular
+    // validity bitmaps are byte-granular; an empty range starts at row0 itself: an importer sizes a var-len child's
+    // payload from offsets[offset + length] but slices it from offsets[offset], so no rows must mean no offset either
+    const int64_t lo = n_rows > 0 ? row0 & ~(int64_t)7 : row0;
     const int64_t delta = row0 - lo, m = n_rows + delta; // rows copied per column; children carry offset = delta
     auto pad = [](size_t b) { return (b + 63) & ~(size_t)63; };
 

@@ -55,6 +55,26 @@ def test_functions_have_the_bench_syntax_tree(name):
     assert ast.dump(ours) == ast.dump(function(bench_tree(), name))
 
 
+@pytest.mark.parametrize("name", ["_splitmix64", "_hex_keys", "gen_device_run"])
+def test_device_generator_has_the_bench_syntax_tree(name):
+    """tests/device_runs.py restates the generator of the bench's C2, C3 and C4 inputs."""
+    import device_runs
+    ours = ast.parse(inspect.getsource(getattr(device_runs, name))).body[0]
+    assert ast.dump(ours) == ast.dump(function(bench_tree(), name))
+
+
+def test_an_edited_generator_is_noticed(tmp_path):
+    """A bench.py whose generator draws string lengths from another range no longer matches the restatement."""
+    import device_runs
+    with open(os.path.join(ROOT, "bench.py")) as f:
+        src = f.read()
+    assert "lens = 8 + ((h >> 3) & 0xffff) % 17" in src
+    moved = tmp_path / "bench.py"
+    moved.write_text(src.replace("lens = 8 + ((h >> 3) & 0xffff) % 17", "lens = 8 + ((h >> 3) & 0xffff) % 16", 1))
+    ours = ast.parse(inspect.getsource(device_runs.gen_device_run)).body[0]
+    assert ast.dump(ours) != ast.dump(function(bench_tree(str(moved)), "gen_device_run"))
+
+
 @pytest.mark.parametrize("codec", ["none", "zstd"])
 def test_c5_writer_arguments(codec):
     calls = [n for n in ast.walk(function(bench_tree(), "c5_bucket"))

@@ -714,6 +714,7 @@ static pg_status execute(Merge *m) {
     pg_status st = ensure_device();
     if (st) return st;
     cudaStream_t sm = m->stream;
+    PG_HOST_MARKS("merge execute");
     free_outputs(m);
     for (size_t r = m->runs.size(); r < m->bound.size(); r++)     // a re-execute takes the merged runs back
         if (!m->runs.emplace_back(m->bound[r].lock())) {
@@ -853,6 +854,7 @@ static pg_status execute(Merge *m) {
     launch_scan(sm, tile_rows, T, row_base, m->d_totals);
     launches += 2;
     PG_CUDA(cudaEventRecord(m->ev[2], sm));
+    PG_HOST_MARK("enqueue");
     {
         SmallReads rb(sm);                   // the one size read-back: output buffers are sized exactly
         pg_status rs = rb.add(m->h_totals, m->d_totals, sizeof(int64_t));
@@ -861,6 +863,7 @@ static pg_status execute(Merge *m) {
         if (rs) return rs;
     }
     if (*m->h_err != KERR_NONE) return kernel_error(*m->h_err, "merge");
+    PG_HOST_MARK("size_readback");
 
     // ---- output buffers
     const int64_t n_out = m->h_totals[0];
@@ -949,6 +952,7 @@ static pg_status execute(Merge *m) {
     launch_emit(ea);
     launches++;
     PG_CUDA(cudaEventRecord(m->ev[3], sm));
+    PG_HOST_MARK("alloc_emit");
     {
         SmallReads rb(sm);
         pg_status rs = rb.add(m->h_err, m->d_err, sizeof(int32_t));
@@ -957,6 +961,7 @@ static pg_status execute(Merge *m) {
         if (rs) return rs;
     }
     PG_CUDA(cudaGetLastError());
+    PG_HOST_MARK("emit_readback");
     m->has_batch = true;
     if (*m->h_err != KERR_NONE) {
         free_outputs(m);
@@ -1394,9 +1399,13 @@ pg_status pg_merge_rebind(uint64_t merge, const uint64_t *runs, int32_t k, const
     if (k < 0 || k > PG_MAX_RUNS) return fail(PG_ERR_INVALID, "bad run count");
     pg_status st = ensure_device();
     if (st) return st;
+    PG_HOST_MARKS("merge rebind");
     PG_CUDA(cudaStreamSynchronize(m->stream));
     free_outputs(m.get());
-    return bind_runs(m.get(), runs, k, start_rows);
+    PG_HOST_MARK("sync");
+    st = bind_runs(m.get(), runs, k, start_rows);
+    PG_HOST_MARK("bind");
+    return st;
 }
 
 pg_status pg_merge_execute(uint64_t merge) {

@@ -1472,45 +1472,33 @@ static void walk_timing_dump() {
 }
 #endif
 
-// The value walk and the expansion.  With var-len columns, the value walk (one lane per page: latency-bound at low
-// occupancy) and the PLAIN BYTE_ARRAY pages that need it run on a side stream beside the expansion of all other pages.
-static pg_status expand_pages(cudaStream_t sm, bool byte_arrays, PqPage *d_pages, int np, const PqPage *d_dicts,
-                              const PqChunk *d_chunks, const PqOut *d_outs, int nc, const int32_t *d_ids, int32_t *d_vstart,
-                              const int32_t *d_dict_off, const int32_t *d_dict_len, int32_t *d_err, int *launches) {
-    if (!byte_arrays) {
-        k_pq_expand<false><<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart,
-                                                       d_dict_off, d_dict_len);
-        (*launches)++;
-        return PG_OK;
-    }
-    static thread_local cudaStream_t side = nullptr;
-    static thread_local cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    if (!side) {
-        // (highest priority: its few, long-running CTAs must get their slots before the expansion's 250 k short
-        // ones fill every SM — otherwise the walk only starts when the expansion drains)
+// The side stream of the calling thread's decodes, and its fork / join events.  Highest priority: the value walk's few,
+// long-running CTAs must get their slots before the expansion's 250 k short ones fill every SM — otherwise the walk
+// only starts when the expansion drains.
+struct SideStream {
+    cudaStream_t s = nullptr;
+    cudaEvent_t fork = nullptr, tables = nullptr, join = nullptr;
+};
+static pg_status side_stream(SideStream **out) {
+    static thread_local SideStream side;
+    if (!side.s) {
         int prio_lo = 0, prio_hi = 0;
         cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-        PG_CUDA(cudaStreamCreateWithPriority(&side, cudaStreamNonBlocking, prio_hi));
-        PG_CUDA(cudaEventCreateWithFlags(&ev_fork, cudaEventDisableTiming));
-        PG_CUDA(cudaEventCreateWithFlags(&ev_join, cudaEventDisableTiming));
+        PG_CUDA(cudaStreamCreateWithPriority(&side.s, cudaStreamNonBlocking, prio_hi));
+        PG_CUDA(cudaEventCreateWithFlags(&side.fork, cudaEventDisableTiming));
+        PG_CUDA(cudaEventCreateWithFlags(&side.tables, cudaEventDisableTiming));
+        PG_CUDA(cudaEventCreateWithFlags(&side.join, cudaEventDisableTiming));
     }
-    PG_CUDA(cudaEventRecord(ev_fork, sm));
-    PG_CUDA(cudaStreamWaitEvent(side, ev_fork, 0));
-    k_pq_walk_values<<<(np + kWvWarps * 32 - 1) / (kWvWarps * 32), kWvWarps * 32, 0, side>>>(
-        d_pages, np, d_chunks, d_vstart, d_err);
-    // the PLAIN BYTE_ARRAY pages follow their walk on the side stream; everything else expands on the main one
-    k_pq_expand<true><<<np, kExpThreads, 0, side>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                                    d_dict_len);
-    PG_CUDA(cudaEventRecord(ev_join, side));
-    k_pq_expand<false><<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                                   d_dict_len);
-    PG_CUDA(cudaStreamWaitEvent(sm, ev_join, 0));
-#ifdef PG_WALK_TIMING
-    walk_timing_dump();
-#endif
-    *launches += 3;
+    *out = &side;
     return PG_OK;
 }
+
+// Synchronises the side stream when a decode returns, before the frame's Scratch synchronises the main stream and
+// gives the buffers back: an error found by read-back 2 returns while the value walk may still run there.
+struct SideSync {
+    cudaStream_t s = nullptr;
+    ~SideSync() { if (s) cudaStreamSynchronize(s); }
+};
 
 // footer0: the footer of files[0], already parsed (the single-file reader), or NULL
 static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg_file_desc *files, int nf, int n_runs,
@@ -1518,6 +1506,8 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
                                 pg_section_info *info, const pq::FileMetaData *footer0 = nullptr) {
     const int nc = s->n_cols();
     SectionFrame fr(s, n_runs, "parquet");
+    SideSync side_sync;                                  // (destroyed before fr: the side stream first)
+    PG_HOST_MARKS("parquet decode_section");
     RunBuilder &b = fr.b;
     cudaStream_t sm = fr.stream;
     { pg_status st = fr.start(read_cols, names); if (st) return st; }
@@ -1541,6 +1531,7 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
     } catch (const std::exception &e) {
         return rd.st ? rd.st : fail(PG_ERR_FORMAT, e.what());
     }
+    PG_HOST_MARK("footers");
     std::vector<uint8_t> any_optional(nc, 0);
     for (int f = 0; f < nf; f++) {
         pg_status st = map_file_schema(b, *meta[f], files[f].run);
@@ -1554,6 +1545,7 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
     ChunkTables ct;
     { pg_status st = build_chunk_tables(s.get(), files, fr.d_file, meta, b, ct); if (st) return st; }
     const int n_chunks = (int)ct.chunks.size(), n_pairs = (int)ct.pairs.size();
+    PG_HOST_MARK("chunk_tables");
 
     // ---- output columns (the rows of files that lack a column stay NULL and get defined contents)
     { pg_status st = b.alloc(any_optional, b.missing); if (st) return st; }
@@ -1572,12 +1564,14 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
     const size_t tb_outs = align256(sizeof(PqOut) * outs.size());
     const size_t tb_pairs = align256(sizeof(PqPair) * (size_t)std::max(n_pairs, 1));
     const size_t tb_tot = align256(sizeof(int64_t) * (size_t)(8 + n_pairs));
-    unsigned char *tb = (unsigned char *)fr.scratch.take(tb_chunks + tb_outs + tb_pairs + tb_tot + 256);
-    if (!tb) return oom("parquet", "the chunk tables", tb_chunks + tb_outs + tb_pairs + tb_tot);
+    // (two output tables: the second one adds the var-len payload pointers, known only after read-back 2)
+    unsigned char *tb = (unsigned char *)fr.scratch.take(tb_chunks + 2 * tb_outs + tb_pairs + tb_tot + 256);
+    if (!tb) return oom("parquet", "the chunk tables", tb_chunks + 2 * tb_outs + tb_pairs + tb_tot);
     PqChunk *d_chunks = (PqChunk *)tb;
     PqOut *d_outs = (PqOut *)(tb + tb_chunks);
-    PqPair *d_pairs = (PqPair *)(tb + tb_chunks + tb_outs);
-    int64_t *d_totals = (int64_t *)(tb + tb_chunks + tb_outs + tb_pairs);      // [0..5] chunk totals, [8..] pair totals
+    PqOut *d_outs2 = (PqOut *)(tb + tb_chunks + tb_outs);
+    PqPair *d_pairs = (PqPair *)(tb + tb_chunks + 2 * tb_outs);
+    int64_t *d_totals = (int64_t *)(tb + tb_chunks + 2 * tb_outs + tb_pairs);  // [0..5] chunk totals, [8..] pair totals
     int32_t *d_err = (int32_t *)(d_totals + 6);
     PG_CUDA(cudaMemsetAsync(d_totals, 0, tb_tot, sm));
     // (tables go through small_h2d: a kernel reads them out of mapped host memory, so they do not queue behind an
@@ -1586,6 +1580,7 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
     { pg_status ts = small_h2d(d_outs, outs.data(), sizeof(PqOut) * outs.size(), sm); if (ts) return ts; }
     if (n_pairs) { pg_status ts = small_h2d(d_pairs, ct.pairs.data(), sizeof(PqPair) * n_pairs, sm); if (ts) return ts; }
     int64_t h_tot[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    PG_HOST_MARK("tables");
     if (n_chunks) {
         k_pq_walk<false><<<(n_chunks + 63) / 64, 64, 0, sm>>>(d_chunks, n_chunks, nullptr, nullptr, nullptr, d_err);
         k_pq_chunk_scan<<<1, kScanThreads, 0, sm>>>(d_chunks, n_chunks, d_totals);
@@ -1601,6 +1596,7 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
     const int64_t n_pages = h_tot[0], n_dicts = h_tot[1], sc_bytes = h_tot[2], dict_entries = h_tot[3],
                   ids_entries = h_tot[4];
     fr.page_bytes = h_tot[5];
+    PG_HOST_MARK("readback1");
     if (n_pages > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet: too many pages in one section");
 
     // ---- page table + scratch, fill pass, inflate
@@ -1657,34 +1653,86 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
         if (n_pairs) {
             k_pq_scan_pages<<<(n_pairs * 32 + 127) / 128, 128, 0, sm>>>(d_pages, d_chunks, d_pairs, n_pairs, d_totals + 8, d_err);
             fr.launches++;
-            {
-                SmallReads rb(sm);                       // read-back 2: exact payload sizes of the var-len columns
-                pg_status rs = rb.add(pair_tot.data(), d_totals + 8, sizeof(int64_t) * n_pairs);
-                if (!rs) rs = rb.add(h_tot, d_totals, sizeof(int64_t) * 8);
-                if (!rs) rs = rb.finish();
-                if (!rs) rs = kernel_error((int)(h_tot[6] & 0xffffffff), "parquet");
-                if (rs) return rs;
-            }
         }
     }
 
-    // ---- var-len payload buffers (one per run), then the value walk and the expansion
-    if (n_pairs) {
+    // ---- the value walk and the expansion.  With var-len columns the value walk (one lane per page: latency-bound at
+    // low occupancy) and the PLAIN BYTE_ARRAY pages that need it run on a side stream beside the expansion of all other
+    // pages.  Read-back 2 (the exact payload sizes) is issued first, and the walk and the main-stream expansion are
+    // enqueued before the host waits for it: neither needs the payload buffers, so the device keeps working through
+    // the wait, the payload allocation and the upload of the second output table.  Only dictionary-encoded strings,
+    // which the main-stream expansion copies, make it wait for the payload buffers.
+    if (n_pairs == 0) {
+        if (np > 0) {
+            k_pq_expand<false><<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart,
+                                                           d_dict_off, d_dict_len);
+            fr.launches++;
+        }
+    } else {
+        SmallReads rb(sm);                               // read-back 2: exact payload sizes of the var-len columns
+        pg_status rs = rb.add(pair_tot.data(), d_totals + 8, sizeof(int64_t) * n_pairs);
+        if (!rs) rs = rb.add(h_tot, d_totals, sizeof(int64_t) * 8);
+        if (rs) return rs;
+        SideStream *side = nullptr;
+        { pg_status st = side_stream(&side); if (st) return st; }
+        side_sync.s = side->s;
+        PG_CUDA(cudaEventRecord(side->fork, sm));        // (behind read-back 2: its event)
+        const bool main_early = dict_entries == 0;
+        if (np > 0) {
+            PG_CUDA(cudaStreamWaitEvent(side->s, side->fork, 0));
+            k_pq_walk_values<<<(np + kWvWarps * 32 - 1) / (kWvWarps * 32), kWvWarps * 32, 0, side->s>>>(
+                d_pages, np, d_chunks, d_vstart, d_err);
+            fr.launches++;
+            if (main_early) {
+                k_pq_expand<false><<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart,
+                                                               d_dict_off, d_dict_len);
+                fr.launches++;
+            }
+        }
+        PG_HOST_MARK("enqueue");
+        rs = rb.finish(side->fork);
+        if (!rs) rs = kernel_error((int)(h_tot[6] & 0xffffffff), "parquet");
+        if (rs) return rs;
+        PG_HOST_MARK("readback2");
+        // ---- var-len payload buffers (one per run), in a second output table: the first one is being read
         std::vector<int64_t> payload((size_t)n_runs * nc, 0);
         for (const PqPair &pr : ct.pairs) payload[(size_t)pr.run * nc + pr.col] = pair_tot[pr.idx];
         { pg_status st = b.alloc_payload(payload); if (st) return st; }
         fill_outs();
-        { pg_status ts = small_h2d(d_outs, outs.data(), sizeof(PqOut) * outs.size(), sm); if (ts) return ts; }
-    }
-    if (np > 0) {
-        pg_status st = expand_pages(sm, n_pairs > 0, d_pages, np, d_dicts, d_chunks, d_outs, nc, d_ids, d_vstart, d_dict_off,
-                                    d_dict_len, d_err, &fr.launches);
-        if (st) return st;
+        if (main_early) {
+            pg_status ts = small_h2d(d_outs2, outs.data(), sizeof(PqOut) * outs.size(), side->s);
+            if (ts) return ts;
+        } else {
+            pg_status ts = small_h2d(d_outs2, outs.data(), sizeof(PqOut) * outs.size(), sm);
+            if (ts) return ts;
+            PG_CUDA(cudaEventRecord(side->tables, sm));
+            PG_CUDA(cudaStreamWaitEvent(side->s, side->tables, 0));
+            if (np > 0) {
+                k_pq_expand<false><<<np, kExpThreads, 0, sm>>>(d_pages, d_dicts, d_chunks, d_outs2, nc, d_ids, d_vstart,
+                                                               d_dict_off, d_dict_len);
+                fr.launches++;
+            }
+        }
+        if (np > 0) {
+            // the PLAIN BYTE_ARRAY pages follow their walk on the side stream
+            k_pq_expand<true><<<np, kExpThreads, 0, side->s>>>(d_pages, d_dicts, d_chunks, d_outs2, nc, d_ids, d_vstart,
+                                                               d_dict_off, d_dict_len);
+            fr.launches++;
+        }
+        PG_CUDA(cudaEventRecord(side->join, side->s));
+        PG_CUDA(cudaStreamWaitEvent(sm, side->join, 0));
+#ifdef PG_WALK_TIMING
+        if (np > 0) walk_timing_dump();
+#endif
+        PG_HOST_MARK("payload");
     }
     if (any_empty && n_pairs) {
         k_pq_zero_first_offset<<<(n_runs * nc + 127) / 128, 128, 0, sm>>>(d_outs, n_runs * nc);
         fr.launches++;
     }
+    // (the parsed footers go while the expansions run, not between the decode and the merge that follows it)
+    meta.clear();
+    std::vector<pq::FileMetaData>().swap(own_meta);
     { pg_status st = fr.finish(d_err, out_runs, info); if (st) return st; }
     if (info) {
         info->n_chunks = n_chunks;

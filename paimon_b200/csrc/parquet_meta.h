@@ -74,6 +74,13 @@ FileMetaData parse_footer(const uint8_t *file, int64_t size);
 // the last 8 bytes of every file ([footer length:4 LE]["PAR1"]), then every footer.  No range is queued before it is
 // checked against its file.  Unlike parse_footer, the leading "PAR1" is not read.
 std::vector<FileMetaData> read_footers(RangeReader &rd, const std::vector<uint64_t> &sizes);
+// The Thrift footers (without length and magic) of several files, in order.  Throws the error of the first malformed
+// footer in the order given.
+struct FooterBytes {
+    const uint8_t *bytes;
+    int64_t size;
+};
+std::vector<FileMetaData> parse_footers(const std::vector<FooterBytes> &footers);
 
 inline void put_varint(std::vector<uint8_t> &b, uint64_t v) {
     while (v >= 0x80) { b.push_back((uint8_t)(v | 0x80)); v >>= 7; }

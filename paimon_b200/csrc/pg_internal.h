@@ -3,7 +3,9 @@
 
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include <stdio.h>
 
+#include <chrono>
 #include <memory>
 #include <mutex>
 #include <string>
@@ -218,6 +220,33 @@ struct RunBuilder {
     std::vector<OutColumn> out;
     int64_t decoded_bytes = 0;       // validity (n + 7) / 8, values n * width, offsets 4 (n + 1), payload bytes
 };
+
+// Host phase times of a call, in a timing build only (EXTRA_DEFS=-DPG_HOST_TIMING; compiled out by default): a call
+// opens PG_HOST_MARKS(who), marks the end of each host phase with PG_HOST_MARK(phase), and prints on return one line
+// "[host timing] <who>: <phase> <ms> ..." to stderr, so that each idle gap of a device trace has a named host phase.
+#ifdef PG_HOST_TIMING
+struct HostMarks {
+    explicit HostMarks(const char *who) : who(who), t0(std::chrono::steady_clock::now()), last(t0) {}
+    void mark(const char *phase) {
+        const auto t = std::chrono::steady_clock::now();
+        line += std::string(" ") + phase + " " + std::to_string(std::chrono::duration<double, std::milli>(t - last).count());
+        last = t;
+    }
+    ~HostMarks() {
+        mark("rest");
+        fprintf(stderr, "[host timing] %s:%s total %.4f\n", who, line.c_str(),
+                std::chrono::duration<double, std::milli>(last - t0).count());
+    }
+    const char *who;
+    std::chrono::steady_clock::time_point t0, last;
+    std::string line;
+};
+#define PG_HOST_MARKS(who) pg::HostMarks pg_host_marks_(who)
+#define PG_HOST_MARK(phase) pg_host_marks_.mark(phase)
+#else
+#define PG_HOST_MARKS(who) do {} while (0)
+#define PG_HOST_MARK(phase) do {} while (0)
+#endif
 
 // the two events ms_decode is measured between
 struct SectionTimer {
@@ -480,14 +509,16 @@ void launch_emit(const EmitArgs &ea);
 
 // readback.cu: small device -> host reads through device-mapped page-locked memory (a kernel stores them), so that
 // they do not queue behind another thread's large copies on the device -> host copy engine.  add() enqueues on the
-// stream, finish() synchronises the stream and delivers the bytes.  One object per synchronisation point, per thread.
+// stream, finish() synchronises the stream and delivers the bytes.  finish(ev) waits for an event the caller recorded on
+// the stream behind the last add() instead, so that work enqueued after it keeps the device busy meanwhile.  One object
+// per synchronisation point, per thread.
 pg_status small_h2d(void *dev_dst, const void *host_src, size_t n, cudaStream_t stream);   // tables / descriptors
 
 class SmallReads {
  public:
     explicit SmallReads(cudaStream_t s) : stream_(s) {}
     pg_status add(void *host_dst, const void *dev_src, size_t n);
-    pg_status finish();
+    pg_status finish(cudaEvent_t after = nullptr);
 
  private:
     struct Item { void *dst; size_t off, n; };

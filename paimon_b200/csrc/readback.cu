@@ -102,8 +102,9 @@ pg_status SmallReads::add(void *host_dst, const void *dev_src, size_t n) {
     return PG_OK;
 }
 
-pg_status SmallReads::finish() {
-    PG_CUDA(cudaStreamSynchronize(stream_));
+pg_status SmallReads::finish(cudaEvent_t after) {
+    if (after) PG_CUDA(cudaEventSynchronize(after));
+    else PG_CUDA(cudaStreamSynchronize(stream_));
     for (const Item &it : items_) memcpy(it.dst, g_stage.h + it.off, it.n);
     items_.clear();
     used_ = 0;

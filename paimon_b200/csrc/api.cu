@@ -24,12 +24,11 @@ pg_status fail(pg_status code, const std::string &msg) {
 
 static int g_device = -1;
 
-// grow-only device arena with a bump pointer
+// grow-only device allocation, carved by its user (Carver)
 struct Arena {
     unsigned char *base = nullptr;
-    size_t cap = 0, top = 0;
+    size_t cap = 0;
     cudaError_t reserve(size_t bytes) {
-        top = 0;
         if (bytes <= cap) return cudaSuccess;
         if (base) cudaFree(base);
         base = nullptr;
@@ -38,18 +37,54 @@ struct Arena {
         if (e == cudaSuccess) cap = bytes;
         return e;
     }
-    void *take(size_t bytes) {
-        size_t a = align256(top);
-        if (a + bytes > cap) return nullptr;
-        top = a + bytes;
-        return base + a;
-    }
     void release() {
         if (base) cudaFree(base);
         base = nullptr;
-        cap = top = 0;
+        cap = 0;
     }
     ~Arena() { release(); }
+};
+
+// the device descriptors of a merge handle, carved from one allocation (Merge::d_desc)
+struct MergeDesc {
+    const void **key_ptrs;              // [run * n_key + field]
+    const int32_t **key_offs;
+    const int64_t **seq_ptrs;           // [k]
+    const int8_t **kind_ptrs;           // [k]
+    const void **data;                  // ColPtrs: [col * k + run]
+    const int32_t **offsets;
+    const uint32_t **validity;
+    int64_t *run_rows;                  // [k]
+    ColDesc *cols;                      // [n_cols]
+    pg_out_column *out_cols;            // [n_cols]
+    int64_t *totals;                    // [1 + n_varlen]
+    int32_t *err;
+    int32_t *tile_counter;
+    int32_t *col_order;                 // the emit kernel's pass list
+    int32_t *varlen_cols;               // [n_varlen]
+    SeqGroups *groups;                  // NULL on the device without sequence groups
+    ColPtrs ptrs() const { return ColPtrs{data, offsets, validity}; }
+    // the layout, for k runs, nk key fields, nc columns and nv var-len columns: returns its bytes
+    size_t carve(void *base, int k, int nk, int nc, int nv) {
+        Carver cv(base);
+        key_ptrs = cv.take<const void *>((size_t)k * nk);
+        key_offs = cv.take<const int32_t *>((size_t)k * nk);
+        seq_ptrs = cv.take<const int64_t *>(k);
+        kind_ptrs = cv.take<const int8_t *>(k);
+        data = cv.take<const void *>((size_t)k * nc);
+        offsets = cv.take<const int32_t *>((size_t)k * nc);
+        validity = cv.take<const uint32_t *>((size_t)k * nc);
+        run_rows = cv.take<int64_t>(k);
+        cols = cv.take<ColDesc>(nc);
+        out_cols = cv.take<pg_out_column>(nc);
+        totals = cv.take<int64_t>(nv + 1);
+        err = cv.take<int32_t>(1);
+        tile_counter = cv.take<int32_t>(1);
+        col_order = cv.take<int32_t>(2 * (size_t)nc + 2);
+        varlen_cols = cv.take<int32_t>(nv + 1);
+        groups = cv.take<SeqGroups>(1);
+        return cv.bytes();
+    }
 };
 
 struct Merge {
@@ -71,22 +106,9 @@ struct Merge {
     std::vector<uint8_t> emit;          // per column: part of the merged batch (read-type projection)
     // persistent device descriptors
     void *d_desc = nullptr;            // one allocation holding all descriptor arrays
-    const void **d_key_ptrs = nullptr;
-    const int32_t **d_key_offs = nullptr;
-    const int64_t **d_seq_ptrs = nullptr;
-    const int8_t **d_kind_ptrs = nullptr;
-    ColPtrs d_ptrs{};                   // [col * k + run]
-    int64_t *d_run_rows = nullptr;
-    ColDesc *d_cols = nullptr;
-    int32_t *d_tile_counter = nullptr;
-    int32_t *d_col_order = nullptr;
-    int32_t *d_varlen_cols = nullptr;
+    MergeDesc desc{};                  // ... carved into them
     int n_passes = 0;
-    const SeqGroups *d_groups = nullptr;
     bool has_group_aggs = false;
-    pg_out_column *d_out_cols = nullptr;
-    int64_t *d_totals = nullptr;       // [1 + n_varlen]
-    int32_t *d_err = nullptr;
     // pinned host mirror of totals + err
     int64_t *h_totals = nullptr;
     int32_t *h_err = nullptr;
@@ -316,31 +338,35 @@ pg_status RunBuilder::alloc(const std::vector<uint8_t> &bitmap, const std::vecto
     out.assign((size_t)n_runs * nc, OutColumn());
     for (int r = 0; r < n_runs; r++) {
         const int64_t n = run_rows[r];
-        scratch.runs[r] = std::make_unique<Run>(schema, n);
+        OutColumn *o = &out[(size_t)r * nc];
         // values, or int32 offsets
         auto main_bytes = [&](int c) { const int w = type_width(schema->field(c).type); return w ? (size_t)n * w : 4 * (size_t)(n + 1); };
-        const size_t vb = align256((size_t)((n + 31) / 32) * 4 + 64);
-        size_t vbytes = 0;
-        for (int c = 0; c < nc; c++) if (read[c] && bitmap[c]) vbytes += vb;
-        size_t total = vbytes;
-        std::vector<size_t> o_main(nc);
-        for (int c = 0; c < nc; c++) {
-            o_main[c] = total;
-            if (read[c]) total += align256(main_bytes(c) + 64);
-        }
-        scratch.runs[r]->bufs.emplace_back(total + 256);
+        size_t vspan = 0;                                // the bitmaps: [0, vspan)
+        auto carve = [&](void *base) {
+            Carver cv(base);
+            for (int c = 0; c < nc; c++)
+                if (read[c] && bitmap[c]) o[c].validity = cv.take<uint32_t>((size_t)(n + 31) / 32 + kReadPast / 4);
+            vspan = cv.bytes();
+            for (int c = 0; c < nc; c++) {
+                if (!read[c]) continue;
+                if (type_width(schema->field(c).type)) o[c].data = cv.take<uint8_t>(main_bytes(c) + kReadPast);
+                else o[c].offsets = cv.take<int32_t>((size_t)n + 1 + kReadPast / 4);
+            }
+            return cv.bytes();
+        };
+        const size_t total = carve(nullptr);
+        scratch.runs[r] = std::make_unique<Run>(schema, n);
+        scratch.runs[r]->bufs.emplace_back(total);
         unsigned char *base = scratch.runs[r]->bufs.back().get();
         if (!base) return oom(who, "the columns of a run", total);
-        if (vbytes) PG_CUDA(cudaMemsetAsync(base, 0, vbytes, scratch.stream));
-        size_t vt = 0;
+        carve(base);
+        if (vspan) PG_CUDA(cudaMemsetAsync(base, 0, vspan, scratch.stream));
         for (int c = 0; c < nc; c++) {
             if (!read[c]) continue;
-            OutColumn &o = out[(size_t)r * nc + c];
-            if (bitmap[c]) { o.validity = (uint32_t *)(base + vt); vt += vb; decoded_bytes += (n + 7) / 8; }
-            if (type_width(schema->field(c).type)) o.data = base + o_main[c];
-            else o.offsets = (int32_t *)(base + o_main[c]);
+            if (bitmap[c]) decoded_bytes += (n + 7) / 8;
             decoded_bytes += (int64_t)main_bytes(c);
-            if (zero[(size_t)r * nc + c]) PG_CUDA(cudaMemsetAsync(base + o_main[c], 0, main_bytes(c), scratch.stream));
+            void *values = type_width(schema->field(c).type) ? o[c].data : (void *)o[c].offsets;
+            if (zero[(size_t)r * nc + c]) PG_CUDA(cudaMemsetAsync(values, 0, main_bytes(c), scratch.stream));
         }
     }
     return PG_OK;
@@ -351,21 +377,24 @@ pg_status RunBuilder::alloc_payload(const std::vector<int64_t> &payload) {
     for (int c = 0; c < nc; c++) any |= read[c] && is_varlen(schema->field(c).type);
     if (!any) return PG_OK;
     for (int r = 0; r < (int)run_rows.size(); r++) {
-        size_t sum = 256;
-        for (int c = 0; c < nc; c++)
-            if (read[c] && is_varlen(schema->field(c).type)) sum += align256((size_t)payload[(size_t)r * nc + c] + 64);
+        OutColumn *o = &out[(size_t)r * nc];
+        const int64_t *bytes = &payload[(size_t)r * nc];
+        auto carve = [&](void *base) {
+            Carver cv(base);
+            for (int c = 0; c < nc; c++)
+                if (read[c] && is_varlen(schema->field(c).type)) o[c].data = cv.take<uint8_t>((size_t)bytes[c] + kReadPast);
+            return cv.bytes();
+        };
+        const size_t total = carve(nullptr);
         Run &run = *scratch.runs[r];
-        run.bufs.emplace_back(sum);
+        run.bufs.emplace_back(total);
         unsigned char *pl = run.bufs.back().get();
-        if (!pl) return oom(who, "the var-len payload of a run", sum);
-        size_t pt = 0;
+        if (!pl) return oom(who, "the var-len payload of a run", total);
+        carve(pl);
         for (int c = 0; c < nc; c++) {
             if (!read[c] || !is_varlen(schema->field(c).type)) continue;
-            const int64_t bytes = payload[(size_t)r * nc + c];
-            out[(size_t)r * nc + c].data = pl + pt;
-            run.varlen_bytes[c] = bytes;
-            decoded_bytes += bytes;
-            pt += align256((size_t)bytes + 64);
+            run.varlen_bytes[c] = bytes[c];
+            decoded_bytes += bytes[c];
         }
     }
     return PG_OK;
@@ -574,58 +603,41 @@ static pg_status build_descriptors(Merge *m) {
         }
     }
 
-    // one device allocation for all descriptor arrays
+    // one device allocation for all descriptor arrays, filled through a host mirror of the same layout
     const int k = m->k, nk = s->n_key, nv = (int)m->varlen_cols.size();
-    size_t o_key = 0;
-    size_t o_koff = o_key + align256(sizeof(void *) * k * nk);
-    size_t o_seq = o_koff + align256(sizeof(void *) * k * nk);
-    size_t o_kind = o_seq + align256(sizeof(void *) * k);
-    size_t o_pd = o_kind + align256(sizeof(void *) * k);
-    size_t o_po = o_pd + align256(sizeof(void *) * (size_t)k * nc);
-    size_t o_pv = o_po + align256(sizeof(void *) * (size_t)k * nc);
-    size_t o_rows = o_pv + align256(sizeof(void *) * (size_t)k * nc);
-    size_t o_cols = o_rows + align256(sizeof(int64_t) * k);
-    size_t o_out = o_cols + align256(sizeof(ColDesc) * nc);
-    size_t o_tot = o_out + align256(sizeof(pg_out_column) * nc);
-    size_t o_err = o_tot + align256(sizeof(int64_t) * (nv + 1));
-    size_t o_cnt = o_err + 256;
-    size_t o_ord = o_cnt + 256;
-    size_t o_vlc = o_ord + align256(sizeof(int32_t) * (2 * (size_t)nc + 2));
-    size_t o_sg = o_vlc + align256(sizeof(int32_t) * (size_t)(nv + 1));
-    size_t total = o_sg + align256(sizeof(SeqGroups));
+    MergeDesc h;
+    const size_t total = h.carve(nullptr, k, nk, nc, nv);
     std::vector<unsigned char> host(total, 0);
+    h.carve(host.data(), k, nk, nc, nv);
     m->varlen_bound.assign(nv, 0);
     for (int r = 0; r < k; r++) {
         const Run *run = m->runs[r].get();
         for (int f = 0; f < nk; f++) {
-            ((const void **)(host.data() + o_key))[r * nk + f] = run->cols[f].data;
-            ((const void **)(host.data() + o_koff))[r * nk + f] = run->cols[f].offsets;
+            h.key_ptrs[r * nk + f] = run->cols[f].data;
+            h.key_offs[r * nk + f] = run->cols[f].offsets;
         }
-        ((const void **)(host.data() + o_seq))[r] = run->cols[nk].data;
-        ((const void **)(host.data() + o_kind))[r] = run->cols[nk + 1].data;
+        h.seq_ptrs[r] = (const int64_t *)run->cols[nk].data;
+        h.kind_ptrs[r] = (const int8_t *)run->cols[nk + 1].data;
         for (int c = 0; c < nc; c++) {
-            ((const void **)(host.data() + o_pd))[(size_t)c * k + r] = run->cols[c].data;
-            ((const void **)(host.data() + o_po))[(size_t)c * k + r] = run->cols[c].offsets;
-            ((const void **)(host.data() + o_pv))[(size_t)c * k + r] = run->cols[c].validity;
+            h.data[(size_t)c * k + r] = run->cols[c].data;
+            h.offsets[(size_t)c * k + r] = run->cols[c].offsets;
+            h.validity[(size_t)c * k + r] = (const uint32_t *)run->cols[c].validity;
             if (m->cols[c].varlen_index >= 0) m->varlen_bound[m->cols[c].varlen_index] += run->varlen_bytes[c];
         }
-        ((int64_t *)(host.data() + o_rows))[r] = run->n_rows;
+        h.run_rows[r] = run->n_rows;
     }
-    memcpy(host.data() + o_cols, m->cols.data(), sizeof(ColDesc) * nc);
+    memcpy(h.cols, m->cols.data(), sizeof(ColDesc) * nc);
     {
         // the emit kernel's pass list: var-len columns first (their cross-tile look-back then happens while the CTAs of
         // a wave are still close together in time), then everything else; columns the read type leaves out are skipped
-        int32_t *ord = (int32_t *)(host.data() + o_ord);
-        int32_t *vlc = (int32_t *)(host.data() + o_vlc);
         int n = 0;
-        for (int c = 0; c < nc; c++) if (m->emit[c] && m->cols[c].width == 0) ord[n++] = c;
-        for (int c = 0; c < nc; c++) if (m->emit[c] && m->cols[c].width != 0) ord[n++] = c;
+        for (int c = 0; c < nc; c++) if (m->emit[c] && m->cols[c].width == 0) h.col_order[n++] = c;
+        for (int c = 0; c < nc; c++) if (m->emit[c] && m->cols[c].width != 0) h.col_order[n++] = c;
         m->n_passes = n;
-        for (int v = 0; v < nv; v++) vlc[v] = m->varlen_cols[v];
+        for (int v = 0; v < nv; v++) h.varlen_cols[v] = m->varlen_cols[v];
     }
-    m->d_groups = nullptr;
     if (sp->n_groups() > 0) {
-        SeqGroups *sg = (SeqGroups *)(host.data() + o_sg);
+        SeqGroups *sg = h.groups;
         sg->n = sp->n_groups();
         for (int g = 0; g <= sg->n; g++) sg->start[g] = sp->group_seq_start[g];
         for (int j = 0; j < sp->group_seq_start[sg->n]; j++) {
@@ -644,23 +656,8 @@ static pg_status build_descriptors(Merge *m) {
     }
     { pg_status ts = small_h2d(m->d_desc, host.data(), total, m->stream); if (ts) return ts; }
     PG_CUDA(cudaStreamSynchronize(m->stream));
-    unsigned char *d = (unsigned char *)m->d_desc;
-    m->d_key_ptrs = (const void **)(d + o_key);
-    m->d_key_offs = (const int32_t **)(d + o_koff);
-    m->d_seq_ptrs = (const int64_t **)(d + o_seq);
-    m->d_kind_ptrs = (const int8_t **)(d + o_kind);
-    m->d_ptrs.data = (const void *const *)(d + o_pd);
-    m->d_ptrs.offsets = (const int32_t *const *)(d + o_po);
-    m->d_ptrs.validity = (const uint32_t *const *)(d + o_pv);
-    m->d_run_rows = (int64_t *)(d + o_rows);
-    m->d_cols = (ColDesc *)(d + o_cols);
-    m->d_out_cols = (pg_out_column *)(d + o_out);
-    m->d_totals = (int64_t *)(d + o_tot);
-    m->d_err = (int32_t *)(d + o_err);
-    m->d_tile_counter = (int32_t *)(d + o_cnt);
-    m->d_col_order = (int32_t *)(d + o_ord);
-    m->d_varlen_cols = (int32_t *)(d + o_vlc);
-    if (sp->n_groups() > 0) m->d_groups = (const SeqGroups *)(d + o_sg);
+    m->desc.carve(m->d_desc, k, nk, nc, nv);
+    if (sp->n_groups() == 0) m->desc.groups = nullptr;        // (the plan kernel's test for sequence groups)
     if (!m->h_totals) PG_CUDA(cudaMallocHost((void **)&m->h_totals, sizeof(int64_t) * (nv + 1) + 16));
     m->h_err = (int32_t *)(m->h_totals + nv + 1);
     return PG_OK;
@@ -757,108 +754,96 @@ static pg_status execute(Merge *m) {
     m->stats.n_levels = top;
     m->stats.n_tiles = n_tiles[0];
 
-    PG_CUDA(cudaMemsetAsync(m->d_err, 0, sizeof(int32_t), sm));
+    PG_CUDA(cudaMemsetAsync(m->desc.err, 0, sizeof(int32_t), sm));
     PG_CUDA(cudaEventRecord(m->ev[0], sm));
 
-    MergeLaunch ml{k, m->key, KeySrc{m->d_key_ptrs, m->d_key_offs}, sm, m->d_err, nullptr};
-    // Workspace: one grow-only device allocation per merge handle, carved with a bump pointer.  Its size
-    // depends only on the input shapes, so a reader that is executed repeatedly (or a pool of readers of
-    // one bucket layout) never goes back to the driver allocator.
-    {
-        size_t need = 4096;
-        auto add = [&](size_t b) { need += align256(b ? b : 16); };
+    MergeLaunch ml{k, m->key, KeySrc{m->desc.key_ptrs, m->desc.key_offs}, sm, m->desc.err, nullptr};
+    // Workspace: one grow-only device allocation per merge handle.  Its size depends only on the input shapes, so a
+    // reader that is executed repeatedly (or a pool of readers of one bucket layout) never goes back to the driver
+    // allocator.  The plan-sized arrays are indexed by sums of absolute rows (N counts the rows a rebind skips) and
+    // keep 16 bytes behind their last entry.
+    const int T = n_tiles[0];
+    int64_t N = m->n_in;
+    for (int r = 0; r < k; r++) N += m->row0[r];
+    int *d_skip = nullptr;
+    std::vector<int64_t *> bounds(top + 1);
+    std::vector<uint64_t *> sk(top + 1), sref(top + 1);   // level l > 0: its sorted keys, and the rows they came from
+    uint16_t *plan = nullptr;
+    uint32_t *gplan = nullptr, *gagg = nullptr;
+    int32_t *tile_rows = nullptr;
+    int64_t *tmp_seq = nullptr, *row_base = nullptr;
+    int8_t *tmp_kind = nullptr;
+    uint64_t *vl_state = nullptr;
+    const size_t vl_words = (size_t)T * std::max(nv, 1);
+    auto carve_work = [&](void *base) {
+        Carver cv(base);
+        if (!m->key.exact) d_skip = cv.take<int>(1);
         for (int l = top; l >= 0; l--) {
-            add(sizeof(int64_t) * (size_t)(n_tiles[l] + 1) * k);
-            if (l > 0) { add(sizeof(uint64_t) * (size_t)std::max<int64_t>(level_total[l], 1)); add(sizeof(uint64_t) * (size_t)std::max<int64_t>(level_total[l], 1)); }
+            bounds[l] = cv.take<int64_t>((size_t)(n_tiles[l] + 1) * k);
+            if (l > 0) {
+                sk[l] = cv.take<uint64_t>((size_t)std::max<int64_t>(level_total[l], 1));
+                sref[l] = cv.take<uint64_t>((size_t)std::max<int64_t>(level_total[l], 1));
+            }
         }
-        int64_t skipped = 0;                      // plan-sized arrays are indexed by sums of absolute rows
-        for (int r = 0; r < k; r++) skipped += m->row0[r];
-        const size_t N_ = (size_t)(m->n_in + skipped), T_ = (size_t)n_tiles[0];
-        add(2 * N_ + 16); add(m->d_groups ? 4 * N_ + 16 : 16); add(m->has_group_aggs ? 4 * N_ + 16 : 16); add(4 * T_); add(8 * N_ + 16); add(N_ + 16); add(8 * T_); add(8 * T_ * std::max(nv, 1));
-        PG_CUDA(m->work.reserve(need));
-    }
-    auto talloc = [&](size_t bytes, void **out) -> cudaError_t {
-        *out = m->work.take(bytes ? bytes : 16);
-        return *out ? cudaSuccess : cudaErrorMemoryAllocation;
+        plan = cv.take<uint16_t>((size_t)N + 8);
+        if (m->desc.groups) gplan = cv.take<uint32_t>((size_t)N + 4);
+        if (m->has_group_aggs) gagg = cv.take<uint32_t>((size_t)N + 4);
+        tile_rows = cv.take<int32_t>(T);
+        tmp_seq = cv.take<int64_t>((size_t)N + 2);
+        tmp_kind = cv.take<int8_t>((size_t)N + 16);
+        row_base = cv.take<int64_t>(T);
+        vl_state = cv.take<uint64_t>(vl_words);
+        return cv.bytes();
     };
+    PG_CUDA(m->work.reserve(carve_work(nullptr)));
+    carve_work(m->work.base);
 
     if (!m->key.exact) {
         // window keys start behind the prefix all keys share (strings like "user_0000123", wide composites)
-        int *d_skip = nullptr;
-        PG_CUDA(talloc(sizeof(int), (void **)&d_skip));
         launch_key_lcp(ml, views[0], d_skip);
         ml.skip = d_skip;
         launches++;
     }
-    int64_t *bounds0 = nullptr;
-    uint64_t *sk_above = nullptr;         // sorted sample keys of the level above the current one
-    uint64_t *sref_above = nullptr;       // ... and the rows they came from (non-exact keys)
     for (int l = top; l >= 0; l--) {
-        int64_t *bounds = nullptr;
-        PG_CUDA(talloc(sizeof(int64_t) * (size_t)(n_tiles[l] + 1) * k, (void **)&bounds));
-        launch_partition(ml, views[l], sk_above, sref_above, q, n_tiles[l], bounds);
+        // the sorted sample keys of the level above split this one
+        launch_partition(ml, views[l], l < top ? sk[l + 1] : nullptr, l < top ? sref[l + 1] : nullptr, q, n_tiles[l],
+                         bounds[l]);
         launches++;
         if (l > 0) {
-            uint64_t *sk = nullptr;
-            PG_CUDA(talloc(sizeof(uint64_t) * (size_t)std::max<int64_t>(level_total[l], 1), (void **)&sk));
-            uint64_t *sref = nullptr;
-            PG_CUDA(talloc(sizeof(uint64_t) * (size_t)std::max<int64_t>(level_total[l], 1), (void **)&sref));
-            launch_merge_keys(ml, views[l], bounds, n_tiles[l], sk, sref);
-            sref_above = sref;
+            launch_merge_keys(ml, views[l], bounds[l], n_tiles[l], sk[l], sref[l]);
             launches++;
-            sk_above = sk;
-        } else {
-            bounds0 = bounds;
         }
     }
     PG_CUDA(cudaEventRecord(m->ev[1], sm));
 
     // ---- plan + scan
-    const int T = n_tiles[0];
-    int64_t N = m->n_in;
-    for (int r = 0; r < k; r++) N += m->row0[r];
-    uint16_t *plan = nullptr;
-    int32_t *tile_rows = nullptr;
-    int64_t *tmp_seq = nullptr, *row_base = nullptr;
-    uint64_t *vl_state = nullptr;
-    int8_t *tmp_kind = nullptr;
-    PG_CUDA(talloc(sizeof(uint16_t) * (size_t)N + 16, (void **)&plan));
-    uint32_t *gplan = nullptr;
-    if (m->d_groups) PG_CUDA(talloc(sizeof(uint32_t) * (size_t)N + 16, (void **)&gplan));
-    uint32_t *gagg = nullptr;
-    if (m->has_group_aggs) PG_CUDA(talloc(sizeof(uint32_t) * (size_t)N + 16, (void **)&gagg));
-    PG_CUDA(talloc(sizeof(int32_t) * (size_t)T, (void **)&tile_rows));
-    PG_CUDA(talloc(sizeof(int64_t) * (size_t)N + 16, (void **)&tmp_seq));
-    PG_CUDA(talloc((size_t)N + 16, (void **)&tmp_kind));
-    PG_CUDA(talloc(sizeof(int64_t) * (size_t)T, (void **)&row_base));
-    PG_CUDA(talloc(sizeof(uint64_t) * (size_t)T * std::max(nv, 1), (void **)&vl_state));
-    PG_CUDA(cudaMemsetAsync(vl_state, 0, sizeof(uint64_t) * (size_t)T * std::max(nv, 1), sm));
-    PG_CUDA(cudaMemsetAsync(m->d_tile_counter, 0, sizeof(int32_t), sm));
+    PG_CUDA(cudaMemsetAsync(vl_state, 0, sizeof(uint64_t) * vl_words, sm));
+    PG_CUDA(cudaMemsetAsync(m->desc.tile_counter, 0, sizeof(int32_t), sm));
 
     PlanArgs pa{};
-    pa.bounds = bounds0;
+    pa.bounds = bounds[0];
     pa.n_tiles = T;
-    pa.seq_ptrs = m->d_seq_ptrs;
-    pa.kind_ptrs = m->d_kind_ptrs;
+    pa.seq_ptrs = m->desc.seq_ptrs;
+    pa.kind_ptrs = m->desc.kind_ptrs;
     pa.flags = m->flags;
     pa.seq = m->seq;
-    pa.ptrs = m->d_ptrs;
+    pa.ptrs = m->desc.ptrs();
     pa.plan = plan;
     pa.tile_rows = tile_rows;
     pa.tmp_seq = tmp_seq;
     pa.tmp_kind = tmp_kind;
-    pa.groups = m->d_groups;
+    pa.groups = m->desc.groups;
     pa.gplan = gplan;
     pa.gagg = gagg;
     launch_plan(ml, pa);
-    launch_scan(sm, tile_rows, T, row_base, m->d_totals);
+    launch_scan(sm, tile_rows, T, row_base, m->desc.totals);
     launches += 2;
     PG_CUDA(cudaEventRecord(m->ev[2], sm));
     PG_HOST_MARK("enqueue");
     {
         SmallReads rb(sm);                   // the one size read-back: output buffers are sized exactly
-        pg_status rs = rb.add(m->h_totals, m->d_totals, sizeof(int64_t));
-        if (!rs) rs = rb.add(m->h_err, m->d_err, sizeof(int32_t));
+        pg_status rs = rb.add(m->h_totals, m->desc.totals, sizeof(int64_t));
+        if (!rs) rs = rb.add(m->h_err, m->desc.err, sizeof(int32_t));
         if (!rs) rs = rb.finish();
         if (rs) return rs;
     }
@@ -869,61 +854,47 @@ static pg_status execute(Merge *m) {
     const int64_t n_out = m->h_totals[0];
     m->n_out = n_out;
     m->out_cols.assign(nc, pg_out_column{});
+    // output arena (grow-only, reused until pg_merge_release): the validity bitmaps first and contiguous, so that one
+    // memset clears them all, then per column its values, or its var-len payload and offsets.  The exact payload size
+    // is only known after the emit kernel's look-back; every output cell is one input cell, so the runs' payload bytes
+    // bound it.
+    size_t vspan = 0;                                    // the bitmaps: [0, vspan)
     int64_t bytes_out = 0;
-    {
-        // output arena (grow-only, reused until pg_merge_release): validity bitmaps first and contiguous,
-        // so that one memset clears them all
-        size_t need = 4096, vbytes = 0;
+    auto carve_out = [&](void *base) {
+        Carver cv(base);
+        bytes_out = 0;
+        for (int c = 0; c < nc; c++)
+            if (m->cols[c].nullable && m->emit[c]) {
+                m->out_cols[c].validity = cv.take<uint8_t>((size_t)((n_out + 31) / 32) * 4 + kReadPast);
+                bytes_out += (n_out + 7) / 8;
+            }
+        vspan = cv.bytes();
         for (int c = 0; c < nc; c++) {
             const ColDesc &cd = m->cols[c];
-            if (!m->emit[c]) continue;
-            if (cd.nullable) vbytes += align256((size_t)((n_out + 31) / 32) * 4 + 64);
-            if (cd.width > 0) need += align256((size_t)n_out * cd.width + 64);
-            else need += align256((size_t)m->varlen_bound[cd.varlen_index] + 64) + align256(4 * (size_t)(n_out + 1) + 64);
+            pg_out_column &oc = m->out_cols[c];
+            if (!m->emit[c]) continue;                       // not part of the read type: the batch has no such column
+            if (cd.width > 0) {
+                oc.data_bytes = n_out * cd.width;
+                oc.data = cv.take<uint8_t>((size_t)oc.data_bytes + kReadPast);
+                bytes_out += oc.data_bytes;
+            } else {
+                oc.data_bytes = m->varlen_bound[cd.varlen_index];
+                oc.data = cv.take<uint8_t>((size_t)oc.data_bytes + kReadPast);
+                oc.offsets = cv.take<int32_t>((size_t)n_out + 1 + kReadPast / 4);
+                bytes_out += 4 * (n_out + 1);
+            }
         }
-        if (nv > 0) need += align256(sizeof(uint16_t) * (size_t)nv * (size_t)(n_out + 64) + 64);   // k_emit's source scratch
-        PG_CUDA(m->outbuf.reserve(need + vbytes));
-        if (vbytes) {
-            void *v0 = m->outbuf.take(vbytes);
-            PG_CUDA(cudaMemsetAsync(v0, 0, vbytes, sm));
-            m->outbuf.top = 0;                       // validity buffers are taken again, one by one, below
-        }
-    }
-    auto oalloc = [&](size_t bytes, void **out) -> cudaError_t {
-        *out = m->outbuf.take(bytes);
-        return *out ? cudaSuccess : cudaErrorMemoryAllocation;
+        return cv.bytes();
     };
-    // pass 1: validity bitmaps (the zeroed region), pass 2: data + offsets
-    for (int c = 0; c < nc; c++) {
-        if (m->cols[c].nullable && m->emit[c]) {
-            size_t vb = (size_t)((n_out + 31) / 32) * 4 + 64;
-            PG_CUDA(oalloc(vb, (void **)&m->out_cols[c].validity));
-            bytes_out += (n_out + 7) / 8;
-        }
-    }
-    for (int c = 0; c < nc; c++) {
-        const ColDesc &cd = m->cols[c];
-        pg_out_column &oc = m->out_cols[c];
-        if (!m->emit[c]) continue;                       // not part of the read type: the batch has no such column
-        if (cd.width > 0) {
-            oc.data_bytes = n_out * cd.width;
-            PG_CUDA(oalloc((size_t)oc.data_bytes + 64, &oc.data));
-        } else {
-            // exact size is only known after the emit kernel's look-back; every output cell is one input
-            // cell, so the runs' payload bytes bound it
-            oc.data_bytes = m->varlen_bound[cd.varlen_index];
-            PG_CUDA(oalloc((size_t)oc.data_bytes + 64, &oc.data));
-            PG_CUDA(oalloc(sizeof(int32_t) * (size_t)(n_out + 1) + 64, (void **)&oc.offsets));
-            bytes_out += 4 * (n_out + 1);
-        }
-        if (cd.width > 0) bytes_out += oc.data_bytes;
-    }
+    PG_CUDA(m->outbuf.reserve(carve_out(nullptr)));
+    carve_out(m->outbuf.base);
+    if (vspan) PG_CUDA(cudaMemsetAsync(m->outbuf.base, 0, vspan, sm));
     m->stats.bytes_out = bytes_out;
-    { pg_status ts = small_h2d(m->d_out_cols, m->out_cols.data(), sizeof(pg_out_column) * nc, sm); if (ts) return ts; }
+    { pg_status ts = small_h2d(m->desc.out_cols, m->out_cols.data(), sizeof(pg_out_column) * nc, sm); if (ts) return ts; }
 
     // ---- emit
     EmitArgs ea{};
-    ea.bounds = bounds0;
+    ea.bounds = bounds[0];
     ea.n_tiles = (T + 1) / 2;
     ea.n_plan_tiles = T;
     ea.tile_rows = tile_rows;
@@ -934,19 +905,19 @@ static pg_status execute(Merge *m) {
     ea.tmp_kind = tmp_kind;
     ea.gplan = gplan;
     ea.gagg = gagg;
-    ea.cols = m->d_cols;
-    ea.col_order = m->d_col_order;
+    ea.cols = m->desc.cols;
+    ea.col_order = m->desc.col_order;
     ea.n_passes = m->n_passes;
-    ea.varlen_cols = m->d_varlen_cols;
-    ea.ptrs = m->d_ptrs;
-    ea.run_rows = m->d_run_rows;
+    ea.varlen_cols = m->desc.varlen_cols;
+    ea.ptrs = m->desc.ptrs();
+    ea.run_rows = m->desc.run_rows;
     ea.n_cols = nc;
     ea.n_varlen = nv;
-    ea.out_cols = m->d_out_cols;
-    ea.totals = m->d_totals;
+    ea.out_cols = m->desc.out_cols;
+    ea.totals = m->desc.totals;
     ea.vl_state = vl_state;
-    ea.tile_counter = m->d_tile_counter;
-    ea.err = m->d_err;
+    ea.tile_counter = m->desc.tile_counter;
+    ea.err = m->desc.err;
     ea.stream = sm;
     PG_CUDA(cudaEventRecord(m->ev[4], sm));
     launch_emit(ea);
@@ -955,8 +926,8 @@ static pg_status execute(Merge *m) {
     PG_HOST_MARK("alloc_emit");
     {
         SmallReads rb(sm);
-        pg_status rs = rb.add(m->h_err, m->d_err, sizeof(int32_t));
-        if (!rs) rs = rb.add(m->h_totals, m->d_totals, sizeof(int64_t) * (nv + 1));
+        pg_status rs = rb.add(m->h_err, m->desc.err, sizeof(int32_t));
+        if (!rs) rs = rb.add(m->h_totals, m->desc.totals, sizeof(int64_t) * (nv + 1));
         if (!rs) rs = rb.finish();
         if (rs) return rs;
     }

@@ -40,6 +40,13 @@ struct OrcTaskRef {            // stream table indexes of a task (-1 = absent)
     int32_t s_present, s_data, s_length, s_dict, s_secondary;
 };
 
+// the words a section decode's kernels report in, cleared by one memset
+struct OrcWords {
+    int32_t err;               // the kernel error word
+    int32_t counter;           // k_orc_inflate's stream ticket
+    int64_t sc_total;          // k_orc_scan: bytes of the stream scratch
+};
+
 // one thread per stream: the bound of the bytes its compression chunks inflate to, from the chunk headers (0 for the
 // streams of uncompressed files, which are read in place); a chunk cut off by the stream's end sets *err
 __global__ void k_orc_walk(OrcStream *streams, int n_streams, int32_t *err) {
@@ -267,27 +274,35 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
         dict_base += plans[f].dict_entries;
     }
     const int n_streams = (int)h_streams.size(), n_tasks = (int)h_tasks.size();
-    const size_t tb_s = align256(sizeof(OrcStream) * (size_t)std::max(n_streams, 1)), tb_t = align256(sizeof(orcdev::Task) * (size_t)std::max(n_tasks, 1));
-    const size_t tb_r = align256(sizeof(OrcTaskRef) * (size_t)std::max(n_tasks, 1)), tb_o = align256(4 * (size_t)std::max(n_tasks, 1));
-    const size_t tb_p = align256(sizeof(void *) * b.out.size());
     int sms = 132, dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int inflate_ctas = !any_compressed ? std::max(1, std::min(sms, (n_streams + kOrcWarps - 1) / kOrcWarps))
                                                   : std::max(1, std::min(sms * 4, (n_streams + kOrcWarps - 1) / kOrcWarps));
-    const size_t tb_lit = any_zstd ? align256((size_t)inflate_ctas * kOrcWarps * (size_t)(zs::kMaxBlock + 64)) : 256;
-    unsigned char *tb = (unsigned char *)fr.scratch.take(tb_s + tb_t + tb_r + tb_o + tb_p + tb_lit + 1024);
-    if (!tb) return oom("orc", "the stream and task tables", tb_s + tb_t + tb_r + tb_o + tb_p + tb_lit);
-    OrcStream *d_streams = (OrcStream *)tb;
-    orcdev::Task *d_tasks = (orcdev::Task *)(tb + tb_s);
-    OrcTaskRef *d_refs = (OrcTaskRef *)(tb + tb_s + tb_t);
-    int32_t *d_task_out = (int32_t *)(tb + tb_s + tb_t + tb_r);
-    uint8_t **d_payload = (uint8_t **)(tb + tb_s + tb_t + tb_r + tb_o);
-    uint8_t *d_lit = tb + tb_s + tb_t + tb_r + tb_o + tb_p;
-    int32_t *d_err = (int32_t *)(d_lit + tb_lit);
-    int32_t *d_counter = d_err + 4;
-    int64_t *d_sc_total = (int64_t *)(d_err + 8);
-    PG_CUDA(cudaMemsetAsync(d_err, 0, 64, sm));
+    OrcStream *d_streams;
+    orcdev::Task *d_tasks;
+    OrcTaskRef *d_refs;
+    int32_t *d_task_out;
+    uint8_t **d_payload;
+    uint8_t *d_lit;                                      // the zstd literal scratch of each inflate warp
+    OrcWords *d_words;
+    auto carve = [&](void *base) {
+        Carver cv(base);
+        d_streams = cv.take<OrcStream>((size_t)std::max(n_streams, 1));
+        d_tasks = cv.take<orcdev::Task>((size_t)std::max(n_tasks, 1));
+        d_refs = cv.take<OrcTaskRef>((size_t)std::max(n_tasks, 1));
+        d_task_out = cv.take<int32_t>((size_t)std::max(n_tasks, 1));
+        d_payload = cv.take<uint8_t *>(b.out.size());
+        d_lit = cv.take<uint8_t>(any_zstd ? (size_t)inflate_ctas * kOrcWarps * (size_t)(zs::kMaxBlock + 64) : 0);
+        d_words = cv.take<OrcWords>(1);
+        return cv.bytes();
+    };
+    const size_t tb_bytes = carve(nullptr);
+    void *tb = fr.scratch.take(tb_bytes);
+    if (!tb) return oom("orc", "the stream and task tables", tb_bytes);
+    carve(tb);
+    int32_t *d_err = &d_words->err;
+    PG_CUDA(cudaMemsetAsync(d_words, 0, sizeof(OrcWords), sm));
     // (tables go through small_h2d: a kernel reads them out of mapped host memory, so they do not queue behind an
     // asynchronous upload of the next section on the copy engine)
     if (n_streams) { pg_status ts = small_h2d(d_streams, h_streams.data(), sizeof(OrcStream) * n_streams, sm); if (ts) return ts; }
@@ -301,14 +316,14 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
     uint8_t *d_sc = nullptr;
     if (any_compressed && n_streams) {
         k_orc_walk<<<(n_streams + 127) / 128, 128, 0, sm>>>(d_streams, n_streams, d_err);
-        k_orc_scan<<<1, kOrcScanThreads, 0, sm>>>(d_streams, n_streams, d_sc_total);
+        k_orc_scan<<<1, kOrcScanThreads, 0, sm>>>(d_streams, n_streams, &d_words->sc_total);
         fr.launches += 2;
         int32_t herr = 0;
         int64_t sc_bytes = 0;
         {
             SmallReads rb(sm);
             pg_status rs = rb.add(&herr, d_err, 4);
-            if (!rs) rs = rb.add(&sc_bytes, d_sc_total, 8);
+            if (!rs) rs = rb.add(&sc_bytes, &d_words->sc_total, 8);
             if (!rs) rs = rb.finish();
             if (!rs) rs = kernel_error(herr, "orc");
             if (rs) return rs;
@@ -317,7 +332,7 @@ static pg_status orc_decode_section(const std::shared_ptr<const Schema> &s, cons
         if (!d_sc) return oom("orc", "the stream scratch", (size_t)sc_bytes);
     }
     if (n_streams) {
-        k_orc_inflate<<<inflate_ctas, kOrcWarps * 32, 0, sm>>>(d_streams, n_streams, d_sc, d_lit, d_counter, d_err);
+        k_orc_inflate<<<inflate_ctas, kOrcWarps * 32, 0, sm>>>(d_streams, n_streams, d_sc, d_lit, &d_words->counter, d_err);
         fr.launches++;
     }
     if (n_tasks) {

@@ -1560,20 +1560,26 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
     const bool any_empty = std::find(b.run_rows.begin(), b.run_rows.end(), 0) != b.run_rows.end();
 
     // ---- tables to the device, page count pass
-    const size_t tb_chunks = align256(sizeof(PqChunk) * (size_t)std::max(n_chunks, 1));
-    const size_t tb_outs = align256(sizeof(PqOut) * outs.size());
-    const size_t tb_pairs = align256(sizeof(PqPair) * (size_t)std::max(n_pairs, 1));
-    const size_t tb_tot = align256(sizeof(int64_t) * (size_t)(8 + n_pairs));
     // (two output tables: the second one adds the var-len payload pointers, known only after read-back 2)
-    unsigned char *tb = (unsigned char *)fr.scratch.take(tb_chunks + 2 * tb_outs + tb_pairs + tb_tot + 256);
-    if (!tb) return oom("parquet", "the chunk tables", tb_chunks + 2 * tb_outs + tb_pairs + tb_tot);
-    PqChunk *d_chunks = (PqChunk *)tb;
-    PqOut *d_outs = (PqOut *)(tb + tb_chunks);
-    PqOut *d_outs2 = (PqOut *)(tb + tb_chunks + tb_outs);
-    PqPair *d_pairs = (PqPair *)(tb + tb_chunks + 2 * tb_outs);
-    int64_t *d_totals = (int64_t *)(tb + tb_chunks + 2 * tb_outs + tb_pairs);  // [0..5] chunk totals, [8..] pair totals
+    PqChunk *d_chunks;
+    PqOut *d_outs, *d_outs2;
+    PqPair *d_pairs;
+    int64_t *d_totals;               // [0..5] chunk totals, [6] error word, [7] zstd ticket, [8..] pair totals
+    auto carve_tables = [&](void *base) {
+        Carver cv(base);
+        d_chunks = cv.take<PqChunk>((size_t)std::max(n_chunks, 1));
+        d_outs = cv.take<PqOut>(outs.size());
+        d_outs2 = cv.take<PqOut>(outs.size());
+        d_pairs = cv.take<PqPair>((size_t)std::max(n_pairs, 1));
+        d_totals = cv.take<int64_t>(8 + (size_t)n_pairs);
+        return cv.bytes();
+    };
+    const size_t tb_bytes = carve_tables(nullptr);
+    void *tb = fr.scratch.take(tb_bytes);
+    if (!tb) return oom("parquet", "the chunk tables", tb_bytes);
+    carve_tables(tb);
     int32_t *d_err = (int32_t *)(d_totals + 6);
-    PG_CUDA(cudaMemsetAsync(d_totals, 0, tb_tot, sm));
+    PG_CUDA(cudaMemsetAsync(d_totals, 0, sizeof(int64_t) * (8 + (size_t)n_pairs), sm));
     // (tables go through small_h2d: a kernel reads them out of mapped host memory, so they do not queue behind an
     // asynchronous upload of the next section on the copy engine)
     if (n_chunks) { pg_status ts = small_h2d(d_chunks, ct.chunks.data(), sizeof(PqChunk) * n_chunks, sm); if (ts) return ts; }
@@ -1600,12 +1606,6 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
     if (n_pages > 0x7fffffffLL) return fail(PG_ERR_UNSUPPORTED, "parquet: too many pages in one section");
 
     // ---- page table + scratch, fill pass, inflate
-    const size_t sb_pages = align256(sizeof(PqPage) * (size_t)std::max<int64_t>(n_pages, 1));
-    const size_t sb_dicts = align256(sizeof(PqPage) * (size_t)std::max<int64_t>(n_dicts, 1));
-    const size_t sb_sc = align256((size_t)sc_bytes + 64);
-    const size_t sb_de = align256(4 * (size_t)(dict_entries + 1));
-    const size_t sb_ids = align256(4 * (size_t)(ids_entries + 1));
-    const size_t sb_vs = align256(4 * (size_t)(ct.pair_rows + n_pages + n_pairs + 2));
     int zs_ctas = 0;
     if (ct.any_zstd) {
         int dev = 0, sms = 132;
@@ -1613,17 +1613,25 @@ static pg_status decode_section(const std::shared_ptr<const Schema> &s, const pg
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
         zs_ctas = (int)std::min<int64_t>((int64_t)sms * 5, (n_pages + n_dicts + kZsWarps - 1) / kZsWarps);
     }
-    const size_t sb_zs = align256((size_t)zs_ctas * kZsWarps * (size_t)(zs::kMaxBlock + 64));
-    unsigned char *sbuf = (unsigned char *)fr.scratch.take(sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs + 256);
-    if (!sbuf) return oom("parquet", "the page table and scratch", sb_pages + sb_dicts + sb_sc + 2 * sb_de + sb_ids + sb_vs + sb_zs);
-    PqPage *d_pages = (PqPage *)sbuf;
-    PqPage *d_dicts = (PqPage *)(sbuf + sb_pages);
-    uint8_t *d_sc = sbuf + sb_pages + sb_dicts;
-    int32_t *d_dict_off = (int32_t *)(d_sc + sb_sc);
-    int32_t *d_dict_len = (int32_t *)(d_sc + sb_sc + sb_de);
-    int32_t *d_ids = (int32_t *)(d_sc + sb_sc + 2 * sb_de);
-    int32_t *d_vstart = (int32_t *)(d_sc + sb_sc + 2 * sb_de + sb_ids);
-    uint8_t *d_zs_lit = (uint8_t *)d_vstart + sb_vs;
+    PqPage *d_pages, *d_dicts;
+    uint8_t *d_sc, *d_zs_lit;
+    int32_t *d_dict_off, *d_dict_len, *d_ids, *d_vstart;
+    auto carve_pages = [&](void *base) {
+        Carver cv(base);
+        d_pages = cv.take<PqPage>((size_t)std::max<int64_t>(n_pages, 1));
+        d_dicts = cv.take<PqPage>((size_t)std::max<int64_t>(n_dicts, 1));
+        d_sc = cv.take<uint8_t>((size_t)sc_bytes + kReadPast);
+        d_dict_off = cv.take<int32_t>((size_t)dict_entries + 1);
+        d_dict_len = cv.take<int32_t>((size_t)dict_entries + 1);
+        d_ids = cv.take<int32_t>((size_t)ids_entries + 1);
+        d_vstart = cv.take<int32_t>((size_t)(ct.pair_rows + n_pages + n_pairs + 2));
+        d_zs_lit = cv.take<uint8_t>((size_t)zs_ctas * kZsWarps * (size_t)(zs::kMaxBlock + 64));
+        return cv.bytes();
+    };
+    const size_t sb_bytes = carve_pages(nullptr);
+    void *sbuf = fr.scratch.take(sb_bytes);
+    if (!sbuf) return oom("parquet", "the page table and scratch", sb_bytes);
+    carve_pages(sbuf);
     const int np = (int)n_pages, nd = (int)n_dicts;
     std::vector<int64_t> pair_tot(std::max(n_pairs, 1), 0);
     if (np > 0) {

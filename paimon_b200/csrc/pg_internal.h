@@ -13,6 +13,7 @@
 #include <utility>
 #include <vector>
 
+#include "device_layout.h"
 #include "paimon_gpu.h"
 #include "range_reader.h"
 

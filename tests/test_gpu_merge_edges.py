@@ -391,3 +391,49 @@ def test_one_emit_tile_above_2GiB_is_refused_and_the_handle_recovers():
         rd.close()
     want = pyoracle.merge(BIN_SCHEMA, DeduplicateMergeFunction.factory().create(), small, pyoracle.SORT_LOSER_TREE)
     assert got.equals(want), got.first_difference(want)
+
+
+# ---- one handle rebound to a larger input that needs every optional workspace region, then to a smaller one
+
+GROUP_VT = RowType((DataField("k", "STRING", False), DataField("g", "BIGINT", True), DataField("v", "BIGINT", True),
+                    DataField("s", "STRING", True)))
+GROUP_SCHEMA = KeyValueSchema.of(GROUP_VT, ["k"])
+
+
+def group_runs(n_keys, n_runs, seed):
+    """String keys sharing a prefix (non-exact: the key-prefix skip), a sequence group whose field sums (group plan and
+    group aggregates) and a var-len column (look-back state)."""
+    rng = np.random.default_rng(seed)
+    rows_of_run = [[] for _ in range(n_runs)]
+    seq = 0
+    for key in range(n_keys):
+        k = f"user_{key:07d}"
+        for r in sorted(rng.choice(n_runs, size=int(rng.integers(1, n_runs + 1)), replace=False)):
+            seq += 1
+            g = None if rng.random() < 0.2 else int(rng.integers(0, 5))
+            v = None if rng.random() < 0.2 else int(rng.integers(-1000, 1000))
+            s = None if rng.random() < 0.2 else "x" * int(rng.integers(0, 24))
+            rows_of_run[r].append((k, seq, 0, k, g, v, s))
+    return [KeyValueBatch.from_rows(GROUP_SCHEMA, rows) for rows in rows_of_run if rows]
+
+
+def test_rebind_to_a_larger_input_with_every_workspace_region_and_back():
+    spec = PartialUpdateMergeFunction.factory({"fields.g.sequence-group": "v", "fields.v.aggregate-function": "sum"},
+                                              GROUP_VT, ["k"]).create()
+    inputs = [group_runs(500, 3, seed=1), group_runs(40_000, 4, seed=2), group_runs(300, 2, seed=3)]
+    rd = SortMergeReader([SortedRunReader(GROUP_SCHEMA, b) for b in inputs[0]], spec)
+    try:
+        for i, runs in enumerate(inputs):
+            if i:
+                previous = rd.readers
+                rd.rebind([SortedRunReader(GROUP_SCHEMA, b) for b in runs])
+                for r in previous:                             # the merge no longer holds them: free them now
+                    r.close()
+            rd.execute()
+            got = rd.fetch()
+            if i == 1:
+                assert rd.stats().n_levels >= 2
+            want = pyoracle.merge(GROUP_SCHEMA, spec, runs, pyoracle.SORT_LOSER_TREE)
+            assert got.equals(want), (i, got.first_difference(want))
+    finally:
+        rd.close()

@@ -4,6 +4,7 @@
 // (include/paimon_gpu.h).  There is no CPU fallback anywhere in this file: a spec the kernels do not
 // implement is refused with PG_ERR_UNSUPPORTED.
 #include <algorithm>
+#include <atomic>
 #include <cstdlib>
 #include <cstring>
 #include <map>
@@ -112,6 +113,7 @@ struct Merge {
     // pinned host mirror of totals + err
     int64_t *h_totals = nullptr;
     int32_t *h_err = nullptr;
+    H2dRing ring;                      // small_h2d's staging for `stream`, freed with the handle
     // output of the last execute
     std::vector<pg_out_column> out_cols;
     Arena work;                        // temporaries of one execute (bounds, sample keys, plan, ...)
@@ -149,8 +151,8 @@ pg_status ensure_device() {
 static pg_status copy_batch(std::vector<void *> &dsts, std::vector<void *> &srcs, std::vector<size_t> &sizes,
                             cudaMemcpyKind kind, cudaStream_t stream) {
     if (dsts.empty()) return PG_OK;
-    static bool batch_ok = true;
-    if (batch_ok && dsts.size() > 1) {
+    static std::atomic<bool> batch_ok{true};        // read and cleared by any thread
+    if (batch_ok.load(std::memory_order_relaxed) && dsts.size() > 1) {
         cudaMemcpyAttributes attr{};
         attr.srcAccessOrder = cudaMemcpySrcAccessOrderStream;
         size_t attr_idx = 0, fail_idx = 0;
@@ -158,7 +160,7 @@ static pg_status copy_batch(std::vector<void *> &dsts, std::vector<void *> &srcs
                                              &fail_idx, stream);
         if (e == cudaSuccess) return PG_OK;
         cudaGetLastError();
-        batch_ok = false;                               // not supported here: fall back for good
+        batch_ok.store(false, std::memory_order_relaxed);   // not supported here: fall back for good
     }
     for (size_t i = 0; i < dsts.size(); i++) PG_CUDA(cudaMemcpyAsync(dsts[i], srcs[i], sizes[i], kind, stream));
     return PG_OK;
@@ -654,7 +656,7 @@ static pg_status build_descriptors(Merge *m) {
         PG_CUDA(cudaMalloc(&m->d_desc, total));
         m->desc_cap = total;
     }
-    { pg_status ts = small_h2d(m->d_desc, host.data(), total, m->stream); if (ts) return ts; }
+    { pg_status ts = small_h2d(m->d_desc, host.data(), total, m->stream, m->ring); if (ts) return ts; }
     PG_CUDA(cudaStreamSynchronize(m->stream));
     m->desc.carve(m->d_desc, k, nk, nc, nv);
     if (sp->n_groups() == 0) m->desc.groups = nullptr;        // (the plan kernel's test for sequence groups)
@@ -890,7 +892,7 @@ static pg_status execute(Merge *m) {
     carve_out(m->outbuf.base);
     if (vspan) PG_CUDA(cudaMemsetAsync(m->outbuf.base, 0, vspan, sm));
     m->stats.bytes_out = bytes_out;
-    { pg_status ts = small_h2d(m->desc.out_cols, m->out_cols.data(), sizeof(pg_out_column) * nc, sm); if (ts) return ts; }
+    { pg_status ts = small_h2d(m->desc.out_cols, m->out_cols.data(), sizeof(pg_out_column) * nc, sm, m->ring); if (ts) return ts; }
 
     // ---- emit
     EmitArgs ea{};
@@ -1178,6 +1180,10 @@ pg_status pg_run_open(uint64_t schema, const pg_run_desc *desc, int32_t mem, uin
         Scratch scratch(cs);                          // the run's buffer until its copies are done
         unsigned char *d = (unsigned char *)scratch.take(total + 256);
         if (!d) return fail(PG_ERR_CUDA, "out of device memory for a run");
+        // the buffer comes from the recycled-buffer cache as some earlier user left it: zero it first, so that what the
+        // caller's bytes do not cover (validity bits past row n up to the word, the read-past slack of every region)
+        // reads as zero to kernels that load whole words, as it does in decoded runs
+        PG_CUDA(cudaMemsetAsync(d, 0, total, cs));
         std::vector<void *> cp_dst, cp_src;
         std::vector<size_t> cp_size;
         auto add_copy = [&](void *dst, const void *src, size_t bytes) {

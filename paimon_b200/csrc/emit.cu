@@ -21,6 +21,7 @@
 // (column, ColDesc, output buffers) are staged in shared memory once per tile instead of being read from the device
 // tables at the top of every pass (two dependent global round trips in front of all 16 warps).
 #include <stdio.h>
+#include <mutex>
 
 #include "device_utils.cuh"
 
@@ -853,14 +854,13 @@ void emit_timing_dump() {
 }
 #endif
 
-static bool g_emit_attr = false;
+static std::once_flag g_emit_attr_once;          // (set_attrs in merge.cu: the same, for k_emit)
 void launch_emit(const EmitArgs &ea) {
     EmitLayout L = emit_layout(ea.k);
-    if (!g_emit_attr) {
+    std::call_once(g_emit_attr_once, [] {
         cudaFuncSetAttribute(k_emit<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
         cudaFuncSetAttribute(k_emit<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        g_emit_attr = true;
-    }
+    });
     if (ea.gagg) k_emit<true><<<ea.n_tiles, kEmitThreads, L.total, ea.stream>>>(ea);
     else k_emit<false><<<ea.n_tiles, kEmitThreads, L.total, ea.stream>>>(ea);
 #ifdef PG_EMIT_TIMING

@@ -14,6 +14,8 @@
 //   4. emit kernel         per tile and column: select / fold the group's members, coalesced stores
 //
 // No tensor cores: the path is integer compare + gather (HBM bound).
+#include <mutex>
+
 #include "device_utils.cuh"
 
 namespace pg {
@@ -781,14 +783,15 @@ __global__ void k_scan(const int32_t *tile_rows, int n_tiles, int64_t *row_base,
 
 // ------------------------------------------------------------------ launchers
 
-static bool g_attr_done = false;
+// once per process, whichever thread launches first: the other threads wait until the attributes are set
+static std::once_flag g_attr_once;
 static void set_attrs() {
-    if (g_attr_done) return;
-    cudaFuncSetAttribute(k_merge_keys<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem);
-    cudaFuncSetAttribute(k_merge_keys<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem);
-    cudaFuncSetAttribute(k_plan<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPlanSmem);
-    cudaFuncSetAttribute(k_plan<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPlanSmem);
-    g_attr_done = true;
+    std::call_once(g_attr_once, [] {
+        cudaFuncSetAttribute(k_merge_keys<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem);
+        cudaFuncSetAttribute(k_merge_keys<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTileSmem);
+        cudaFuncSetAttribute(k_plan<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPlanSmem);
+        cudaFuncSetAttribute(k_plan<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kPlanSmem);
+    });
 }
 
 void launch_partition(const MergeLaunch &ml, const LevelView &lv, const uint64_t *splitter_keys,

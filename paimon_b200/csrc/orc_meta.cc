@@ -68,8 +68,8 @@ std::vector<uint8_t> inflate_section(const uint8_t *p, uint64_t n, int codec, ui
     const int64_t bound = orcdev::chunk_bound(p, (int64_t)n, codec, (int64_t)block_size);
     if (bound < 0) throw std::runtime_error("orc: truncated compression chunk");
     std::vector<uint8_t> out((size_t)bound), lit(zs::kMaxBlock + 64);
-    static thread_local zs::Tables *zt = nullptr;
-    if (!zt) zt = new zs::Tables();
+    static thread_local std::unique_ptr<zs::Tables> zt;          // (freed when the thread exits)
+    if (!zt) zt.reset(new zs::Tables());
     const int64_t got = orcdev::inflate_chunks(p, (int64_t)n, codec, (int64_t)block_size, out.data(), bound, *zt, lit.data());
     if (got < 0) throw std::runtime_error("orc: a metadata compression chunk does not inflate");
     out.resize((size_t)got);

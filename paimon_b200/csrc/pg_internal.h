@@ -508,13 +508,29 @@ struct EmitArgs {
 };
 void launch_emit(const EmitArgs &ea);
 
+// readback.cu, small_h2d: host -> device copies of tables and descriptors through a device-mapped page-locked ring of
+// 8 MiB that a kernel reads.  A ring serves one stream (it is reused once that stream has drained), and whoever owns the
+// stream owns the ring: a merge handle keeps one for its stream and frees it with the handle.  The overload without a
+// ring uses the calling thread's ring for `stream`, which must be one of that thread's own streams (its copy stream, the
+// decode's side stream); those are freed when the thread exits.  (Rings of merge streams kept per thread would pile up:
+// 8 MiB of pinned host memory for every merge handle a thread ever executed.)
+struct H2dRing {
+    uint8_t *h = nullptr, *d = nullptr;
+    size_t cap = 0, off = 0;
+    bool tried = false;                // allocation attempted (cap stays 0 without mapped memory: plain copies)
+    H2dRing() = default;
+    H2dRing(const H2dRing &) = delete;
+    H2dRing &operator=(const H2dRing &) = delete;
+    ~H2dRing();
+};
+pg_status small_h2d(void *dev_dst, const void *host_src, size_t n, cudaStream_t stream, H2dRing &ring);
+pg_status small_h2d(void *dev_dst, const void *host_src, size_t n, cudaStream_t stream);
+
 // readback.cu: small device -> host reads through device-mapped page-locked memory (a kernel stores them), so that
 // they do not queue behind another thread's large copies on the device -> host copy engine.  add() enqueues on the
 // stream, finish() synchronises the stream and delivers the bytes.  finish(ev) waits for an event the caller recorded on
 // the stream behind the last add() instead, so that work enqueued after it keeps the device busy meanwhile.  One object
 // per synchronisation point, per thread.
-pg_status small_h2d(void *dev_dst, const void *host_src, size_t n, cudaStream_t stream);   // tables / descriptors
-
 class SmallReads {
  public:
     explicit SmallReads(cudaStream_t s) : stream_(s) {}

@@ -8,6 +8,7 @@
 // device-mapped host memory instead; the host reads them after synchronising the stream.
 #include <algorithm>
 #include <cstring>
+#include <memory>
 #include <stdexcept>
 #include <utility>
 #include <vector>
@@ -43,42 +44,48 @@ __global__ void k_small_read(const uint8_t *src, uint8_t *dst, size_t n) {
 // copied into a device-mapped page-locked ring and a kernel moves them to their device buffer, so that they do not
 // queue behind an asynchronous upload of the next section's files on the host -> device copy engine.
 namespace {
-struct Ring {
-    uint8_t *h = nullptr, *d = nullptr;
-    size_t cap = 0, off = 0;
-    ~Ring() { if (h) cudaFreeHost(h); }
-};
 constexpr size_t kRingBytes = 8u << 20;
 }  // namespace
 
-pg_status small_h2d(void *dev_dst, const void *host_src, size_t n, cudaStream_t stream) {
+H2dRing::~H2dRing() { if (h) cudaFreeHost(h); }
+
+pg_status small_h2d(void *dev_dst, const void *host_src, size_t n, cudaStream_t stream, H2dRing &r) {
     if (n == 0) return PG_OK;
-    thread_local std::vector<std::pair<cudaStream_t, Ring *>> rings;       // one ring per (thread, stream)
-    Ring *r = nullptr;
-    for (auto &p : rings) if (p.first == stream) r = p.second;
-    if (!r) {
-        r = new Ring();
-        if (cudaHostAlloc((void **)&r->h, kRingBytes, cudaHostAllocMapped) == cudaSuccess &&
-            cudaHostGetDevicePointer((void **)&r->d, r->h, 0) == cudaSuccess)
-            r->cap = kRingBytes;
+    if (!r.tried) {
+        r.tried = true;
+        if (cudaHostAlloc((void **)&r.h, kRingBytes, cudaHostAllocMapped) == cudaSuccess &&
+            cudaHostGetDevicePointer((void **)&r.d, r.h, 0) == cudaSuccess)
+            r.cap = kRingBytes;
         else
             cudaGetLastError();
-        rings.push_back({stream, r});
     }
-    if (n > r->cap) {
+    if (n > r.cap) {
         PG_CUDA(cudaMemcpyAsync(dev_dst, host_src, n, cudaMemcpyHostToDevice, stream));
         return PG_OK;
     }
-    size_t off = (r->off + 15) & ~(size_t)15;
-    if (off + n > r->cap) {
+    size_t off = (r.off + 15) & ~(size_t)15;
+    if (off + n > r.cap) {
         PG_CUDA(cudaStreamSynchronize(stream));        // every kernel that read the ring so far is done
         off = 0;
     }
-    memcpy(r->h + off, host_src, n);
+    memcpy(r.h + off, host_src, n);
     const int blocks = (int)std::min<size_t>(128, (n + 4095) / 4096);
-    k_small_read<<<blocks, 256, 0, stream>>>(r->d + off, (uint8_t *)dev_dst, n);
-    r->off = off + n;
+    k_small_read<<<blocks, 256, 0, stream>>>(r.d + off, (uint8_t *)dev_dst, n);
+    r.off = off + n;
     return PG_OK;
+}
+
+pg_status small_h2d(void *dev_dst, const void *host_src, size_t n, cudaStream_t stream) {
+    // the thread's own streams only (two at most): the rings are freed when the thread exits, when every call it made
+    // has synchronised its streams
+    thread_local std::vector<std::pair<cudaStream_t, std::unique_ptr<H2dRing>>> rings;
+    H2dRing *r = nullptr;
+    for (auto &p : rings) if (p.first == stream) r = p.second.get();
+    if (!r) {
+        rings.emplace_back(stream, std::make_unique<H2dRing>());
+        r = rings.back().second.get();
+    }
+    return small_h2d(dev_dst, host_src, n, stream, *r);
 }
 
 pg_status SmallReads::add(void *host_dst, const void *dev_src, size_t n) {

@@ -9,7 +9,7 @@ SRCS := paimon_b200/csrc/merge.cu paimon_b200/csrc/emit.cu paimon_b200/csrc/api.
 HDRS := include/paimon_gpu.h paimon_b200/csrc/pg_internal.h paimon_b200/csrc/device_utils.cuh paimon_b200/csrc/parquet_meta.h \
 	paimon_b200/csrc/zstd_device.cuh paimon_b200/csrc/zstd_encode_device.cuh paimon_b200/csrc/inflate_device.cuh paimon_b200/csrc/lz4_device.cuh paimon_b200/csrc/snappy_device.cuh paimon_b200/csrc/orc_device.cuh paimon_b200/csrc/orc_meta.h \
 	paimon_b200/csrc/orc_encode_device.cuh paimon_b200/csrc/encoded_file.h paimon_b200/csrc/xxhash64_device.cuh paimon_b200/csrc/murmur3_device.cuh \
-	paimon_b200/csrc/scan_kernels.cuh paimon_b200/csrc/range_reader.h paimon_b200/csrc/device_layout.h
+	paimon_b200/csrc/scan_kernels.cuh paimon_b200/csrc/range_reader.h paimon_b200/csrc/device_layout.h paimon_b200/csrc/sbbf_device.cuh
 LIB := paimon_b200/libpaimon_gpu.so
 
 all: $(LIB) oracle

@@ -428,6 +428,34 @@ pg_status pg_parquet_encode(uint64_t source, const char *const *column_names, in
 pg_status pg_parquet_encode_compressed(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
                                        const pg_parquet_write_options *options, int32_t codec, int32_t level,
                                        uint64_t *out_file);
+
+/* ---- the same encode with Parquet bloom filters -------------------------------------------------------------
+ * What parquet-mr 1.16 writes for 'parquet.bloom.filter.enabled' and its per-column forms
+ * 'parquet.bloom.filter.enabled#<col>', 'parquet.bloom.filter.expected.ndv#<col>' and 'parquet.bloom.filter.fpp#<col>'
+ * (paimon-format/.../parquet/writer/RowDataParquetBuilder.java:96-116): per (row group, bloom column) one split-block
+ * bloom filter (Parquet BloomFilter.md: XXH64 of each non-NULL value's PLAIN bytes, 32-byte blocks, eight salted bits
+ * per value), which Paimon's Parquet reader uses to drop row groups (ParquetFileReader.java:418-419, 1051-1120).  The
+ * filter has 1 MiB (parquet-mr's default maximum; Paimon does not set parquet.bloom.filter.max.bytes) without an ndv,
+ * else parquet-mr's optimalNumOfBits(ndv, fpp) / 8 bytes, at least 32, rounded up to a power of two, at most 1 MiB.
+ * The bits are set on the device inside the file image.  Every filter follows the page index (when written), row group
+ * major then column: a BloomFilterHeader (numBytes, BLOCK, XXHASH, UNCOMPRESSED) placed so that the bitset behind it
+ * starts on a 32-byte boundary of the file; ColumnMetaData fields 14 / 15 (bloom_filter_offset / _length, header and
+ * bitset) point at it.  Filters are never compressed; `codec` and `level` apply to the pages as for
+ * pg_parquet_encode_compressed, and are refused the same way.
+ * A NULL `bloom` or n_columns = 0 writes the bytes of pg_parquet_encode_compressed.  Before any device work:
+ * PG_ERR_INVALID for n_columns < 0, a column outside the schema or listed twice, ndv < 0, fpp outside (0, 1);
+ * PG_ERR_UNSUPPORTED for a BOOLEAN column (the specification defines no BOOLEAN hash). */
+typedef struct {
+    int32_t column;   /* file column index */
+    int64_t ndv;      /* 'parquet.bloom.filter.expected.ndv#<col>'; 0 = unset: the filter takes the 1 MiB maximum */
+    double  fpp;      /* 'parquet.bloom.filter.fpp#<col>' (parquet-mr default 0.01), in (0, 1); used with an ndv */
+} pg_parquet_bloom_column;
+typedef struct { int32_t n_columns; const pg_parquet_bloom_column *columns; } pg_parquet_bloom_options;
+
+pg_status pg_parquet_encode_bloom(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
+                                  const pg_parquet_write_options *options, int32_t codec, int32_t level,
+                                  const pg_parquet_bloom_options *bloom, uint64_t *out_file);
+
 pg_status pg_parquet_file_meta(uint64_t file, pg_file_meta *out);
 /* whole-file statistics of one column: null count; min / max for fixed-width columns (integers and BOOLEAN as
  * int64, FLOAT / DOUBLE as double; absent when every value is NULL or a NaN was seen) */

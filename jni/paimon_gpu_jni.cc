@@ -290,6 +290,37 @@ JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetEncodeComp
     PG_CHECK(pg_parquet_encode_compressed((uint64_t)source, ptrs.data(), row0, nRows, &opt, codec, level, &h));
     return (jlong)h;
 }
+// parquetEncodeCompressed with Parquet bloom filters: per i, file column bloomColumns[i] with ndv[i]
+// (parquet.bloom.filter.expected.ndv#col, 0 = unset) and fpp[i] (parquet.bloom.filter.fpp#col); null = none:
+// pg_parquet_encode_bloom.
+JNIEXPORT jlong JNICALL Java_org_apache_paimon_gpu_NativeMerge_parquetEncodeBloom(
+        JNIEnv *env, jclass, jlong source, jobjectArray names, jlong row0, jlong nRows, jlong rowGroupRows,
+        jlong pageRows, jboolean pageIndex, jint codec, jint level, jintArray bloomColumns, jlongArray ndv,
+        jdoubleArray fpp) {
+    std::vector<std::string> keep;
+    std::vector<const char *> ptrs = utf_names(env, names, keep);
+    pg_parquet_write_options opt{rowGroupRows, pageRows, pageIndex ? 1 : 0};
+    const jsize n = bloomColumns ? env->GetArrayLength(bloomColumns) : 0;
+    if ((n && (!ndv || !fpp)) || (ndv && env->GetArrayLength(ndv) != n) || (fpp && env->GetArrayLength(fpp) != n)) {
+        env->ThrowNew(env->FindClass("java/lang/IllegalArgumentException"),
+                      "parquetEncodeBloom: bloomColumns, ndv and fpp differ in length");
+        return 0;
+    }
+    std::vector<jint> c(n);
+    std::vector<jlong> d(n);
+    std::vector<jdouble> f(n);
+    if (n) {
+        env->GetIntArrayRegion(bloomColumns, 0, n, c.data());
+        env->GetLongArrayRegion(ndv, 0, n, d.data());
+        env->GetDoubleArrayRegion(fpp, 0, n, f.data());
+    }
+    std::vector<pg_parquet_bloom_column> cols;
+    for (jsize i = 0; i < n; i++) cols.push_back(pg_parquet_bloom_column{c[i], d[i], f[i]});
+    pg_parquet_bloom_options bloom{(int32_t)n, cols.data()};
+    uint64_t h = 0;
+    PG_CHECK(pg_parquet_encode_bloom((uint64_t)source, ptrs.data(), row0, nRows, &opt, codec, level, &bloom, &h));
+    return (jlong)h;
+}
 // types = 4 ints per column (kind, precision, scale, max length; pg_orc_column_type), or null for the kinds of the
 // physical types
 static std::vector<pg_orc_column_type> orc_types(JNIEnv *env, jintArray types) {

@@ -101,6 +101,14 @@ class PgOrcIndexOptions(C.Structure):
                 ("bloom_columns", C.POINTER(C.c_int32)), ("bloom_fpp", C.c_double)]
 
 
+class PgParquetBloomColumn(C.Structure):
+    _fields_ = [("column", C.c_int32), ("ndv", C.c_int64), ("fpp", C.c_double)]
+
+
+class PgParquetBloomOptions(C.Structure):
+    _fields_ = [("n_columns", C.c_int32), ("columns", C.POINTER(PgParquetBloomColumn))]
+
+
 class PgBloomFilterSpec(C.Structure):
     _fields_ = [("column", C.c_int32), ("items", C.c_int32), ("fpp", C.c_double)]
 
@@ -171,6 +179,9 @@ _SIGNATURES = {
     "pg_parquet_encode_compressed": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,
                                                  C.POINTER(PgParquetWriteOptions), C.c_int32, C.c_int32,
                                                  C.POINTER(C.c_uint64)]),
+    "pg_parquet_encode_bloom": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,
+                                            C.POINTER(PgParquetWriteOptions), C.c_int32, C.c_int32,
+                                            C.POINTER(PgParquetBloomOptions), C.POINTER(C.c_uint64)]),
     "pg_orc_encode": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,
                                   C.POINTER(PgOrcWriteOptions), C.POINTER(C.c_uint64)]),
     "pg_orc_encode_indexed": (C.c_int32, [C.c_uint64, C.POINTER(C.c_char_p), C.c_int64, C.c_int64,

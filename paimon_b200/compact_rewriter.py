@@ -169,6 +169,43 @@ def file_column_names(schema: KeyValueSchema) -> List[str]:
     return [f.name for f in schema.file_fields()]
 
 
+# parquet-mr's bloom filter fpp when 'parquet.bloom.filter.fpp#<col>' is not set (ParquetProperties)
+PARQUET_BLOOM_DEFAULT_FPP = 0.01
+
+
+def parquet_bloom_for_level(schema: KeyValueSchema, options: Optional[Dict[str, object]]) -> List[Tuple[int, int, float]]:
+    """The Parquet bloom filters of a data file as (file column, ndv, fpp), from the table options parquet-mr receives
+    (RowDataParquetBuilder.java:96-116; options starting with 'parquet.' keep the prefix, FileFormat
+    .getIdentifierPrefixOptions).  'parquet.bloom.filter.enabled' (default false) covers every file column, _KEY_<pk>,
+    _SEQUENCE_NUMBER and _VALUE_KIND included, and 'parquet.bloom.filter.enabled#<col>' overrides it for one column
+    either way; 'parquet.bloom.filter.expected.ndv#<col>' (0 = unset: a 1 MiB filter) and
+    'parquet.bloom.filter.fpp#<col>' (default 0.01) size its filter.  A '#<col>' naming no file column is ignored, as
+    ColumnConfigParser ignores it.  BOOLEAN columns get no filter: the Parquet specification defines no BOOLEAN hash.
+    A malformed ndv or fpp, or one outside ndv > 0 / 0 < fpp < 1, is refused here, before any device work."""
+    options = options or {}
+    ndv, fpp = {}, {}
+    for key, value in options.items():
+        for prefix, out, parse in (("parquet.bloom.filter.expected.ndv#", ndv, int),
+                                   ("parquet.bloom.filter.fpp#", fpp, float)):
+            if not str(key).startswith(prefix):
+                continue
+            try:
+                v = parse(str(value).strip())
+            except ValueError:
+                raise N.PaimonGpuError(1, f"parquet encode: option {key} = {value!r} is not a number") from None
+            if not (v > 0 if parse is int else 0 < v < 1):
+                raise N.PaimonGpuError(1, f"parquet encode: option {key} = {value!r} is outside "
+                                          f"{'ndv > 0' if parse is int else '(0, 1)'}")
+            out[str(key)[len(prefix):]] = v
+    enabled = str(options.get("parquet.bloom.filter.enabled", "false")).strip().lower() == "true"
+    out = []
+    for c, (name, t) in enumerate(zip(file_column_names(schema), schema.physical_types())):
+        on = options.get(f"parquet.bloom.filter.enabled#{name}")
+        if (enabled if on is None else str(on).strip().lower() == "true") and t != PhysicalType.BOOL:
+            out.append((c, ndv.get(name, 0), fpp.get(name, PARQUET_BLOOM_DEFAULT_FPP)))
+    return out
+
+
 class KeyValueDataFileWriter:
     """Encodes rows [row0, row0 + n_rows) of a device batch (a merge handle holding a batch, or a run handle) as
     one data file of `file_format` ('parquet' or 'orc') and returns its DataFileMeta.  `compression` names the codec
@@ -183,13 +220,16 @@ class KeyValueDataFileWriter:
     `row_index_stride` (rows per row group of its row index, 0 = none), `bloom_filter_columns` (value-field names
     with a bloom filter per row group, built on the device) and `bloom_filter_fpp`, as orc-core writes them for
     'orc.row.index.stride', 'orc.bloom.filter.columns' and 'orc.bloom.filter.fpp'; Parquet files ignore them.  Index
-    options the device cannot write are refused here, before any device work."""
+    options the device cannot write are refused here, before any device work.  A Parquet file takes `parquet_bloom`,
+    (file column, ndv, fpp) per column with a Parquet bloom filter per row group (parquet_bloom_for_level), built on the
+    device; ORC files ignore it."""
 
     def __init__(self, schema: KeyValueSchema, path: str, level: int, file_io: Optional[LocalFileIO] = None,
                  row_group_rows: int = 0, page_rows: int = 0, compression: str = "none", zstd_level: int = 1,
                  file_format: str = "parquet", stripe_rows: int = 0, compression_block_size: int = 0,
                  file_index: Optional[FileIndexOptions] = None, page_index: bool = False,
-                 row_index_stride: int = 0, bloom_filter_columns: Sequence[str] = (), bloom_filter_fpp: float = 0.01):
+                 row_index_stride: int = 0, bloom_filter_columns: Sequence[str] = (), bloom_filter_fpp: float = 0.01,
+                 parquet_bloom: Sequence[Tuple[int, int, float]] = ()):
         self.schema = schema
         self.path = path
         self.level = level
@@ -210,6 +250,10 @@ class KeyValueDataFileWriter:
             self.orc_opts = N.PgOrcWriteOptions(stripe_rows, self.codec, self.zstd_level, compression_block_size,
                                                 self._orc_types)
             self.orc_index = orc_index_options(schema, row_index_stride, bloom_filter_columns, bloom_filter_fpp)
+        bloom = list(parquet_bloom)
+        self._bloom_cols = (N.PgParquetBloomColumn * max(len(bloom), 1))(
+            *[N.PgParquetBloomColumn(int(c), int(ndv), float(fpp)) for c, ndv, fpp in bloom])
+        self.parquet_bloom = N.PgParquetBloomOptions(len(bloom), self._bloom_cols)
         self.index_writer = None
         if file_index is not None and not file_index.is_empty():
             self.index_writer = DataFileIndexWriter(schema, file_index)
@@ -222,11 +266,9 @@ class KeyValueDataFileWriter:
         if self.file_format == "orc":
             N.check(self.lib.pg_orc_encode_indexed(source_handle, arr, row0, n_rows, C.byref(self.orc_opts),
                                                    C.byref(self.orc_index), C.byref(fh)))
-        elif self.codec == 0:
-            N.check(self.lib.pg_parquet_encode(source_handle, arr, row0, n_rows, C.byref(self.opts), C.byref(fh)))
         else:
-            N.check(self.lib.pg_parquet_encode_compressed(source_handle, arr, row0, n_rows, C.byref(self.opts),
-                                                          self.codec, self.zstd_level, C.byref(fh)))
+            N.check(self.lib.pg_parquet_encode_bloom(source_handle, arr, row0, n_rows, C.byref(self.opts), self.codec,
+                                                     self.zstd_level, C.byref(self.parquet_bloom), C.byref(fh)))
         try:
             meta = N.PgFileMeta()
             N.check(self.lib.pg_parquet_file_meta(fh.value, C.byref(meta)))
@@ -317,7 +359,8 @@ class MergeTreeCompactRewriter:
     cannot build them); without, they are uncompressed Parquet (or the writer arguments' file_format).  With
     `page_index` the files of Parquet output levels carry the page index (ColumnIndex and OffsetIndex); ORC output
     levels ignore it.  With `row_index` the files of ORC output levels carry a row index and bloom filters as the
-    table options ask for them (orc_index_for_level); Parquet output levels ignore it."""
+    table options ask for them (orc_index_for_level); Parquet output levels ignore it.  The files of Parquet output
+    levels carry the Parquet bloom filters the table options ask for (parquet_bloom_for_level)."""
 
     def __init__(self, schema: KeyValueSchema, mf_factory: MergeFunctionFactory, directory: str,
                  user_defined_seq_comparator=None, file_io: Optional[LocalFileIO] = None, device: int = 0,
@@ -355,6 +398,7 @@ class MergeTreeCompactRewriter:
                  writer_args["compression_block_size"]) = orc_compression_for_level(self.options, output_level)
             else:
                 writer_args["compression"], writer_args["zstd_level"] = compression_for_level(self.options, output_level)
+                writer_args["parquet_bloom"] = parquet_bloom_for_level(self.schema, self.options)
             file_index = FileIndexOptions.from_options(self.options)
             if not file_index.is_empty():
                 DataFileIndexWriter(self.schema, file_index)          # refuses before any device work

@@ -14,8 +14,10 @@
 //
 // Layout written: PAR1 | per row group, per column: data pages V1, PLAIN, uncompressed or one zstd frame per page
 // body (pg_parquet_encode_compressed) | with page_index: every ColumnIndex, then every OffsetIndex (parquet-mr's
-// order) | FileMetaData | len | PAR1.  Page bounds come from k_pw_stats, run per page (the chunk statistics are
-// folded from the page words on the host), and for STRING / BINARY from k_pw_minmax_bytes.
+// order) | with bloom columns (pg_parquet_encode_bloom): every bloom filter, row group major, each a BloomFilterHeader
+// and its bitset (32-byte aligned) | FileMetaData | len | PAR1.  Page bounds come from k_pw_stats, run per page (the
+// chunk statistics are folded from the page words on the host), and for STRING / BINARY from k_pw_minmax_bytes.  The
+// bloom filters' bits (sbbf_device.cuh) are set by k_pw_sbbf straight into the file image.
 // Pages start at multiples of 8 rows, so a nullable column's definition levels (bit width 1, bit-packed LSB first)
 // ARE the bytes of the Arrow validity bitmap: they are copied, not re-encoded.  Values of non-null rows are
 // compacted by a block-wide scan; BYTE_ARRAY values are written as [len:int32][bytes].
@@ -25,6 +27,7 @@
 #include "device_utils.cuh"
 #include "encoded_file.h"
 #include "parquet_meta.h"
+#include "sbbf_device.cuh"
 
 namespace pg {
 
@@ -140,6 +143,88 @@ k_pw_encode(const EncColumn *cols, const EncJob *jobs, uint8_t *file) {
     }
 }
 
+// ------------------------------------------------------------------ bloom filters (SBBF)
+
+struct SbbfJob {                  // the filter of one column chunk
+    int32_t col;
+    uint32_t n_blocks;            // bitset bytes / 32
+    int64_t row0, n_rows;         // the chunk's rows
+    int64_t bits_off;             // file offset of the bitset, a multiple of 32
+};
+
+// One thread per row of a chunk, blockIdx.y (strided) = the job: skip NULLs, hash the value's PLAIN bytes, set its
+// eight bits in the bitset inside the file image (zeroed at allocation) with word atomics.
+__global__ void __launch_bounds__(256) k_pw_sbbf(const EncColumn *cols, const SbbfJob *jobs, int n_jobs, uint8_t *file) {
+    for (int jb = blockIdx.y; jb < n_jobs; jb += gridDim.y) {
+        const SbbfJob j = jobs[jb];
+        const EncColumn c = cols[j.col];
+        uint32_t *bits = (uint32_t *)(file + j.bits_off);
+        for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < j.n_rows;
+             i += (int64_t)gridDim.x * blockDim.x) {
+            const int64_t row = j.row0 + i;
+            if (!valid_bit(c.validity, row)) continue;
+            uint64_t h;
+            if (c.width == 0) {
+                const int32_t a = c.offsets[row], b = c.offsets[row + 1];
+                h = fi::xxh64((const uint8_t *)c.data + a, b - a);
+            } else if (c.width == 8) {
+                h = sbbf::hash8(((const uint64_t *)c.data)[row]);
+            } else {                                           // INT8 / INT16 sign-extended to INT32, FLOAT's bits
+                const uint64_t v = load_fixed(c.data, c.width, row);
+                h = sbbf::hash4(c.type == PG_FLOAT ? (uint32_t)v : (uint32_t)(int32_t)sext(v, c.width));
+            }
+            // the block as four 64-bit words (little-endian word pairs); an atomic only where a bit is still clear,
+            // so that the rows of a low-cardinality column do not all queue on the same few addresses (a bit once
+            // set stays set, so a stale read costs an atomic, never a bit)
+            unsigned long long *blk = (unsigned long long *)(bits + 8 * (size_t)sbbf::block_of(h, j.n_blocks));
+#pragma unroll
+            for (int w = 0; w < 4; w++) {
+                const unsigned long long m =
+                    sbbf::mask_word(h, 2 * w) | (unsigned long long)sbbf::mask_word(h, 2 * w + 1) << 32;
+                if ((__ldcg(blk + w) & m) != m) atomicOr(blk + w, m);
+            }
+        }
+    }
+}
+
+// The bitset bytes of each file column's filter (0 = none) from `bloom`, or the refusal of a bad list
+static pg_status bloom_sizes(const Schema &s, const pg_parquet_bloom_options *bloom, std::vector<int64_t> *bytes) {
+    const int nc = s.n_cols();
+    bytes->assign(nc, 0);
+    if (!bloom || bloom->n_columns == 0) return PG_OK;
+    if (bloom->n_columns < 0 || !bloom->columns)
+        return fail(PG_ERR_INVALID, "parquet encode: bloom n_columns " + std::to_string(bloom->n_columns) +
+                                        " is negative or its columns are NULL");
+    for (int i = 0; i < bloom->n_columns; i++) {
+        const pg_parquet_bloom_column &b = bloom->columns[i];
+        const std::string col = "parquet encode: bloom column " + std::to_string(b.column);
+        if (b.column < 0 || b.column >= nc) return fail(PG_ERR_INVALID, col + " is outside the schema");
+        if ((*bytes)[b.column]) return fail(PG_ERR_INVALID, col + " is listed twice");
+        if (b.ndv < 0) return fail(PG_ERR_INVALID, col + ": ndv " + std::to_string(b.ndv) + " is negative");
+        if (!(b.fpp > 0 && b.fpp < 1))
+            return fail(PG_ERR_INVALID, col + ": fpp " + std::to_string(b.fpp) + " is outside (0, 1)");
+        if (s.field(b.column).type == PG_BOOL)
+            return fail(PG_ERR_UNSUPPORTED, col + " is BOOLEAN, which Parquet bloom filters do not cover");
+        (*bytes)[b.column] = sbbf::num_bytes(b.ndv, b.fpp);
+    }
+    return PG_OK;
+}
+
+// BloomFilterHeader: numBytes, algorithm BLOCK, hash XXHASH, compression UNCOMPRESSED (each union's first member, an
+// empty struct)
+static std::vector<uint8_t> bloom_header(int64_t bytes) {
+    pq::ThriftWriter w;
+    w.i32(1, (int32_t)bytes);
+    for (int f = 2; f <= 4; f++) {
+        w.struct_field(f);
+        w.struct_field(1);
+        w.end();
+        w.end();
+    }
+    w.end();
+    return std::move(w.b);
+}
+
 // ------------------------------------------------------------------ page index: bounds of var-len pages
 
 constexpr int kTruncate = 64;     // parquet-mr's default column-index truncation length
@@ -250,6 +335,8 @@ struct Chunk {
     int64_t first_page = 0, total_uncompressed = 0, total_compressed = 0;
     int64_t column_index_off = -1, offset_index_off = -1;   // -1: not written
     int32_t column_index_len = 0, offset_index_len = 0;
+    int64_t bloom_off = -1;       // its BloomFilterHeader, -1: no filter
+    int32_t bloom_len = 0;        // header and bitset
 };
 struct Plan {
     int64_t n_groups = 0;
@@ -632,6 +719,10 @@ static std::vector<uint8_t> footer(const Plan &pl, const char *const *names, int
             w.i64(3, ch.st.null_count);
             if (ch.st.has_minmax) write_min_max(w, pl.cols[c], ch.st);
             w.end();
+            if (ch.bloom_off >= 0) {
+                w.i64(14, ch.bloom_off);
+                w.i32(15, ch.bloom_len);
+            }
             w.end();                                           // ColumnMetaData
             if (ch.offset_index_off >= 0) {
                 w.i64(4, ch.offset_index_off);
@@ -664,7 +755,8 @@ static std::vector<uint8_t> footer(const Plan &pl, const char *const *names, int
 }
 
 static pg_status encode(uint64_t source, const char *const *names, int64_t row0, int64_t n_rows,
-                        const pg_parquet_write_options *opt, int codec, uint64_t *out_file) {
+                        const pg_parquet_write_options *opt, int codec, const pg_parquet_bloom_options *bloom,
+                        uint64_t *out_file) {
     if (opt && opt->page_index != 0 && opt->page_index != 1)
         return fail(PG_ERR_INVALID, "parquet encode: page_index " + std::to_string(opt->page_index) + " is not 0 or 1");
     const bool page_index = opt && opt->page_index == 1;
@@ -673,6 +765,8 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
     if (st) return st;
     const Schema *s = batch.schema.get();
     const int nc = s->n_cols();
+    std::vector<int64_t> bloom_bytes;                        // per column: its filters' bitset bytes, 0 = none
+    if ((st = bloom_sizes(*s, bloom, &bloom_bytes))) return st;
 
     SectionTimer tm;
     if ((st = start_encode(tm))) return st;
@@ -785,6 +879,23 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
             ef->host_parts.push_back({ch.offset_index_off, std::move(oi)});
         }
     }
+    // every bloom filter (row group major, then column), each header placed so that its bitset starts on a 32-byte
+    // boundary; the bitsets are written on the device, so the device's part of the image reaches to the last one
+    std::vector<SbbfJob> bjobs;
+    int64_t bloom_rows = 0;
+    for (Chunk &ch : pl.chunks) {
+        const int64_t nb = bloom_bytes[ch.col];
+        if (!nb) continue;
+        std::vector<uint8_t> hdr = bloom_header(nb);
+        const int64_t hb = (int64_t)hdr.size(), bits_off = (pos + hb + 31) & ~(int64_t)31;
+        ch.bloom_off = bits_off - hb;
+        ch.bloom_len = (int32_t)(hb + nb);
+        ef->host_parts.push_back({ch.bloom_off, std::move(hdr)});
+        bjobs.push_back(SbbfJob{ch.col, (uint32_t)(nb / 32), ch.row0, ch.n_rows, bits_off});
+        bloom_rows = std::max(bloom_rows, ch.n_rows);
+        pos = bits_off + nb;
+        ef->data_end = pos;
+    }
     ef->host_parts.push_back({pos, footer(pl, names, n_rows, zstd)});
     ef->file_bytes = pos + (int64_t)ef->host_parts.back().second.size();
 
@@ -796,6 +907,15 @@ static pg_status encode(uint64_t source, const char *const *names, int64_t row0,
         for (Part &prefix : place_bodies(pl, body_off)) ef->host_parts.push_back(std::move(prefix));
         PG_CUDA(cudaMemcpy(d_jobs, pl.jobs.data(), sizeof(EncJob) * nj, cudaMemcpyHostToDevice));
         k_pw_encode<<<(unsigned)nj, 256>>>(d_cols, d_jobs, ef->d_file);
+        launches++;
+    }
+    if (!bjobs.empty()) {
+        SbbfJob *d_bjobs = (SbbfJob *)scratch.take(sizeof(SbbfJob) * bjobs.size());
+        if (!d_bjobs) return fail(PG_ERR_CUDA, "parquet encode: out of device memory for the bloom filter jobs");
+        PG_CUDA(cudaMemcpy(d_bjobs, bjobs.data(), sizeof(SbbfJob) * bjobs.size(), cudaMemcpyHostToDevice));
+        const int64_t bx = std::min<int64_t>(std::max<int64_t>((bloom_rows + 255) / 256, 1), 4096);
+        const unsigned by = (unsigned)std::min<size_t>(bjobs.size(), 65535);
+        k_pw_sbbf<<<dim3((unsigned)bx, by), 256>>>(d_cols, d_bjobs, (int)bjobs.size(), ef->d_file);
         launches++;
     }
     ef->meta.n_rows = n_rows;
@@ -813,12 +933,18 @@ extern "C" {
 pg_status pg_parquet_encode(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
                             const pg_parquet_write_options *options, uint64_t *out_file) {
     if (!out_file) return fail(PG_ERR_INVALID, "null argument");
-    return encode(source, column_names, row0, n_rows, options, pq::C_UNCOMPRESSED, out_file);
+    return encode(source, column_names, row0, n_rows, options, pq::C_UNCOMPRESSED, nullptr, out_file);
 }
 
 pg_status pg_parquet_encode_compressed(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
                                        const pg_parquet_write_options *options, int32_t codec, int32_t level,
                                        uint64_t *out_file) {
+    return pg_parquet_encode_bloom(source, column_names, row0, n_rows, options, codec, level, nullptr, out_file);
+}
+
+pg_status pg_parquet_encode_bloom(uint64_t source, const char *const *column_names, int64_t row0, int64_t n_rows,
+                                  const pg_parquet_write_options *options, int32_t codec, int32_t level,
+                                  const pg_parquet_bloom_options *bloom, uint64_t *out_file) {
     if (!out_file) return fail(PG_ERR_INVALID, "null argument");
     if (codec < pq::C_UNCOMPRESSED || codec > pq::C_LZ4_RAW)
         return fail(PG_ERR_INVALID, "parquet encode: codec " + std::to_string(codec) + " is not a Parquet CompressionCodec");
@@ -828,7 +954,7 @@ pg_status pg_parquet_encode_compressed(uint64_t source, const char *const *colum
     if (codec == pq::C_ZSTD && (level == 0 || level > 1))
         return fail(PG_ERR_UNSUPPORTED, "parquet encode: file.compression.zstd-level " + std::to_string(level) +
                                             " is not written on the device (level 1 and the negative fast levels are)");
-    return encode(source, column_names, row0, n_rows, options, codec, out_file);
+    return encode(source, column_names, row0, n_rows, options, codec, bloom, out_file);
 }
 
 }  // extern "C"
